@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — FSK demod + center + digitize of a synthetic 1 GiSample complex64 capture per B200 (BASELINE.json configs[1]).
+"""bench.py — FSK demod + center + digitize of a synthetic 1 GiSample complex64 capture per GPU (BASELINE.json configs[1]).
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun, one rank per GPU)
     python bench.py --impl reference --gpus N --steps K --warmup W   (CPU arm: the reference's own kernels)
+    python bench.py ... --dump-outputs DIR                   (also write the last timed step's results as DIR/<name>.npy)
 
 One "step" (default --center detect) = ONE library call per GPU, urh_demod_center_digitize (N>1:
 urh_shard_demod_center_digitize): afp_demod FSK with per-tile statistics -> capture-wide detect_center (rank window, bin
@@ -11,7 +12,7 @@ edges, histogram, peak pick: all on the device) -> grab_pulse_lens over qad -> p
 `other_variant` otherwise.
 `value` = whole-job MSamples/s with the IQ already in HBM; `e2e` = the same step fed from pinned HOST memory through the
 public Python API (H2D of the IQ and D2H of the pulse table inside the timed region).  The capture (8 GiB / GPU) is far
-larger than the 126 MB L2, so no explicit L2 flush is needed.
+larger than the H100's 50 MB L2, so no explicit L2 flush is needed.
 After the timed loops every run checks itself against the CPU oracle (outside the timed region): `parity` in the JSON line.
 """
 import argparse
@@ -39,13 +40,17 @@ NOISE_MAG = 0.05
 SIGMA = 0.01
 TOL = 5
 CENTER = 0.0
-# dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel: read at run time from the committed summary of this
-# round's `ncu --set full` capture (tools/ncu_summary.py writes profiles/traffic.json: bytes per sample per kernel, captured at
-# 2^28 samples; the kernels stream, so DRAM bytes scale with n).  null when the file is missing.
+# dram__bytes_read.sum + dram__bytes_write.sum of the dominant kernel, read at run time from profiles/traffic.json when an
+# `ncu --set full` capture has been summarised there (tools/ncu_summary.py --traffic-json: bytes per sample per kernel; the
+# kernels stream, so DRAM bytes scale with n).  No such file is committed: `traffic` is null then.
 TRAFFIC_FILE = os.path.join(ROOT, "profiles", "traffic.json")
 ALG_BYTES_PER_SAMPLE = 12  # dominant kernel, SURVEY §8d: read IQ 8 B + write qad 4 B (pulse table ~0.1 B/sample ignored)
 STEP_BYTES_PER_SAMPLE = {"detect": 16, "given": 12}  # SURVEY §8d per-path budgets (detect: qad re-read once)
 PARITY_LOG2 = 24  # parity windows of 2^24 samples (first / middle / last of every shard)
+# --dump-outputs: seeded samples of qad (float32 values + float64 positions: 24 MB) and of the pulse table (float64 rows +
+# indices: 24 MB), split over the ranks, so that the files stay under 64 MB in all
+DUMP_QAD_SAMPLES = 1 << 21
+DUMP_ROWS = 1 << 20
 
 
 def env_int(name, default):
@@ -58,9 +63,9 @@ def env_int(name, default):
 def capture_gaps(n, rank):
     """Every 2^log2n-sample block of the capture has the same structure: bursts of 5 M samples every 6 M, one long gap at 40-43 % of
     the block and silence from 97 % on.  One block per GPU: the per-GPU work is the same at every N (weak scaling).  With the long
-    gap and the tail defined on the WHOLE capture instead, two of eight shards hold them all and the other six do 8 % more work in
-    the histogram and digitizer passes than the single-GPU run (silent tiles are skipped): measured with tools/timeline_dist.py,
-    profiles/r02_timeline_n4_globalgaps_*.json - 318 of the 390 us a step lost from 1 to 8 GPUs were that imbalance, 87 us the exchanges."""
+    gap and the tail defined on the WHOLE capture instead, two of eight shards would hold them all and the other six would do more
+    work in the histogram and digitizer passes than the single-GPU run (those passes skip silent tiles), which tools/timeline_dist.py
+    shows as load imbalance rather than exchange cost."""
     off = n * rank
     return off + int(0.40 * n), off + int(0.43 * n), off + int(0.97 * n)
 
@@ -272,6 +277,30 @@ def parity_block(ctx, rank, world, dist, d_iq, halo_host, d_qad, rows, center, n
     return out
 
 
+def dump_outputs(out_dir, d_qad, rows, center, n, offset, rank, world):
+    """What the last timed step returned, as DIR/<name>.npy: the detected center (detect only), qad at a fixed seeded sample of
+    positions, the pulse-table row count and a seeded sample of its rows (all of them when fewer).  world > 1: one set per rank."""
+    os.makedirs(out_dir, exist_ok=True)
+    sfx = "" if world == 1 else "_rank%d" % rank
+    rng = np.random.default_rng(20240 + rank)
+    pos = np.sort(rng.choice(n, min(n, DUMP_QAD_SAMPLES // world), replace=False))
+    q = np.empty(len(pos), np.float32)
+    chunk = 1 << 26
+    for a in range(0, n, chunk):
+        lo, hi = np.searchsorted(pos, [a, a + chunk])
+        if hi > lo:
+            q[lo:hi] = d_qad[a: min(n, a + chunk)].get()[pos[lo:hi] - a]
+    k = len(rows)
+    idx = np.arange(k) if k <= DUMP_ROWS // world else np.sort(rng.choice(k, DUMP_ROWS // world, replace=False))
+    out = {"qad_sample": q, "qad_sample_position": (offset + pos).astype(np.float64),
+           "pulse_rows_count": np.array([k], np.float64), "pulse_rows_sample": rows[idx].astype(np.float64),
+           "pulse_rows_sample_index": idx.astype(np.float64)}
+    if center is not None:
+        out["center"] = np.array([center], np.float64)
+    for name, arr in out.items():
+        np.save(os.path.join(out_dir, name + sfx + ".npy"), arr)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -287,8 +316,13 @@ def main():
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--worst", action="store_true",
                     help="also time the unfavourable inputs (noise gate off / white-noise IQ / +-300 kHz deviation: every sample pair "
-                         "leaves the packed-f32x2 fast path) and report them under `worst_case`")
+                         "leaves the paired fast path) and report them under `worst_case`")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results (seeded samples) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU implementation")
 
     rank = env_int("RANK", 0)
     local_rank = env_int("LOCAL_RANK", 0)
@@ -308,7 +342,7 @@ def main():
     if args.impl == "reference":
         if rank != 0:
             return 0
-        r = cpu_reference_arm(1 << args.cpu_log2n, 5, max(1, min(args.warmup, 2)), detect=args.center == "detect")
+        r = cpu_reference_arm(1 << args.cpu_log2n, args.steps, args.warmup, detect=args.center == "detect")
         line = dict(base)
         line.update({"impl": "reference", "value": r["value"], "ms_per_step": r["ms_per_step"],
                      "cpu_baseline": {k: r[k] for k in ("value", "unit", "cores", "kind", "sample")},
@@ -428,12 +462,17 @@ def main():
     ms_per_step = total_ms / args.steps
     value = world * n / (ms_per_step * 1e-3) / 1e6
 
-    # ---- parity of the last timed step against the CPU oracle (outside the timed region) ----------------------------
-    parity = None
-    if not args.no_parity:
+    rows_last = None
+    if not args.no_parity or args.dump_outputs:
         rows_last = np.empty((k_rows, 2), dtype=np.int64)
         if k_rows:
             ctx.check(lib.urh_fetch_pulses(ctx.handle, rows_last.ctypes.data_as(C.c_void_p), k_rows))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, d_qad, rows_last, center_seen[0] if args.center == "detect" else None, n, offset, rank, world)
+
+    # ---- parity of the last timed step against the CPU oracle (outside the timed region) ----------------------------
+    parity = None
+    if not args.no_parity:
         lens = int(rows_last[:, 1].sum())
         if dist is not None:
             import torch
@@ -446,8 +485,8 @@ def main():
                               offset)
         parity["sum_of_pulse_lengths_is_n_minus_tol"] = lens == n_total - TOL
         parity["ok"] = bool(parity["ok"] and parity["sum_of_pulse_lengths_is_n_minus_tol"])
-        del rows_last
         barrier()
+    del rows_last
 
     # ---- the other variant, for the record (not the headline): same capture, same timing rules, fewer steps ------
     other = step_given if args.center == "detect" else step_detect
@@ -602,7 +641,7 @@ def main():
         peak = float(json.load(open(peaks_path))["hbm_gbs"])
         peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3)"
     dense = float(np.mean(dense_ms))
     achieved = ALG_BYTES_PER_SAMPLE * n / (dense * 1e-3) / 1e9
     kernel_key = "k_fsk_fifo<WRITE,STATS>" if args.center == "detect" else "k_fsk_fifo<DIGITIZE,WRITE>"

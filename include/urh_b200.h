@@ -1,5 +1,5 @@
 /*
- * urh_b200 — C ABI of the B200-native IQ hot path (drop-in for urh.cythonext.* on this path).
+ * urh_b200 — C ABI of the H100-native IQ hot path (drop-in for urh.cythonext.* on this path).
  *
  * Every entry point is `extern "C"`, takes plain pointers and sizes, and returns 0 on success or a
  * negative URH_ERR_* code (the ctypes shim maps these onto the Python exceptions the reference raises).
@@ -287,7 +287,7 @@ int urh_last_dense_ms(urh_ctx* ctx, float* ms);
 /* speculative Costas loop diagnostics of the last PSK demodulation: {chunks matched in O(1), chunks walked, samples stepped serially} */
 int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3);
 int64_t urh_costas_last_redone(urh_ctx* ctx);
-/* packed (f32x2) division used by the FSK fast path vs __fdiv_rn on `count` random operand pairs */
+/* paired (float2) division used by the FSK fast path vs __fdiv_rn on `count` random operand pairs */
 int urh_selftest_packed_div(urh_ctx* ctx, uint64_t seed, int64_t count, int64_t* mismatches, int64_t* tested);
 /* synthetic phase-continuous 2-FSK bursts + AWGN + noise-only gaps generated in HBM (SURVEY 8d recipe) */
 int urh_synth_fsk(urh_ctx* ctx, float* d_iq, int64_t n, int64_t global_offset, int sps, const int8_t* d_sym_bit,

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): CUDA afp_demod / grab_pulse_lens / fused path vs the
+"""GPU parity tests (run with -m gpu on the H100): CUDA afp_demod / grab_pulse_lens / fused path vs the
 oracle and the committed golden vectors.  Bit-exact is the bar for ASK/FSK/PSK demodulated samples and for all
 pulse tables."""
 import numpy as np

@@ -2,47 +2,55 @@
 32 bit, one and two channels), Flipper ``.sub`` run lengths, ``.coco`` archives and the raw sample formats by file extension -
 loaded by urh_b200.signalprocessing.Signal and by the reference's own class: same samples, dtype, sample rate and
 already-demodulated flag.  The noise threshold is fixed through the settings so that no GPU is needed (with "automatic" the
-constructor runs detect_noise_level on the device).  Needs the reference tree (build container); skipped elsewhere."""
-import os
+constructor runs detect_noise_level on the device).  The reference's answers are recorded in tests/golden/ref_signal_files.json
+(oracle/cassette.py)."""
 import tarfile
 import wave
 
 import numpy as np
 import pytest
 
-REF = "/root/reference/src/urh/signalprocessing/Signal.py"
-needs_reference = pytest.mark.skipif(not os.path.isfile(REF), reason="reference tree not present")
+from oracle.cassette import RECORD, Cassette, same
+
+
+@pytest.fixture
+def cassette(request):
+    c = Cassette("signal_files", request.node.name)
+    yield c
+    c.close()
 
 
 @pytest.fixture(scope="module")
 def classes():
-    from oracle import ref_loader
-    ns = ref_loader.load_python_layer()
     from urh_b200 import settings
     from urh_b200.signalprocessing.Signal import Signal
 
+    ref_cls = None
+    if RECORD:
+        from oracle import ref_loader
+        ref_cls = ref_loader.load_python_layer().Signal
     settings.write("default_noise_threshold", "3")
-    yield Signal, ns.Signal
+    yield Signal, ref_cls
     settings.write("default_noise_threshold", "automatic")
 
 
-def both(classes, path):
+def both(cassette, classes, path):
     mine_cls, ref_cls = classes
-    mine, ref = mine_cls(str(path), "t"), ref_cls(str(path), "t")
-    a, b = np.asarray(mine.iq_array.data), np.asarray(ref.iq_array.data)
-    assert a.dtype == b.dtype and a.shape == b.shape
-    assert np.array_equal(a.view(np.uint8), b.view(np.uint8))          # bit-identical samples
-    assert mine.sample_rate == ref.sample_rate
-    assert mine.already_demodulated == ref.already_demodulated
-    assert mine.wav_mode == ref.wav_mode
-    assert mine.num_samples == ref.num_samples
-    return mine, ref
+    mine, ref = mine_cls(str(path), "t"), cassette.make(lambda: ref_cls(str(path), "t"))
+    a = np.asarray(mine.iq_array.data)
+    assert a.dtype == cassette.want(lambda: np.asarray(ref.iq_array.data).dtype)
+    assert a.shape == cassette.want(lambda: np.asarray(ref.iq_array.data).shape)
+    assert same(a.view(np.uint8), cassette.want(lambda: np.asarray(ref.iq_array.data).view(np.uint8)))   # bit-identical samples
+    assert mine.sample_rate == cassette.want(lambda: ref.sample_rate)
+    assert mine.already_demodulated == cassette.want(lambda: ref.already_demodulated)
+    assert mine.wav_mode == cassette.want(lambda: ref.wav_mode)
+    assert mine.num_samples == cassette.want(lambda: ref.num_samples)
+    return mine
 
 
-@needs_reference
 @pytest.mark.parametrize("width", [1, 2, 3, 4])
 @pytest.mark.parametrize("channels", [1, 2])
-def test_wav(classes, tmp_path, width, channels):
+def test_wav(cassette, classes, tmp_path, width, channels):
     rng = np.random.default_rng(10 * width + channels)
     frames, rate = 1234, 48000 if channels == 1 else 250000
     raw = rng.integers(0, 256, frames * channels * width, dtype=np.uint8).tobytes()
@@ -52,24 +60,22 @@ def test_wav(classes, tmp_path, width, channels):
         f.setsampwidth(width)
         f.setframerate(rate)
         f.writeframes(raw)
-    mine, ref = both(classes, path)
+    mine = both(cassette, classes, path)
     assert mine.sample_rate == rate
     assert mine.already_demodulated == (channels == 1)
 
 
-@needs_reference
-def test_flipper_sub(classes, tmp_path):
+def test_flipper_sub(cassette, classes, tmp_path):
     path = tmp_path / "remote.sub"
     path.write_text("Filetype: Flipper SubGhz RAW File\nVersion: 1\nFrequency: 433920000\nProtocol: RAW\n"
                     "RAW_Data: 300 -900 300 -300 900 -9000\nRAW_Data: 450 -450 1350 -100\nsomething else: 5\n")
-    mine, _ = both(classes, path)
+    mine = both(cassette, classes, path)
     assert mine.already_demodulated and mine.num_samples == 300 + 900 + 300 + 300 + 900 + 9000 + 450 + 450 + 1350 + 100
 
 
-@needs_reference
 @pytest.mark.parametrize("ext,dtype", [(".complex", np.float32), (".cs8", np.int8), (".complex16s", np.int8), (".cs16", np.int16),
                                        (".complex32s", np.int16)])
-def test_raw_formats_and_coco(classes, tmp_path, ext, dtype):
+def test_raw_formats_and_coco(cassette, classes, tmp_path, ext, dtype):
     rng = np.random.default_rng(len(ext))
     n = 777
     if dtype == np.float32:
@@ -79,13 +85,13 @@ def test_raw_formats_and_coco(classes, tmp_path, ext, dtype):
         data = rng.integers(info.min, info.max + 1, (n, 2)).astype(dtype)
     path = tmp_path / ("capture" + ext)
     data.tofile(str(path))
-    mine, _ = both(classes, path)
+    mine = both(cassette, classes, path)
     assert mine.iq_array.data.dtype == dtype and np.array_equal(mine.iq_array.data, data)
     # the same file inside a .coco archive (Signal.py:190-205)
     coco = tmp_path / ("capture" + ext.replace(".", "_") + ".coco")
     with tarfile.open(str(coco), "w:bz2") as tar:
         tar.add(str(path), arcname="capture" + ext)
-    mine2, _ = both(classes, coco)
+    mine2 = both(cassette, classes, coco)
     assert np.array_equal(mine2.iq_array.data, data)
 
 

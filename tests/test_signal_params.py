@@ -1,13 +1,27 @@
 """CPU: the parameter setters of urh_b200.signalprocessing.Signal (one descriptor table) behave like the reference's
 hand-written properties (Signal.py:215-400): same values, same events in the same order with the same arguments, same
-invalidation of the cached demodulation.  Needs the reference tree (build container); skipped elsewhere."""
-import os
-
+invalidation of the cached demodulation.  The reference's answers are recorded in tests/golden/ref_signal_params.json
+(oracle/cassette.py)."""
 import numpy as np
 import pytest
 
-REF = "/root/reference/src/urh/signalprocessing/Signal.py"
-pytestmark = pytest.mark.skipif(not os.path.isfile(REF), reason="reference tree not present")
+from oracle.cassette import RECORD, Cassette, fingerprint, same
+
+
+@pytest.fixture
+def cassette(request):
+    c = Cassette("signal_params", request.node.name)
+    yield c
+    c.close()
+
+
+@pytest.fixture(scope="module")
+def ref():
+    if not RECORD:
+        return None
+    from oracle import ref_loader
+    return ref_loader.load_python_layer()
+
 
 EVENTS = ("samples_per_symbol_changed", "tolerance_changed", "noise_threshold_changed", "center_changed",
           "center_spacing_changed", "name_changed", "sample_rate_changed", "modulation_type_changed",
@@ -49,58 +63,54 @@ SCRIPT = [
 ]
 
 
-def test_parameter_setters_match_reference():
-    from oracle import ref_loader
-    ns = ref_loader.load_python_layer()
+def test_parameter_setters_match_reference(cassette, ref):
     from urh_b200.signalprocessing.Signal import Signal
 
-    mine, ref = Signal("", "x", sample_rate=1e6), ns.Signal("", "x", sample_rate=1e6)
-    log_mine, log_ref = instrument(mine), instrument(ref)
+    mine = Signal("", "x", sample_rate=1e6)
+    theirs = cassette.make(lambda: ref.Signal("", "x", sample_rate=1e6))
+    log_mine, log_ref = instrument(mine), cassette.make(lambda: instrument(theirs))
     for attr, value in SCRIPT:
-        for s in (mine, ref):
-            s._qad = np.zeros(3, np.float32)   # a cached demodulation that the setter may have to drop
+        mine._qad = np.zeros(3, np.float32)   # a cached demodulation that the setter may have to drop
         setattr(mine, attr, value)
-        setattr(ref, attr, value)
-        assert (mine._qad is None) == (ref._qad is None), (attr, value)
+        cassette.make(lambda: setattr(theirs, "_qad", np.zeros(3, np.float32)))
+        cassette.make(lambda: setattr(theirs, attr, value))
+        assert (mine._qad is None) == cassette.want(lambda: theirs._qad is None), (attr, value)
         if attr != "block_protocol_update":
-            assert getattr(mine, attr) == getattr(ref, attr), (attr, value)
-            assert type(getattr(mine, attr)) is type(getattr(ref, attr)), (attr, value)
-    assert log_mine == log_ref
-    assert mine.modulation_order == ref.modulation_order == 8
+            got = getattr(mine, attr)
+            assert got == cassette.want(lambda: getattr(theirs, attr)), (attr, value)
+            assert type(got).__name__ == cassette.want(lambda: type(getattr(theirs, attr)).__name__), (attr, value)
+    assert log_mine == cassette.want(lambda: log_ref)
+    assert mine.modulation_order == cassette.want(lambda: theirs.modulation_order) == 8
 
 
-def test_construction_defaults_match_reference():
-    from oracle import ref_loader
-    ns = ref_loader.load_python_layer()
+def test_construction_defaults_match_reference(cassette, ref):
     from urh_b200.signalprocessing.Signal import Signal
 
     for kw in (dict(), dict(modulation="ASK", sample_rate=250e3, timestamp=3.0)):
-        mine, ref = Signal("", "n", **kw), ns.Signal("", "n", **kw)
+        mine, theirs = Signal("", "n", **kw), cassette.make(lambda: ref.Signal("", "n", **kw))
         for attr in ("name", "tolerance", "samples_per_symbol", "pause_threshold", "message_length_divisor", "costas_loop_bandwidth",
                      "center", "sample_rate", "bits_per_symbol", "center_spacing", "modulation_type", "timestamp", "noise_threshold",
                      "already_demodulated", "modulation_order"):
-            assert getattr(mine, attr) == getattr(ref, attr), attr
-        assert mine.parameter_cache == ref.parameter_cache
+            assert getattr(mine, attr) == cassette.want(lambda: getattr(theirs, attr)), attr
+        assert mine.parameter_cache == cassette.want(lambda: theirs.parameter_cache)
 
 
-def test_edit_operations_match_reference():
+def test_edit_operations_match_reference(cassette, ref):
     """insert / delete / mute / crop (Signal.py:613-651) on host data: same samples, same cached demodulation, same flags"""
-    from oracle import ref_loader
-    ns = ref_loader.load_python_layer()
     from urh_b200.signalprocessing.Signal import Signal
 
     rng = np.random.default_rng(8)
     for trial in range(20):
         n = int(rng.integers(20, 200))
         iq = rng.integers(-100, 100, (n, 2)).astype(np.int16) if trial % 2 else rng.standard_normal((n, 2)).astype(np.float32)
-        mine, ref = Signal.from_samples(iq.copy(), "e", 1e6), ns.Signal.from_samples(iq.copy(), "e", 1e6)
+        mine, theirs = Signal.from_samples(iq.copy(), "e", 1e6), cassette.make(lambda: ref.Signal.from_samples(iq.copy(), "e", 1e6))
         qad = rng.standard_normal(n).astype(np.float32)
-        for s in (mine, ref):
-            s._qad = qad.copy()
-            s.parameter_cache["FSK"]["center"] = 0.5
         a, b = sorted(int(v) for v in rng.integers(0, n, 2))
         op = trial % 4
-        for s in (mine, ref):
+
+        def edit(s):
+            s._qad = qad.copy()
+            s.parameter_cache["FSK"]["center"] = 0.5
             if op == 0:
                 s.mute_range(a, b)
             elif op == 1:
@@ -109,9 +119,13 @@ def test_edit_operations_match_reference():
                 s.crop_to_range(a, max(b, a + 1))
             else:
                 s.insert_data(a, iq[:5].copy())
-        assert np.array_equal(mine.iq_array.data, ref.iq_array.data), (trial, op)
-        assert (mine._qad is None) == (ref._qad is None), (trial, op)
+        edit(mine)
+        cassette.make(lambda: edit(theirs))
+        assert same(mine.iq_array.data, cassette.want(lambda: np.asarray(theirs.iq_array.data))), (trial, op)
+        assert mine.iq_array.data.dtype == cassette.want(lambda: theirs.iq_array.data.dtype)
+        ref_qad = cassette.want(lambda: None if theirs._qad is None else np.asarray(theirs._qad))
+        assert (mine._qad is None) == (ref_qad is None), (trial, op)
         if mine._qad is not None:
-            assert np.array_equal(mine._qad, ref._qad), (trial, op)
-        assert mine.changed == ref.changed and mine.num_samples == ref.num_samples
-        assert mine.parameter_cache == ref.parameter_cache
+            assert same(mine._qad, ref_qad), (trial, op)
+        assert mine.changed == cassette.want(lambda: theirs.changed) and mine.num_samples == cassette.want(lambda: theirs.num_samples)
+        assert fingerprint(mine.parameter_cache) == cassette.want(lambda: fingerprint(theirs.parameter_cache))

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""BASELINE.json configs[2] and configs[3] end to end on one B200 (data resident in HBM, CUDA-event timing per stage).
+"""BASELINE.json configs[2] and configs[3] end to end on one H100 (data resident in HBM, CUDA-event timing per stage).
 One JSON object per line.
 
   configs[2]: 256 MiSample ASK capture -> FIR band-pass (101 taps) -> ASK demod -> spectrogram STFT(1024, hop 512)
   configs[3]: GFSK Modulator.modulate of 10 M random bits -> IQ -> FSK demod + digitize -> bits, bit-exact round trip
 
-    python tools/bench_configs.py [--log2n 28] [--bits 10000000] > profiles/r01_configs.jsonl
+    python tools/bench_configs.py [--log2n 28] [--bits 10000000] > configs.jsonl
 """
 import argparse
 import ctypes as C

@@ -2,7 +2,7 @@
 """Secondary measurements (not the headline bench): every other row of the scope table with data resident in HBM,
 CUDA-event timing, algorithmic bytes per SURVEY §8d.  Writes one JSON object per line.
 
-    python tools/bench_paths.py [--log2n 26] > profiles/r01_secondary.jsonl
+    python tools/bench_paths.py [--log2n 26] > secondary.jsonl
 """
 import argparse
 import ctypes as C
@@ -45,7 +45,7 @@ def main():
     ctx = _lib.default_context()
     lib = ctx.lib
     n = 1 << args.log2n
-    peak = 6574.1
+    peak = 3350.0   # H100 SXM data sheet (HBM3), unless MEASURED_PEAKS.json gives a measured figure
     try:
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
@@ -56,7 +56,7 @@ def main():
         if bytes_per_sample:
             rec["algorithmic_B_per_sample"] = bytes_per_sample
             rec["GB_per_s"] = samples * bytes_per_sample / ms / 1e6
-            rec["frac_of_measured_hbm_peak"] = rec["GB_per_s"] / peak
+            rec["frac_of_hbm_peak"] = rec["GB_per_s"] / peak
         if note:
             rec["note"] = note
         print(json.dumps(rec), flush=True)

@@ -6,7 +6,7 @@ the CPU oracle (C restatement / reference build, all host threads), compared bit
   * detect_center within 2e-6
 Needs ~30 GB of host memory and a minute or two of CPU time at 2^30; not part of the pytest suite.
 
-    python tools/parity_full.py [--log2n 30] > profiles/rNN_parity_full.json
+    python tools/parity_full.py [--log2n 30] > parity_full.json
 """
 import argparse
 import ctypes as C

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""SASS evidence for profiles/: opcode histogram + the hottest basic block (by static size heuristics: the longest run of
+"""SASS evidence: opcode histogram + the hottest basic block (by static size heuristics: the longest run of
 arithmetic between two branches) of one kernel in a built object.
 
-    python tools/sass_excerpt.py urh_b200/build/digitize.o 'k_fsk_fifoILi4ELb0ELb1ELb1' > profiles/r02_sass_k_fsk_fifo_stats.txt"""
+    python tools/sass_excerpt.py urh_b200/build/digitize.o 'k_fsk_fifoILi4ELb0ELb1ELb1' > sass_k_fsk_fifo_stats.txt"""
 import collections
 import re
 import subprocess

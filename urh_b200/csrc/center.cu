@@ -381,7 +381,7 @@ template <bool SMEM, bool FAST>
 __device__ __forceinline__ void hist_put(HistCache& hc, const HistBins& hb, unsigned int* s_hist, unsigned long long* hist, float f,
                                          unsigned one) {
     // per entry: two compares chained into one predicate and a predicated increment, spelled out in PTX.  The kernel is bound by
-    // the ALU pipe (FSETP, predicate logic: ncu r02), so the increments are multiply-adds by a run-time 1 - IMAD runs on the
+    // the ALU pipe (FSETP, predicate logic), so the increments are multiply-adds by a run-time 1 - IMAD runs on the
     // FMA pipe - and the hit path tests the lower validity bound only (noise samples sit below it; a sample above the last edge
     // falls through to the miss path, which tests both bounds).  miss = not below the range and in no cached bin.
     unsigned miss;

@@ -99,7 +99,7 @@ k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
 }
 
 // Fast kernel: full, aligned, order-2 FSK tiles [tile_begin, tile_begin + tile_count), tile_begin >= 1
-// (fsk_fast.cuh: packed f32x2 math, same bits as the generic kernel).
+// (fsk_fast.cuh: float2-paired math, same bits as the generic kernel).
 template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
 __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, URH_FAST_MIN_BLOCKS)
 k_fsk_fast(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
@@ -211,7 +211,7 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
                    tile_stats);
         return URH_OK;
     };
-    // FSK on aligned buffers with a binary digitizer: tiles 1 .. nfull-1 take the packed-f32x2 kernel
+    // FSK on aligned buffers with a binary digitizer: tiles 1 .. nfull-1 take the paired fast kernel
     const int64_t nfull = n / URH_TILE;
     const bool fast = MOD == URH_MOD_FSK && vec_in && (!d_qad || vec_out) && (!DIG || cls.order == 2) && nfull > 1;
     URH_PROF_BEGIN(ctx);
@@ -219,7 +219,7 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
         const int64_t fb = tile_lo > 1 ? tile_lo : 1, fe = tile_hi < nfull ? tile_hi : nfull;
         if (fe > fb) {
             const unsigned grid = (unsigned)urh_div_up(fe - fb, URH_WARPS_PER_BLOCK);
-            // the variant that stages its input through the shared-memory FIFO (float32: 2230 vs 2417 us at 2^30 samples)
+            // the variant that stages its input through the shared-memory FIFO (URH_B200_FSK_NO_FIFO selects the register-fed loop)
             static const bool fifo = getenv("URH_B200_FSK_NO_FIFO") == nullptr;
             const bool ff = fifo;
             if (tile_stats && d_qad && !DIG) {

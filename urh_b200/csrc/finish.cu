@@ -12,7 +12,7 @@
 //   D  rows                per tile: walk again, write (state, length) rows at the tile's row offset; the last
 //                          tile appends the tail row (pyx:485-493) and the row count
 // (C and D run one THREAD per tile: a tile holds ~20 candidates, and 32 independent walks per warp keep far more loads in
-// flight than one warp per tile did — measured 42 + 104 us against 113 + 128 us at 2^19 tiles.)
+// flight than one warp per tile would.)
 //
 // One read-back (row count) ends the call.  Rows go straight into the context's pulse buffer, sized optimistically;
 // an overflow only repeats stage D.  ASK (short pauses relabelled, pyx:471-473, so equal neighbours can meet) runs a

@@ -5,7 +5,7 @@
 // Provenance of every constant and of the operation order: NOT glibc source, but the machine code and
 // .rodata of THIS image's /usr/lib/x86_64-linux-gnu/libm.so.6 (glibc 2.39-0ubuntu8.5, build-id
 // 0d9969fe206760d250ec30a5a9be18aefbf84ea8), read with objdump/readelf in round 1:
-//   * sinf / cosf are IFUNCs; on CPUs with FMA+AVX2 (this container's Xeon and the B200 host) they resolve
+//   * sinf / cosf are IFUNCs; on CPUs with FMA+AVX2 (the x86-64 hosts the GPUs sit in) they resolve
 //     to the FMA variants at 0x7e800 / 0x7e330, whose double-precision polynomial steps are contracted
 //     into vfmadd exactly as written below (fma() here == one IEEE fused operation, as on the GPU);
 //   * the 14-double table __sincosf_table[2] sits at 0xb8120 (signs, 2/pi*2^24, pi/2, c0,c1,s1,c2,s2,c3,s3,c4);

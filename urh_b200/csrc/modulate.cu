@@ -171,8 +171,8 @@ __global__ void __launch_bounds__(128) k_gfsk_phases(const int64_t* __restrict__
             //  * ph normal; every partial sum strictly inside the binade [2^23 + 1, 2^24 - 1] ulps, same sign;
             //  * no increment within 1e-6 ulp of a rounding tie (the double addition's own rounding moves the sum by < 2^-29 ulp,
             //    which then cannot change the float rounding).
-            // (r02 also tried consuming a block in segments split at the binade crossings: 94 % of the steps went through prefix
-            // sums, but the longer dependent chain per block made the kernel slower — 22 ms against 13 ms per 10^9 samples.)
+            // (Consuming a block in segments split at the binade crossings sends more steps through prefix sums, but the longer
+            // dependent chain per block makes the kernel slower.)
             bool fast = false;
             {
                 const uint32_t pb = __float_as_uint(ph);

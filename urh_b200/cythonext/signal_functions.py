@@ -103,7 +103,7 @@ def grab_pulse_lens(samples, center: float, tolerance: int, modulation_type: str
 
 def demod_digitize(samples, noise_mag: float, mod_type: str, center: float, tolerance: int, samples_per_symbol: int,
                    bits_per_symbol: int = 1, center_spacing: float = 0.1, return_qad: bool = True):
-    """Fused afp_demod + grab_pulse_lens in ONE pass over the IQ samples (B200 addition; same results as
+    """Fused afp_demod + grab_pulse_lens in ONE pass over the IQ samples (addition to the reference API; same results as
     calling the two reference functions back to back).  Returns (qad or None, int64[k,2])."""
     samples = _check_iq(samples)
     on_device = isinstance(samples, DeviceArray)
@@ -246,7 +246,7 @@ _MOD_CODES = {"ask": _lib.MOD_ASK, "fsk": _lib.MOD_FSK, "psk": _lib.MOD_PSK, "gf
 def modulate_batch(messages, samples_per_symbol, modulation_type, parameters, bits_per_symbol, carrier_amplitude,
                    carrier_frequency, carrier_phase, sample_rate, pauses, start=0, dtype=np.float32, gauss_bt=0.5,
                    filter_width=1.0, device_result=False):
-    """Modulate a batch of bit arrays that share one parameter set in ONE launch sequence (B200 addition; per message
+    """Modulate a batch of bit arrays that share one parameter set in ONE launch sequence (addition to the reference API; per message
     the result equals modulate_c(bits, ..., pause, start)).  Returns a list of (total,2) arrays (or one DeviceArray +
     offsets when device_result=True)."""
     dtype = np.dtype(dtype)

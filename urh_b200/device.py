@@ -1,4 +1,4 @@
-"""Device-resident arrays (HBM) and pinned host arrays for the B200 hot path."""
+"""Device-resident arrays (HBM) and pinned host arrays for the GPU hot path."""
 import ctypes as C
 
 import numpy as np

@@ -97,10 +97,9 @@ def init_p2p(ctx: _lib.Context, hx: HostExchange):
     """NVLink peer mailboxes for the few-bytes exchanges (p2p.cu): host-side all-gathers and the device-resident, stream-ordered
     all-gather / histogram sum the sharded chains use between their kernels.  Used only if EVERY rank could map every peer (one
     node, <= 8 GPUs, CUDA IPC available); otherwise those exchanges stay on NCCL.
-    Opt-in with URH_B200_P2P=1.  Measured at 2 GPUs (round 2): 8.3 us per device all-gather against 7.2 us for NCCL's, 9.1 / 14.9 us
-    for the histogram sum of 8 / 6000 words against 10.4 us; the step is 4.23 ms with the mailboxes and 4.21 ms with NCCL -- the
-    per-step cost of a sharded capture is rank skew and the small device stages between the exchanges, not the collective's
-    latency -- so NCCL stays the default (DESIGN.md section 6)."""
+    Opt-in with URH_B200_P2P=1: the exchanges carry a few bytes to a few KB, so a sharded step's cost is dominated by rank skew and
+    the small device stages between the exchanges rather than by the collective's latency, and NCCL stays the default
+    (DESIGN.md section 6)."""
     ctx.p2p = False
     ok = hx.world <= 8 and hx.world > 1 and os.environ.get("URH_B200_P2P", "0") == "1"
     handle = C.create_string_buffer(64)
