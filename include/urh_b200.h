@@ -287,6 +287,11 @@ int urh_last_dense_ms(urh_ctx* ctx, float* ms);
 /* speculative Costas loop diagnostics of the last PSK demodulation: {chunks matched in O(1), chunks walked, samples stepped serially} */
 int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3);
 int64_t urh_costas_last_redone(urh_ctx* ctx);
+/* how the stitch pass of the last PSK demodulation resolved its super-chunks: {adopted from family A, adopted from family B,
+ * chained by the stitch warp itself, segments per chunk}; super-chunk 0 of an unsharded capture is not counted.  The serial
+ * kernel (captures shorter than 8192 samples) zeroes these and urh_costas_stats and reports segs = 0.
+ * $URH_B200_COSTAS_SEGS = 2, 4, 8 or 16 forces the speculative path's chunk layout (the result does not depend on it). */
+int urh_costas_stitch_stats(urh_ctx* ctx, int64_t* h_out4);
 /* paired (float2) division used by the FSK fast path vs __fdiv_rn on `count` random operand pairs */
 int urh_selftest_packed_div(urh_ctx* ctx, uint64_t seed, int64_t count, int64_t* mismatches, int64_t* tested);
 /* synthetic phase-continuous 2-FSK bursts + AWGN + noise-only gaps generated in HBM (SURVEY 8d recipe) */

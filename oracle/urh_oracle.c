@@ -43,11 +43,40 @@ float oracle_noise_value(int mod_type) {
     }
 }
 
-/* std::complex<float> product (a+ib)(c+id) as GCC evaluates it without -ffast-math */
+/* std::complex<float> product (a+ib)(c+id) as GCC evaluates it without -ffast-math: the naive product, and when both parts
+ * are NaN, libgcc's __mulsc3 recovery (C99 Annex G, G.5.1): an infinite operand gives an infinite result */
 static inline void cmulf(float a, float b, float c, float d, float* re, float* im) {
     const float ac = a * c, bd = b * d, ad = a * d, bc = b * c;
     *re = ac - bd;
     *im = ad + bc;
+    if (isnan(*re) && isnan(*im)) {
+        int recalc = 0;
+        if (isinf(a) || isinf(b)) {
+            a = copysignf(isinf(a) ? 1.0f : 0.0f, a);
+            b = copysignf(isinf(b) ? 1.0f : 0.0f, b);
+            if (isnan(c)) c = copysignf(0.0f, c);
+            if (isnan(d)) d = copysignf(0.0f, d);
+            recalc = 1;
+        }
+        if (isinf(c) || isinf(d)) {
+            c = copysignf(isinf(c) ? 1.0f : 0.0f, c);
+            d = copysignf(isinf(d) ? 1.0f : 0.0f, d);
+            if (isnan(a)) a = copysignf(0.0f, a);
+            if (isnan(b)) b = copysignf(0.0f, b);
+            recalc = 1;
+        }
+        if (!recalc && (isinf(ac) || isinf(bd) || isinf(ad) || isinf(bc))) {
+            if (isnan(a)) a = copysignf(0.0f, a);
+            if (isnan(b)) b = copysignf(0.0f, b);
+            if (isnan(c)) c = copysignf(0.0f, c);
+            if (isnan(d)) d = copysignf(0.0f, d);
+            recalc = 1;
+        }
+        if (recalc) {
+            *re = INFINITY * (a * c - b * d);
+            *im = INFINITY * (a * d + b * c);
+        }
+    }
 }
 
 /* Costas loop — src/urh/cythonext/signal_functions.pyx:252-330 */

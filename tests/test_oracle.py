@@ -132,3 +132,58 @@ def test_oracle_vs_compiled_reference_random(oracle):
             a[0] = b[0] if mod == "PSK" else a[0]
             assert bits_equal(a, b) == 0, (dt, mod)
         assert np.array_equal(ut.get_magnitudes(iq), oracle.get_magnitudes(iq), equal_nan=True)
+
+
+def _costas_cases():
+    """seeded 40 000-sample PSK captures with bursts and gaps in every dtype, loop orders 2 / 4 / 8, eight loop bandwidths; then
+    float32 captures with huge, infinite and NaN samples"""
+    rng = np.random.default_rng(11)
+    n = 40_000
+    on = (np.arange(n) % 15000) < 11000
+    for dt, (scale, zero, noise) in ((np.int8, (100, 0, 20.0)), (np.uint8, (100, 128, 0.0)), (np.int16, (20000, 0, 4000.0)),
+                                     (np.uint16, (20000, 32768, 0.0)), (np.float32, (1, 0, 0.2))):
+        for order in (2, 4, 8):
+            sym = rng.integers(0, order, n // 300 + 1)
+            x = on * np.exp(1j * (2 * np.pi * 0.025 * np.arange(n) + np.repeat(2 * np.pi * sym / order, 300)[:n]))
+            x = x + 0.05 * (rng.standard_normal(n) + 1j * rng.standard_normal(n))
+            iq = np.stack([x.real, x.imag], axis=1) * scale + zero
+            iq = iq.astype(np.float32) if dt == np.float32 else np.clip(np.round(iq), np.iinfo(dt).min, np.iinfo(dt).max).astype(dt)
+            for bw in (0.001, 0.01, 0.05, 0.1, 0.2, 0.5, 1.0, 2.0):
+                yield iq, noise, order, bw
+    x = np.exp(1j * (2 * np.pi * 0.025 * np.arange(n) + np.pi * np.repeat(rng.integers(0, 2, n // 300 + 1), 300)[:n]))
+    base = np.stack([x.real, x.imag], axis=1).astype(np.float32)
+    for val in ((1e30, -1e30), (-1e30, 1e30), (np.inf, 0.0), (-np.inf, 0.0), (0.3, np.inf), (-0.3, -np.inf), (np.inf, np.inf),
+                (np.nan, 0.5), (0.5, np.nan)):
+        iq = base.copy()
+        iq[[5000, 5007, 30000]] = val
+        for order in (2, 4):
+            yield iq, 0.2, order, 0.1
+
+
+def _costas_words(q):
+    """the result words after index 0 (np.empty in the reference), NaN folded to one word: its payload is not pinned"""
+    w = np.asarray(q, dtype=np.float32)[1:].view(np.uint32).copy()
+    w[np.isnan(np.asarray(q, dtype=np.float32)[1:])] = 0x7FC00000
+    return w
+
+
+def test_oracle_costas_pinned_to_reference(oracle, request):
+    """The oracle's Costas loop (PSK afp_demod) against the reference's compiled costa_demod: every dtype, loop order and
+    bandwidth, and non-finite samples (an infinite imaginary part takes the Annex G recovery of the complex product).  The
+    reference's answers are recorded in tests/golden/ref_costas.json, so the pin also runs without the reference; with
+    oracle/_ref built it also runs live."""
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette, same
+
+    c = Cassette("costas", request.node.name)
+    sf = ref_loader.load_kernels()[0] if (RECORD or ref_loader.kernels_available()) else None
+    cases = 0
+    for iq, noise, order, bw in _costas_cases():
+        mine = _costas_words(oracle.afp_demod(iq, noise, "PSK", order, bw))
+        want = c.want(lambda: _costas_words(sf.afp_demod(iq, noise, "PSK", order, bw)))
+        assert same(mine, want), (iq.dtype, order, bw, cases)
+        if sf is not None:
+            assert np.array_equal(mine, _costas_words(sf.afp_demod(iq, noise, "PSK", order, bw))), (iq.dtype, order, bw, cases)
+        cases += 1
+    c.close()
+    assert cases == 5 * 3 * 8 + 9 * 2

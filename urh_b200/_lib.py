@@ -149,6 +149,7 @@ SIGNATURES = {
     "urh_costas_shard_adopt": (i32, [vp, i32, vp]),
     "urh_costas_stats": (i32, [vp, vp]),
     "urh_costas_last_redone": (i64, [vp]),
+    "urh_costas_stitch_stats": (i32, [vp, vp]),
     "urh_selftest_packed_div": (i32, [vp, C.c_uint64, i64, C.POINTER(i64), C.POINTER(i64)]),
     "urh_bgra_lookup": (i32, [vp, vp, i64, i64, vp, i32, f32, f32, i32, vp]),
     "urh_modulate_stats": (i32, [vp, vp]),

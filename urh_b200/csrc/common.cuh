@@ -60,6 +60,7 @@ struct urh_ctx {
     // NCCL (nccl.cu)
     int64_t costas_stats[3];
     int64_t costas_redone;  // super-chunks the stitch pass had to chain itself
+    int64_t costas_stitch[4];  // {super-chunks adopted from family A, from family B, chained by the stitch warp, segs}
     // cuFFT plans of detect_modulation / cwt_haar: [0] C2C, [1] Z2Z, batch 2, length mod_plan_n
     int mod_plan[2];
     int mod_plan_valid[2];

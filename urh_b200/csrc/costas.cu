@@ -70,8 +70,11 @@ __global__ void __launch_bounds__(32) k_costas(const void* __restrict__ iq, int6
                 // nco_out = cosf(-phase) + 1j*sinf(-phase)
                 const float nr = __fadd_rn(cn, __fsub_rn(__fmul_rn(0.0f, sn), 0.0f));
                 const float ni = __fadd_rn(0.0f, __fadd_rn(0.0f, sn));
-                const float xr = __fsub_rn(__fmul_rn(nr, cs_r), __fmul_rn(ni, cs_i));
-                const float xi = __fadd_rn(__fmul_rn(nr, cs_i), __fmul_rn(ni, cs_r));
+                // nco_times_sample = nco_out * current_sample: GCC's complex product, Annex G recovery included (an
+                // infinite imaginary part of the sample gives an infinite product, not NaN); 1j*jf and 1j*sin above never
+                // reach the recovery (only one of their parts can be NaN unless jf is NaN, and then no operand is infinite)
+                float xr, xi;
+                urh_cmulf(nr, ni, cs_r, cs_i, xr, xi);
                 float err;
                 if (P.order == 2) err = __fmul_rn(xi, xr);
                 else {
@@ -135,6 +138,10 @@ int urh_costas_demod_serial(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     }
     P.order = loop_order > 4 ? 4 : loop_order;  // pyx:285-287
+    // the speculative path's diagnostics describe the last PSK call: this one has no chunks, chains or stitch (segs = 0)
+    for (int i = 0; i < 3; i++) ctx->costas_stats[i] = 0;
+    ctx->costas_redone = 0;
+    for (int i = 0; i < 4; i++) ctx->costas_stitch[i] = 0;
     // result[0] is uninitialised in the reference (np.empty, pyx:265); we define it as 0.
     switch (dtype) {
         case URH_DT_I8: URH_LAUNCH(ctx, k_costas<URH_DT_I8>, 1, 32, 0, d_iq, n, P, d_out, 1); break;

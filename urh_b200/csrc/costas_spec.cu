@@ -19,11 +19,13 @@
 #include "glibc_sincosf.h"
 
 #include <math.h>
+#include <stdlib.h>
 
 #define CS_SEG 256
 #define CS_MAX_SEGS 16          // chunk = segs * 256 samples, segs in {2,4,8,16} chosen from the capture length
 #define CS_WARM 1024
 #define CS_MAXBR 4
+#define CS_STATS 6              // per stitch hypothesis: {O(1) chunks, walked chunks, samples stepped, self-chained, A, B}
 
 struct CsParams {
     float noise_sqrd, alpha, beta, scale, shift;
@@ -60,8 +62,8 @@ __device__ __forceinline__ bool cs_step(CsState& s, float re, float im, const Cs
     if (!ok) sincosf(-s.phase, &sn, &cn);
     const float nr = __fadd_rn(cn, __fmul_rn(0.0f, sn));
     const float ni = __fadd_rn(0.0f, __fadd_rn(0.0f, sn));
-    const float xr = __fsub_rn(__fmul_rn(nr, cs_r), __fmul_rn(ni, cs_i));
-    const float xi = __fadd_rn(__fmul_rn(nr, cs_i), __fmul_rn(ni, cs_r));
+    float xr, xi;
+    urh_cmulf(nr, ni, cs_r, cs_i, xr, xi);   // the products 1j*jf and 1j*sin never reach the Annex G recovery
     float err;
     if (P.order == 2) err = __fmul_rn(xi, xr);
     else {
@@ -382,11 +384,11 @@ __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, i
     const int lane = threadIdx.x;
     const int h = blockIdx.x;
     chosen += (int64_t)h * nsuper;
-    if (stats) stats += 4 * h;
+    if (stats) stats += CS_STATS * h;
     if (st_out) st_out += h;
     const int self_family = 2 * nbr + h;
     int64_t acc[3] = {0, 0, 0};
-    int64_t redone = 0;
+    int64_t redone = 0, adopted_a = 0, adopted_b = 0;   // super-chunk 0 of the first shard has one chain: not counted
     CsState st = st_in;
     if (hyp_mode) st = ckpt[((int64_t)h * nchunks) * (P.segs + 1)];
     int64_t w = 0;
@@ -416,11 +418,13 @@ __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, i
         if (any & 0xffu) {
             const int k = __ffs(any & 0xffu) - 1;
             if (lane == 0) chosen[w] = (uint8_t)k;
+            adopted_a++;
             st = end_a[w * nbr + k];
             for (int q = 0; q < 3; q++) acc[q] += acc_a[(w * nbr + k) * 3 + q];
         } else if (any) {
             const int k = __ffs(any) - 1 - 8;
             if (lane == 0) chosen[w] = (uint8_t)(nbr + k);
+            adopted_b++;
             st = end_b[w * nbr + k];
             for (int q = 0; q < 3; q++) acc[q] += acc_b[(w * nbr + k) * 3 + q];
         } else {
@@ -436,6 +440,8 @@ __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, i
         stats[1] = acc[1];
         stats[2] = acc[2];
         stats[3] = redone;
+        stats[4] = adopted_a;
+        stats[5] = adopted_b;
     }
 }
 
@@ -550,6 +556,12 @@ static int cs_speculate(urh_ctx* ctx, CsRun& R) {
     // enough independent chains to fill the GPU: shrink the chunk for short captures (more warm-up overhead)
     int segs = 16;
     while (segs > 2 && (R.n / (segs * CS_SEG)) * R.P.order < (int64_t)ctx->sm_count * 1024) segs >>= 1;
+    // $URH_B200_COSTAS_SEGS = 2, 4, 8 or 16 forces the chunk layout (tests run every layout on any capture length); the result
+    // does not depend on it
+    if (const char* e = getenv("URH_B200_COSTAS_SEGS")) {
+        const int f = atoi(e);
+        if (f == 2 || f == 4 || f == 8 || f == 16) segs = f;
+    }
     R.P.segs = segs;
     R.P.chunk = segs * CS_SEG;
     R.nchunks = urh_div_up(R.n, R.P.chunk);
@@ -570,7 +582,7 @@ static int cs_speculate(urh_ctx* ctx, CsRun& R) {
     URH_CHECK(urh_arena(ctx, (size_t)R.nsuper, &R.prev_live));
     URH_CHECK(urh_arena(ctx, (size_t)R.nsuper * self_tables, &R.chosen));
     URH_CHECK(urh_arena(ctx, (size_t)R.nchunks, &R.chunk_cnt));
-    URH_CHECK(urh_arena(ctx, (size_t)4 * self_tables, &R.stats));
+    URH_CHECK(urh_arena(ctx, (size_t)CS_STATS * self_tables, &R.stats));
     URH_CHECK(urh_arena(ctx, (size_t)2 * self_tables, &R.st_out));
     R.adopted = 0;
     const dim3 grid((unsigned)urh_div_up(R.nchunks, 128), (unsigned)R.nbr);
@@ -595,10 +607,14 @@ static int cs_finish(urh_ctx* ctx, CsRun& R, float* h_state_out) {
     URH_LAUNCH(ctx, k_cs_assemble, ga, 256, 0, R.cand, R.n, R.T, R.P.segs, chosen, R.out);
     CS_DISPATCH(R, k_cs_fix, (unsigned)min(urh_div_up(R.T.nseg * 32, 128), (int64_t)ctx->sm_count * 16), 128, 0, R.iq, R.n, R.P, R.T, chosen,
                 R.first_shard, R.out);
-    int64_t st4[4];
-    URH_CHECK(urh_read_i64(ctx, R.stats + 4 * R.adopted, 4, st4));
-    for (int i = 0; i < 3; i++) ctx->costas_stats[i] = st4[i];
-    ctx->costas_redone = st4[3];
+    int64_t st6[CS_STATS];
+    URH_CHECK(urh_read_i64(ctx, R.stats + CS_STATS * R.adopted, CS_STATS, st6));
+    for (int i = 0; i < 3; i++) ctx->costas_stats[i] = st6[i];
+    ctx->costas_redone = st6[3];
+    ctx->costas_stitch[0] = st6[4];
+    ctx->costas_stitch[1] = st6[5];
+    ctx->costas_stitch[2] = st6[3];
+    ctx->costas_stitch[3] = R.P.segs;
     if (h_state_out) {
         URH_CUDA(ctx, cudaMemcpyAsync(h_state_out, R.st_out + R.adopted, sizeof(CsState), cudaMemcpyDeviceToHost, ctx->stream));
         URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -700,3 +716,11 @@ extern "C" int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3) {
 
 // super-chunks whose chain the stitch pass had to run itself in the last speculative run (no assumption matched)
 extern "C" int64_t urh_costas_last_redone(urh_ctx* ctx) { return ctx->costas_redone; }
+
+// how the stitch pass of the last PSK demodulation resolved its super-chunks: {adopted from family A, adopted from family B,
+// chained by the stitch warp itself, segs}.  Super-chunk 0 of an unsharded capture (or of the first shard) is not counted: it
+// has one chain only.  The serial kernel reports {0, 0, 0, 0}.
+extern "C" int urh_costas_stitch_stats(urh_ctx* ctx, int64_t* h_out4) {
+    for (int i = 0; i < 4; i++) h_out4[i] = ctx->costas_stitch[i];
+    return URH_OK;
+}

@@ -79,6 +79,43 @@ struct UrhStatAcc {
 };
 
 // ---- IQ sample access ------------------------------------------------------------------------------
+// (a + ib)(c + id) as std::complex<float> multiplies without -ffast-math (GCC): the naive product, and when both of its
+// parts are NaN, libgcc's __mulsc3 recovery of C99 Annex G (an infinite operand gives an infinite result, not NaN).  The
+// Costas loop (signal_functions.pyx:302) reaches the recovery on samples with an infinite imaginary part.
+__device__ __forceinline__ void urh_cmulf(float a, float b, float c, float d, float& re, float& im) {
+    const float ac = __fmul_rn(a, c), bd = __fmul_rn(b, d), ad = __fmul_rn(a, d), bc = __fmul_rn(b, c);
+    re = __fsub_rn(ac, bd);
+    im = __fadd_rn(ad, bc);
+    if (isnan(re) && isnan(im)) {
+        bool recalc = false;
+        if (isinf(a) || isinf(b)) {
+            a = copysignf(isinf(a) ? 1.0f : 0.0f, a);
+            b = copysignf(isinf(b) ? 1.0f : 0.0f, b);
+            if (isnan(c)) c = copysignf(0.0f, c);
+            if (isnan(d)) d = copysignf(0.0f, d);
+            recalc = true;
+        }
+        if (isinf(c) || isinf(d)) {
+            c = copysignf(isinf(c) ? 1.0f : 0.0f, c);
+            d = copysignf(isinf(d) ? 1.0f : 0.0f, d);
+            if (isnan(a)) a = copysignf(0.0f, a);
+            if (isnan(b)) b = copysignf(0.0f, b);
+            recalc = true;
+        }
+        if (!recalc && (isinf(ac) || isinf(bd) || isinf(ad) || isinf(bc))) {
+            if (isnan(a)) a = copysignf(0.0f, a);
+            if (isnan(b)) b = copysignf(0.0f, b);
+            if (isnan(c)) c = copysignf(0.0f, c);
+            if (isnan(d)) d = copysignf(0.0f, d);
+            recalc = true;
+        }
+        if (recalc) {
+            re = __fmul_rn(INFINITY, __fsub_rn(__fmul_rn(a, c), __fmul_rn(b, d)));
+            im = __fmul_rn(INFINITY, __fadd_rn(__fmul_rn(a, d), __fmul_rn(b, c)));
+        }
+    }
+}
+
 template <int DT> struct UrhElem;
 template <> struct UrhElem<URH_DT_I8> { typedef int8_t type; };
 template <> struct UrhElem<URH_DT_U8> { typedef uint8_t type; };
