@@ -168,6 +168,23 @@ int urh_spectrogram_db(urh_ctx* ctx, const float* d_x, int64_t n, int window_siz
  * (max - min))))], colormap = entries x 4 bytes (blue, green, red, alpha); normalize = 0: the data are indices already. */
 int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, int64_t cols, const uint8_t* d_colormap, int entries,
                     float data_min, float data_max, int normalize, uint8_t* d_out);
+/* Spectrogram.create_spectrogram_image / create_image_segments (Spectrogram.py:164-190) in one launch: the BGRA image
+ * apply_bgra_lookup(dB map) of every segment s = d_x[h_seg_start[s] : h_seg_start[s] + h_seg_len[s]] (complex64), each with its own
+ * frame count max(1, (len - W) // hop + 1), zero-padded below W samples, written back to back into d_out: transpose = 0 gives
+ * [W][frames][4] per segment (Spectrogram.create_image(dB)), transpose = 1 gives [frames][W][4] (create_image(flipud(dB.T))).
+ * Bit-identical to urh_spectrogram_db followed by urh_bgra_lookup.  Power-of-two windows 128 .. 4096 with colormaps of up to
+ * 65536 entries take the fused kernel; anything else composes those two stages on the device. */
+int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop, const double* d_window,
+                         const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* d_colormap, int entries,
+                         float data_min, float data_max, int transpose, uint8_t* d_out);
+/* d_out[i] = d_x[start + i * step], i < count (complex64 samples; a Python slice of a capture of n samples, step may be negative) */
+int urh_gather_samples(urh_ctx* ctx, const float* d_x, int64_t n, int64_t start, int64_t step, int64_t count, float* d_out);
+/* Spectrogram.export_to_fta (Spectrogram.py:118-154): rows [row0, row0 + nrows) of the record array [W][frames][reps], packed
+ * records {f8 f, u4 t, f4 a} (include_amplitude, reps = 3) or {f8 f, u4 t} (reps = 2): f = d_freqs[i], t = int(j * time_width),
+ * a = the fftshifted dB map [j][i] (d_db = urh_spectrogram_db's fliplr'ed map).  The caller checks that every t fits a uint32.
+ * h_out != NULL: the band is also copied to that (pinned) host buffer, asynchronously; synchronise before reading it. */
+int urh_fta_records(urh_ctx* ctx, const float* d_db, int64_t frames, int window_size, int64_t row0, int64_t nrows,
+                    const double* d_freqs, double time_width, int include_amplitude, uint8_t* d_out, void* h_out);
 
 /* ---- sharded captures: one contiguous sample range per GPU (digitize.cu, nccl.cu; SURVEY 8e) ----------
  * urh_shard_dense      every rank: demodulate + classify its shard (d_iq[-1] = halo sample when has_halo);

@@ -51,6 +51,9 @@ struct urh_ctx {
     int fft_nfft;
     int64_t fft_batch;
     bool fft_valid;
+    // twiddles of the last window size urh_spectrogram_bgra ran with (spectrogram.cu; 4096 entries allocated)
+    void* img_tw;
+    int img_tw_n;
     // sharded digitizer state between urh_shard_dense and urh_shard_candidates (arena memory)
     void* shard_tiles;
     void* shard_staging;

@@ -98,6 +98,7 @@ extern "C" void urh_ctx_destroy(urh_ctx* ctx) {
     if (ctx->h_mail) cudaFreeHost(ctx->h_mail);
     if (ctx->ts_mem) cudaFree(ctx->ts_mem);
     if (ctx->step_dev) cudaFree(ctx->step_dev);
+    if (ctx->img_tw) cudaFree(ctx->img_tw);
     if (ctx->shard_fin) free(ctx->shard_fin);
     for (int i = 0; i < 2; i++)
         if (ctx->h_stage[i]) cudaFreeHost(ctx->h_stage[i]);

@@ -88,22 +88,98 @@ __device__ __forceinline__ double2 cmul(double2 a, double2 b) {
     return make_double2(fma(a.x, b.x, -a.y * b.y), fma(a.x, b.y, a.y * b.x));
 }
 
-// MODE 0: out = complex128 [F][W] = X / W;  MODE 1: out = float32 [F][W] dB map (fftshift + fliplr + complex64 cast + 10 log10f)
-// W = 2^LOG2W and the thread count are compile-time: every loop below is fully unrolled (the W / THREADS loads of a thread are
-// in flight together — the first version, with run-time W, was bound by the latency of one load after the other — and the index
-// arithmetic of the stages is shifts and masks).
-template <int LOG2W, int THREADS, int MODE>
-__global__ void __launch_bounds__(THREADS) k_stft_fused(const float2* __restrict__ x, int64_t n, int hop,
-                                                       const double* __restrict__ window, const double2* __restrict__ tw,
-                                                       int64_t nframes, void* __restrict__ out_) {
+// ---- MODE 2: the spectrogram image (Spectrogram.create_spectrogram_image / create_image_segments, Spectrogram.py:164-190) -----
+// Each bin takes the dB map's steps (scale, fftshift, complex64 cast, 10 log10f, fliplr), then k_bgra_lookup's (bgra_index), and
+// only the 4-byte colormap entry is written.  One launch covers every frame of every segment of a capture: seg[5 s ..] =
+// {first sample, end sample, frames, first block, first pixel} of segment s; no frame reads at or past its segment's end (the
+// zero-padding of Spectrogram.py:102-103 per segment).  A block owns STFT_IMG_FPB consecutive frames of one segment.
+//   transpose = 0: image [W][F] (row r = dB column r, column f = frame f).  The block keeps its frames' colormap indices in shared
+//                  memory ([W][FPB] uint16) and writes each row's FPB pixels together: 8 frames = 32-byte row segments.  uint16
+//                  rather than the 4-byte entries keeps W = 4096 in shared memory: 139 KB (radix-16 FFT buffers) + 64 KB indices
+//                  + 4 KB colormap = 204 KB of the 227 KB a block may have; 4-byte entries would need 267 KB.  Colormaps of more
+//                  than 65536 entries therefore take the composed path (urh_spectrogram_bgra).
+//   transpose = 1: image [F][W] (np.flipud(dB.T) before the look-up: bins in fftshift order); each frame's row is written as it is
+//                  computed, coalesced.
+// padded shared-memory index of the radix-16 kernel (one element every 16; see k_stft_r16)
+__device__ __forceinline__ int stft_pad(int i) { return i + (i >> 4); }
+constexpr int STFT_IMG_FPB = 8;
+struct StftImage {
+    const int64_t* seg;
+    int nseg;
+    const uint32_t* cmap;
+    int entries;
+    float data_min, range;
+    int transpose;
+};
+
+// Spectrogram.apply_bgra_lookup per value: float32 subtract, divide, multiply, truncate toward zero (astype(int)), np.take(mode="clip");
+// NaN and out-of-range values become INT64_MIN in numpy, which mode="clip" maps to entry 0
+__device__ __forceinline__ int bgra_index(float v, float data_min, float range, float scale, int L, int normalize) {
+    if (normalize) v = __fmul_rn(scale, __fdiv_rn(__fsub_rn(v, data_min), range));
+    long long k = (v == v && fabsf(v) < 9.0e18f) ? (long long)v : LLONG_MIN;
+    k = k < 0 ? 0 : (k > L - 1 ? L - 1 : k);
+    return (int)k;
+}
+
+// fft(base, end) runs one frame's FFT (samples base .. base + W - 1, zeros at and past end) and returns the buffer holding X, the
+// stride of which PAD says (stft_pad or none); `tail` is the shared memory after the FFT buffers
+template <int W, int NT, bool PAD, typename Fft>
+__device__ __forceinline__ void stft_image_block(const StftImage& img, int hop, Fft fft, unsigned char* tail, uint32_t* __restrict__ out) {
+    constexpr int FPB = STFT_IMG_FPB;
+    const int64_t blk = blockIdx.x;
+    int lo = 0, hi = img.nseg - 1;   // the last segment whose first block is <= blk
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (img.seg[5 * mid + 3] <= blk) lo = mid;
+        else hi = mid - 1;
+    }
+    const int64_t* sg = img.seg + 5 * lo;
+    const int64_t start = sg[0], end = sg[1], F = sg[2];
+    const int64_t f0 = (blk - sg[3]) * FPB;
+    const int nf = (int)min((int64_t)FPB, F - f0);
+    uint32_t* o = out + sg[4];
+    uint16_t* s_idx = (uint16_t*)tail;                       // [W][FPB]
+    uint32_t* s_map = (uint32_t*)(tail + W * FPB * sizeof(uint16_t));
+    const bool map_smem = img.entries <= 1024;
+    if (map_smem)
+        for (int i = threadIdx.x; i < img.entries; i += NT) s_map[i] = img.cmap[i];
+    __syncthreads();
+    const uint32_t* map = map_smem ? s_map : img.cmap;
+    const float scale = (float)(img.entries - 1);
+    constexpr int shift = (W + 1) / 2;
+    const double inv = 1.0 / (double)W;
+    for (int k = 0; k < nf; k++) {
+        const double2* a = fft(start + (f0 + k) * hop, end);
+        for (int r = threadIdx.x; r < W; r += NT) {
+            const int j = img.transpose ? W - 1 - r : r;            // dB column (fliplr order)
+            const int src = ((W - 1 - j) + shift) & (W - 1);        // fliplr, then fftshift
+            const double2 v = a[PAD ? stft_pad(src) : src];
+            const float re = (float)(v.x * inv), im = (float)(v.y * inv);
+            const float db = __fmul_rn(10.0f, log10f(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im))));
+            const int idx = bgra_index(db, img.data_min, img.range, scale, img.entries, 1);
+            if (img.transpose) o[(f0 + k) * W + r] = map[idx];
+            else s_idx[r * FPB + k] = (uint16_t)idx;
+        }
+        __syncthreads();   // the next frame's load overwrites the FFT buffers
+    }
+    if (!img.transpose) {
+        for (int t = threadIdx.x; t < W * FPB; t += NT) {
+            const int r = t / FPB, k = t % FPB;
+            if (k < nf) o[(int64_t)r * F + f0 + k] = map[s_idx[t]];
+        }
+    }
+}
+
+// frame at x[base ..], samples at and past n are zeros: window -> Stockham FFT; returns the buffer holding X (natural order)
+template <int LOG2W, int THREADS>
+__device__ __forceinline__ const double2* stft_fused_fft(const float2* __restrict__ x, int64_t n, int64_t base,
+                                                         const double* __restrict__ window, const double2* __restrict__ tw,
+                                                         double2* s_buf) {
     constexpr int W = 1 << LOG2W;
     constexpr int PER = W / THREADS;          // elements per thread in the load / store phases
     constexpr int BPT = (W / 4) / THREADS > 0 ? (W / 4) / THREADS : 1;   // radix-4 butterflies per thread and stage
-    extern __shared__ double2 s_buf[];        // two W-element buffers
     double2* a = s_buf;
     double2* b = s_buf + W;
-    const int64_t f = blockIdx.x;
-    const int64_t base = f * hop;
     {
         float2 sm[PER];
         double g[PER];
@@ -158,6 +234,29 @@ __global__ void __launch_bounds__(THREADS) k_stft_fused(const float2* __restrict
         __syncthreads();
         double2* t = a; a = b; b = t;
     }
+    return a;
+}
+
+// MODE 0: out = complex128 [F][W] = X / W;  MODE 1: out = float32 [F][W] dB map (fftshift + fliplr + complex64 cast + 10 log10f);
+// MODE 2: the image (img, see StftImage)
+// W = 2^LOG2W and the thread count are compile-time: every loop below is fully unrolled (the W / THREADS loads of a thread are
+// in flight together — the first version, with run-time W, was bound by the latency of one load after the other — and the index
+// arithmetic of the stages is shifts and masks).
+template <int LOG2W, int THREADS, int MODE>
+__global__ void __launch_bounds__(THREADS) k_stft_fused(const float2* __restrict__ x, int64_t n, int hop,
+                                                       const double* __restrict__ window, const double2* __restrict__ tw,
+                                                       int64_t nframes, void* __restrict__ out_, StftImage img) {
+    constexpr int W = 1 << LOG2W;
+    constexpr int PER = W / THREADS;
+    extern __shared__ double2 s_buf[];        // two W-element buffers (MODE 2: then the image staging)
+    if (MODE == 2) {
+        stft_image_block<W, THREADS, false>(
+            img, hop, [&](int64_t base, int64_t end) { return stft_fused_fft<LOG2W, THREADS>(x, end, base, window, tw, s_buf); },
+            (unsigned char*)(s_buf + 2 * W), (uint32_t*)out_);
+        return;
+    }
+    const int64_t f = blockIdx.x;
+    const double2* a = stft_fused_fft<LOG2W, THREADS>(x, n, f * hop, window, tw, s_buf);
     const double inv = 1.0 / (double)W;   // W is a power of two: multiplying by 1/W IS the division by W, bit for bit
     if (MODE == 0) {
         double2* out = (double2*)out_ + f * W;
@@ -184,7 +283,6 @@ __global__ void __launch_bounds__(THREADS) k_stft_fused(const float2* __restrict
 // three times (1024 = 16 * 16 * 4) instead of five: the radix-4 kernel above is bound by shared-memory bandwidth.
 // One thread owns 16 points of a pass; W / 16 threads per frame.  Both buffers are padded by one element every 16 (P(i)) so that
 // the stride-16 stores of the first pass do not pile onto the same banks.
-__device__ __forceinline__ int stft_pad(int i) { return i + (i >> 4); }
 __device__ __forceinline__ double2 cadd(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ double2 csub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ double2 cmul_mi(double2 a) { return make_double2(a.y, -a.x); }   // a * (-i)
@@ -213,19 +311,17 @@ __device__ __forceinline__ void dft16(double2 (&v)[16]) {
     for (int r = 0; r < 4; r++) dft4(v[4 * r], v[4 * r + 1], v[4 * r + 2], v[4 * r + 3]);   // v[4 r + s] = y[r + 4 s]
 }
 
-template <int LOG2W, int MODE>
-__global__ void __launch_bounds__((1 << LOG2W) / 16) k_stft_r16(const float2* __restrict__ x, int64_t n, int hop,
-                                                               const double* __restrict__ window, const double2* __restrict__ tw,
-                                                               int64_t nframes, void* __restrict__ out_) {
+// frame at x[base ..], samples at and past n are zeros: window -> radix-16 FFT; returns the (padded) buffer holding X
+template <int LOG2W>
+__device__ __forceinline__ const double2* stft_r16_fft(const float2* __restrict__ x, int64_t n, int64_t base,
+                                                       const double* __restrict__ window, const double2* __restrict__ tw,
+                                                       double2* s_buf) {
     constexpr int W = 1 << LOG2W;
     constexpr int T = W / 16;                 // threads per frame
     constexpr int PADW = W + W / 16;
-    extern __shared__ double2 s_buf[];        // two padded buffers
     double2* a = s_buf;
     double2* b = s_buf + PADW;
     const int tid = threadIdx.x;
-    const int64_t f = blockIdx.x;
-    const int64_t base = f * hop;
     {
         float2 sm[16];
         double g[16];
@@ -282,6 +378,26 @@ __global__ void __launch_bounds__((1 << LOG2W) / 16) k_stft_r16(const float2* __
         __syncthreads();
         double2* t = a; a = b; b = t;
     }
+    return a;
+}
+
+template <int LOG2W, int MODE>
+__global__ void __launch_bounds__((1 << LOG2W) / 16) k_stft_r16(const float2* __restrict__ x, int64_t n, int hop,
+                                                               const double* __restrict__ window, const double2* __restrict__ tw,
+                                                               int64_t nframes, void* __restrict__ out_, StftImage img) {
+    constexpr int W = 1 << LOG2W;
+    constexpr int T = W / 16;                 // threads per frame
+    constexpr int PADW = W + W / 16;
+    extern __shared__ double2 s_buf[];        // two padded buffers (MODE 2: then the image staging)
+    if (MODE == 2) {
+        stft_image_block<W, T, true>(
+            img, hop, [&](int64_t base, int64_t end) { return stft_r16_fft<LOG2W>(x, end, base, window, tw, s_buf); },
+            (unsigned char*)(s_buf + 2 * PADW), (uint32_t*)out_);
+        return;
+    }
+    const int tid = threadIdx.x;
+    const int64_t f = blockIdx.x;
+    const double2* a = stft_r16_fft<LOG2W>(x, n, f * hop, window, tw, s_buf);
     const double inv = 1.0 / (double)W;
     if (MODE == 0) {
         double2* out = (double2*)out_ + f * W;
@@ -313,7 +429,7 @@ static int stft_r16_launch(urh_ctx* ctx, const float* d_x, int64_t n, int hop, c
     if (smem > 48 * 1024)
         URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_r16<LOG2W, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     URH_LAUNCH(ctx, (k_stft_r16<LOG2W, MODE>), (unsigned)num_frames, W / 16, smem, (const float2*)d_x, n, hop, d_window, tw, num_frames,
-               d_out);
+               d_out, StftImage{});
     return URH_OK;
 }
 
@@ -326,7 +442,7 @@ static int stft_fused_launch(urh_ctx* ctx, const float* d_x, int64_t n, int hop,
     if (smem > 48 * 1024)
         URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_fused<LOG2W, THREADS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     URH_LAUNCH(ctx, (k_stft_fused<LOG2W, THREADS, MODE>), (unsigned)num_frames, THREADS, smem, (const float2*)d_x, n, hop, d_window, tw,
-               num_frames, d_out);
+               num_frames, d_out, StftImage{});
     return URH_OK;
 }
 
@@ -413,7 +529,7 @@ extern "C" int urh_spectrogram_db(urh_ctx* ctx, const float* d_x, int64_t n, int
 
 // ---- BGRA colormap look-up (Spectrogram.apply_bgra_lookup, Spectrogram.py:192-206; SURVEY 8f-4) --------------------------------
 // out[c][r] = colormap[clip(int((L - 1) * ((data[r][c] - data_min) / (data_max - data_min))))]   (data.T: the image is transposed)
-// float32 arithmetic in numpy's order: subtract, divide, multiply, truncate toward zero (astype(int)), np.take(mode="clip").
+// float32 arithmetic in numpy's order (bgra_index): subtract, divide, multiply, truncate toward zero (astype(int)), np.take(mode="clip").
 __global__ void k_bgra_lookup(const float* __restrict__ data, int64_t rows, int64_t cols, const uint32_t* __restrict__ colormap, int L,
                               float data_min, float range, int normalize, uint32_t* __restrict__ out) {
     __shared__ uint32_t s_map[1024];
@@ -426,11 +542,7 @@ __global__ void k_bgra_lookup(const float* __restrict__ data, int64_t rows, int6
     const float scale = (float)(L - 1);
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += stride) {
         const int64_t c = idx / rows, r = idx - c * rows;   // output index (c, r) <- data[r][c]
-        float v = data[r * cols + c];
-        if (normalize) v = __fmul_rn(scale, __fdiv_rn(__fsub_rn(v, data_min), range));
-        // astype(int): truncation; NaN and out-of-range values become INT64_MIN in numpy, which mode="clip" maps to entry 0
-        long long k = (v == v && fabsf(v) < 9.0e18f) ? (long long)v : LLONG_MIN;
-        k = k < 0 ? 0 : (k > L - 1 ? L - 1 : k);
+        const int k = bgra_index(data[r * cols + c], data_min, range, scale, L, normalize);
         out[idx] = in_smem ? s_map[k] : colormap[k];
     }
 }
@@ -444,5 +556,207 @@ extern "C" int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, 
     const unsigned grid = (unsigned)min(urh_div_up(rows * cols, 256), (int64_t)ctx->sm_count * 16);
     URH_LAUNCH(ctx, k_bgra_lookup, grid, 256, 0, d_data, rows, cols, (const uint32_t*)d_colormap, entries, data_min, r32, normalize,
                (uint32_t*)d_out);
+    return URH_OK;
+}
+
+// ---- spectrogram images: STFT -> dB -> colormap in one launch (Spectrogram.create_spectrogram_image / create_image_segments) --------
+template <int LOG2W>
+static int stft_image_r16_launch(urh_ctx* ctx, const float* d_x, int hop, const double* d_window, const double2* tw, int64_t blocks,
+                                 const StftImage& img, uint32_t* d_out) {
+    constexpr int W = 1 << LOG2W;
+    const size_t smem = (size_t)2 * (W + W / 16) * sizeof(double2) + (size_t)W * STFT_IMG_FPB * sizeof(uint16_t) + 1024 * sizeof(uint32_t);
+    if (smem > 48 * 1024)
+        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_r16<LOG2W, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    URH_LAUNCH(ctx, (k_stft_r16<LOG2W, 2>), (unsigned)blocks, W / 16, smem, (const float2*)d_x, (int64_t)0, hop, d_window, tw, (int64_t)0,
+               (void*)d_out, img);
+    return URH_OK;
+}
+
+template <int LOG2W>
+static int stft_image_fused_launch(urh_ctx* ctx, const float* d_x, int hop, const double* d_window, const double2* tw, int64_t blocks,
+                                   const StftImage& img, uint32_t* d_out) {
+    constexpr int W = 1 << LOG2W;
+    constexpr int THREADS = (W / 4 >= 256) ? 256 : (W / 4 >= 32 ? W / 4 : 32);
+    const size_t smem = (size_t)2 * W * sizeof(double2) + (size_t)W * STFT_IMG_FPB * sizeof(uint16_t) + 1024 * sizeof(uint32_t);
+    if (smem > 48 * 1024)
+        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_fused<LOG2W, THREADS, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    URH_LAUNCH(ctx, (k_stft_fused<LOG2W, THREADS, 2>), (unsigned)blocks, THREADS, smem, (const float2*)d_x, (int64_t)0, hop, d_window, tw,
+               (int64_t)0, (void*)d_out, img);
+    return URH_OK;
+}
+
+// composed path: one chunk of dB rows (frames f0 .. f0 + nf - 1 of a segment with F frames) through the look-up into its place
+// transpose = 0: out[r][f0 + f] (row pitch F) = lut(db[f][r]);  transpose = 1: out[f0 + f][r] = lut(db[f][W - 1 - r])
+__global__ void k_bgra_place(const float* __restrict__ db, int64_t nf, int W, int64_t F, int64_t f0, const uint32_t* __restrict__ colormap,
+                             int L, float data_min, float range, int transpose, uint32_t* __restrict__ out) {
+    __shared__ uint32_t s_map[1024];
+    const bool in_smem = L <= 1024;
+    if (in_smem)
+        for (int i = threadIdx.x; i < L; i += blockDim.x) s_map[i] = colormap[i];
+    __syncthreads();
+    const int64_t total = nf * W;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const float scale = (float)(L - 1);
+    for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += stride) {
+        int64_t f, r, o;
+        if (transpose) {
+            f = idx / W; r = idx - f * W;
+            o = (f0 + f) * W + r;
+            r = W - 1 - r;
+        } else {
+            r = idx / nf; f = idx - r * nf;
+            o = r * F + f0 + f;
+        }
+        const int k = bgra_index(db[f * W + r], data_min, range, scale, L, 1);
+        out[o] = in_smem ? s_map[k] : colormap[k];
+    }
+}
+
+extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop, const double* d_window,
+                                    const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* d_colormap, int entries,
+                                    float data_min, float data_max, int transpose, uint8_t* d_out) {
+    const int W = window_size;
+    if (W <= 0 || hop <= 0 || nseg <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: bad window/hop/segments");
+    if (entries <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: empty colormap");
+    // per segment {start, end, frames, first block, first pixel}; frames as Spectrogram.stft counts them (short segments: one frame)
+    std::vector<int64_t> seg((size_t)nseg * 5);
+    int64_t blocks = 0, pixels = 0, max_frames = 0;
+    for (int s = 0; s < nseg; s++) {
+        const int64_t st = h_seg_start[s], len = h_seg_len[s];
+        if (st < 0 || len < 0 || st + len > n) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: segment %d outside the capture", s);
+        const int64_t F = len < W ? 1 : (len - W) / hop + 1;
+        int64_t* g = &seg[(size_t)s * 5];
+        g[0] = st; g[1] = st + len; g[2] = F; g[3] = blocks; g[4] = pixels;
+        blocks += urh_div_up(F, STFT_IMG_FPB);
+        pixels += F * W;
+        max_frames = max(max_frames, F);
+    }
+    const float r32 = (float)((double)data_max - (double)data_min);   // as urh_bgra_lookup forms it
+    int log2w = 0;
+    while ((1 << log2w) < W) log2w++;
+    const bool fused = (W & (W - 1)) == 0 && W >= 128 && W <= 4096 && entries <= 65536 && blocks < ((int64_t)1 << 31) &&
+                       !getenv("URH_B200_STFT_CUFFT");
+    if (fused) {
+        if (!ctx->img_tw) URH_CUDA(ctx, cudaMalloc(&ctx->img_tw, (size_t)4096 * sizeof(double2)));
+        if (ctx->img_tw_n != W) {
+            URH_LAUNCH(ctx, k_fft_twiddles, (unsigned)urh_div_up(W, 256), 256, 0, W, (double2*)ctx->img_tw);
+            ctx->img_tw_n = W;
+        }
+        urh_arena_reset(ctx);
+        int64_t* d_seg;
+        URH_CHECK(urh_arena(ctx, seg.size(), &d_seg));
+        URH_CUDA(ctx, cudaMemcpyAsync(d_seg, seg.data(), seg.size() * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
+        const StftImage img{d_seg, nseg, (const uint32_t*)d_colormap, entries, data_min, r32, transpose ? 1 : 0};
+        const double2* tw = (const double2*)ctx->img_tw;
+        uint32_t* out = (uint32_t*)d_out;
+        if (!getenv("URH_B200_STFT_RADIX4")) {
+            if (log2w == 8) return stft_image_r16_launch<8>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            if (log2w == 10) return stft_image_r16_launch<10>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            if (log2w == 12) return stft_image_r16_launch<12>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+        }
+        switch (log2w) {
+            case 7: return stft_image_fused_launch<7>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            case 8: return stft_image_fused_launch<8>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            case 9: return stft_image_fused_launch<9>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            case 10: return stft_image_fused_launch<10>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            case 11: return stft_image_fused_launch<11>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            case 12: return stft_image_fused_launch<12>(ctx, d_x, hop, d_window, tw, blocks, img, out);
+            default: break;
+        }
+        URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: unsupported window size");
+    }
+    // composed: the dB map of up to 256 MiB of frames at a time (stft_run), then its pixels into place
+    const int64_t chunk = min(max_frames, max((int64_t)1, ((int64_t)256 << 20) / ((int64_t)W * 4)));
+    float* db = nullptr;
+    URH_CUDA(ctx, cudaMallocAsync((void**)&db, (size_t)chunk * W * sizeof(float), ctx->stream));
+    int rc = URH_OK;
+    for (int s = 0; s < nseg && rc == URH_OK; s++) {
+        const int64_t* g = &seg[(size_t)s * 5];
+        for (int64_t f0 = 0; f0 < g[2] && rc == URH_OK; f0 += chunk) {
+            const int64_t nf = min(chunk, g[2] - f0), base = g[0] + f0 * hop;
+            rc = stft_run(ctx, d_x + 2 * base, g[1] - base, W, hop, d_window, nf, db, 1);
+            if (rc != URH_OK) break;
+            const unsigned grid = (unsigned)min(urh_div_up(nf * W, 256), (int64_t)ctx->sm_count * 16);
+            k_bgra_place<<<grid, 256, 0, ctx->stream>>>(db, nf, W, g[2], f0, (const uint32_t*)d_colormap, entries, data_min, r32,
+                                                        transpose ? 1 : 0, (uint32_t*)d_out + g[4]);
+            ctx->launches++;
+            const cudaError_t e = cudaGetLastError();
+            if (e != cudaSuccess) {
+                snprintf(ctx->err, sizeof(ctx->err), "spectrogram_bgra: k_bgra_place -> %s", cudaGetErrorString(e));
+                rc = URH_ERR_CUDA;
+            }
+        }
+    }
+    cudaFreeAsync(db, ctx->stream);
+    return rc;
+}
+
+// out[i] = x[start + i * step] (complex64 samples; Python slice semantics, step may be negative)
+__global__ void k_gather_c64(const float2* __restrict__ x, int64_t start, int64_t step, int64_t count, float2* __restrict__ out) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) out[i] = x[start + i * step];
+}
+
+extern "C" int urh_gather_samples(urh_ctx* ctx, const float* d_x, int64_t n, int64_t start, int64_t step, int64_t count, float* d_out) {
+    if (count <= 0) return URH_OK;
+    const int64_t last = start + (count - 1) * step;
+    if (start < 0 || start >= n || last < 0 || last >= n) URH_FAIL(ctx, URH_ERR_INVALID, "gather_samples: index outside the capture");
+    const unsigned grid = (unsigned)min(urh_div_up(count, 256), (int64_t)ctx->sm_count * 16);
+    URH_LAUNCH(ctx, k_gather_c64, grid, 256, 0, (const float2*)d_x, start, step, count, (float2*)d_out);
+    return URH_OK;
+}
+
+// ---- FTA export records (Spectrogram.export_to_fta, Spectrogram.py:118-154) ---------------------------------------------------------
+// The record array is [W][F][reps] of packed records {f8 f, u4 t[, f4 a]} (16 B with the amplitude, reps = 3; 12 B without, reps = 2):
+// record (i, j) = {freqs[i], uint32(int(j * time_width)), dB_shift[j][i]}, each repeated reps times (numpy broadcasts the tuple).
+// dB_shift[j][i] = db[j][W - 1 - i] (db is the fliplr'ed dB map).  A block covers 32 rows (bins) x 32 frames: it reads the dB tile
+// along the bins and writes each row's 32 records, which are contiguous in the output, word by word.
+template <int AMP>
+__global__ void __launch_bounds__(256) k_fta_records(const float* __restrict__ db, int64_t F, int W, int64_t row0, int64_t nrows,
+                                                     const double* __restrict__ freqs, double time_width, uint32_t* __restrict__ out) {
+    constexpr int RW = AMP ? 4 : 3;            // 32-bit words per record
+    constexpr int WPC = RW * (AMP ? 3 : 2);    // words per (i, j) cell
+    __shared__ float s_a[32][33];              // [row][frame]
+    const int64_t j0 = (int64_t)blockIdx.x * 32;
+    const int64_t i0 = row0 + (int64_t)blockIdx.y * 32;
+    if (AMP) {
+        for (int e = threadIdx.x; e < 32 * 32; e += 256) {
+            const int ii = e & 31, jj = e >> 5;
+            const int64_t i = i0 + ii, j = j0 + jj;
+            if (i < row0 + nrows && j < F) s_a[ii][jj] = db[j * W + (W - 1 - i)];
+        }
+        __syncthreads();
+    }
+    for (int e = threadIdx.x; e < 32 * 32 * WPC; e += 256) {
+        const int ii = e / (32 * WPC), rem = e - ii * (32 * WPC);
+        const int jj = rem / WPC, q = (rem - jj * WPC) % RW;
+        const int64_t i = i0 + ii, j = j0 + jj;
+        if (i >= row0 + nrows || j >= F) continue;
+        uint32_t v;
+        if (q < 2) {
+            const unsigned long long fb = (unsigned long long)__double_as_longlong(freqs[i]);
+            v = q == 0 ? (uint32_t)fb : (uint32_t)(fb >> 32);
+        } else if (q == 2) {
+            v = (uint32_t)(long long)__dmul_rn((double)j, time_width);   // int(j * time_width); the host checked the range
+        } else {
+            v = __float_as_uint(s_a[ii][jj]);
+        }
+        out[((i - row0) * F + j) * WPC + (rem - jj * WPC)] = v;
+    }
+}
+
+extern "C" int urh_fta_records(urh_ctx* ctx, const float* d_db, int64_t frames, int window_size, int64_t row0, int64_t nrows,
+                               const double* d_freqs, double time_width, int include_amplitude, uint8_t* d_out, void* h_out) {
+    const int W = window_size;
+    if (W <= 0 || frames <= 0 || row0 < 0 || nrows < 0 || row0 + nrows > W) URH_FAIL(ctx, URH_ERR_INVALID, "fta_records: bad rows");
+    if (nrows == 0) return URH_OK;
+    const dim3 grid((unsigned)urh_div_up(frames, 32), (unsigned)urh_div_up(nrows, 32));
+    if (grid.x >= (1u << 31) || grid.y > 65535) URH_FAIL(ctx, URH_ERR_INVALID, "fta_records: too many frames or rows");
+    if (include_amplitude) URH_LAUNCH(ctx, k_fta_records<1>, grid, 256, 0, d_db, frames, W, row0, nrows, d_freqs, time_width, (uint32_t*)d_out);
+    else URH_LAUNCH(ctx, k_fta_records<0>, grid, 256, 0, d_db, frames, W, row0, nrows, d_freqs, time_width, (uint32_t*)d_out);
+    if (h_out) {
+        const size_t bytes = (size_t)nrows * frames * (include_amplitude ? 48 : 24);
+        URH_CUDA(ctx, cudaMemcpyAsync(h_out, d_out, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+    }
     return URH_OK;
 }

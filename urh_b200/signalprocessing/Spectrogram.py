@@ -1,14 +1,22 @@
 """``Spectrogram`` numerics (reference: src/urh/signalprocessing/Spectrogram.py:94-206).  STFT + dB on the GPU
-(spectrogram.cu: one fused kernel for power-of-two windows, cuFFT for the FFT only otherwise) and the BGRA colormap look-up.
-The QImage wrapping of the reference class is GUI and out of scope."""
+(spectrogram.cu: one fused kernel for power-of-two windows, cuFFT for the FFT only otherwise), the BGRA colormap look-up, the
+spectrogram images (STFT -> dB -> colormap in one launch for every segment of a capture) and the FTA export.
+The QImage wrapping of the reference class is GUI and out of scope (INTEGRATION.md §3 shows the three lines)."""
 import ctypes as C
 import math
 
 import numpy as np
 
 from .. import _lib
-from ..device import DeviceArray, to_device
+from ..device import DeviceArray, PinnedArray, to_device
 from .IQArray import IQArray
+
+# BGRA colormap (entries x 4 uint8: blue, green, red, alpha) of create_spectrogram_image / create_image_segments when the call
+# names none.  The integration sets it from the reference's urh.colormaps.chosen_colormap_numpy_bgra (INTEGRATION.md §3).
+chosen_colormap_numpy_bgra = None
+# bytes of FTA records generated per band in export_to_fta: band b is written to the file while band b + 1 is produced, from two
+# pinned host buffers of this size
+FTA_BAND_BYTES = 64 << 20
 
 
 class Spectrogram(object):
@@ -29,7 +37,10 @@ class Spectrogram(object):
 
     @samples.setter
     def samples(self, value):
-        if isinstance(value, IQArray):
+        if isinstance(value, DeviceArray):
+            if not ((value.dtype == np.complex64 and value.ndim == 1) or (value.dtype == np.float32 and value.ndim == 2 and value.shape[1] == 2)):
+                raise ValueError("device samples must be complex64 (n,) or float32 (n, 2)")
+        elif isinstance(value, IQArray):
             value = value.as_complex64()
         elif isinstance(value, np.ndarray) and value.dtype != np.complex64:
             value = IQArray(value).as_complex64()
@@ -52,21 +63,30 @@ class Spectrogram(object):
     def _num_frames(self, n):
         return max(1, (max(n, self.window_size) - self.window_size) // self.hop_size + 1)
 
-    def _run(self, samples, mode):
-        ctx = _lib.default_context()
+    @staticmethod
+    def _device_samples(samples, ctx):
+        """(device buffer of the complex64 samples, their number); device samples are used in place"""
+        if isinstance(samples, DeviceArray):
+            return samples, len(samples)
         x = np.ascontiguousarray(samples, dtype=np.complex64)
+        return to_device(x.view(np.float32) if len(x) else np.zeros(2, np.float32), ctx), len(x)
+
+    def _window(self, ctx):
+        return to_device(np.ascontiguousarray(self.window_function(int(self.window_size)), dtype=np.float64), ctx)
+
+    def _run(self, samples, mode, keep=False):
+        ctx = _lib.default_context()
+        d_x, n = self._device_samples(samples, ctx)
         W, hop = int(self.window_size), int(self.hop_size)
-        frames = self._num_frames(len(x))
-        window = np.ascontiguousarray(self.window_function(W), dtype=np.float64)
-        d_x = to_device(x.view(np.float32) if len(x) else np.zeros(2, np.float32), ctx)
-        d_w = to_device(window, ctx)
+        frames = self._num_frames(n)
+        d_w = self._window(ctx)
         if mode == 0:
             out = DeviceArray(ctx, (frames, W), np.complex128)
-            ctx.check(ctx.lib.urh_stft(ctx.handle, C.c_void_p(d_x.ptr), len(x), W, hop, C.c_void_p(d_w.ptr), frames, C.c_void_p(out.ptr)))
+            ctx.check(ctx.lib.urh_stft(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr), frames, C.c_void_p(out.ptr)))
         else:
             out = DeviceArray(ctx, (frames, W), np.float32)
-            ctx.check(ctx.lib.urh_spectrogram_db(ctx.handle, C.c_void_p(d_x.ptr), len(x), W, hop, C.c_void_p(d_w.ptr), frames, C.c_void_p(out.ptr)))
-        return out.get()
+            ctx.check(ctx.lib.urh_spectrogram_db(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr), frames, C.c_void_p(out.ptr)))
+        return out if keep else out.get()
 
     def stft(self, samples: np.ndarray):
         """fft(frames * window) / window_size, complex128 [num_frames, window_size] (Spectrogram.py:94-116)"""
@@ -94,3 +114,142 @@ class Spectrogram(object):
                                           float(data_min) if normalize else 0.0, float(data_max) if normalize else 1.0, int(bool(normalize)),
                                           C.c_void_p(out.ptr)))
         return out if on_device else out.get()
+
+    # ---- images (Spectrogram.py:164-190) ---------------------------------------------------------------------------------------
+    @staticmethod
+    def _colormap(colormap):
+        cmap = chosen_colormap_numpy_bgra if colormap is None else colormap
+        if cmap is None:
+            raise ValueError("no colormap: pass one or set Spectrogram.chosen_colormap_numpy_bgra (urh.colormaps.chosen_colormap_numpy_bgra)")
+        cmap = np.ascontiguousarray(cmap, dtype=np.uint8)
+        if cmap.ndim != 2 or cmap.shape[1] != 4 or len(cmap) == 0:
+            raise ValueError("colormap must be entries x 4 bytes (blue, green, red, alpha)")
+        return cmap
+
+    def segment_bounds(self):
+        """[(start, end, frames)] of the slices create_image_segments renders (Spectrogram.py:183-190, the same float arithmetic)"""
+        n = len(self.samples)
+        n_segments = max(1, self.time_bins // self.MAX_LINES_PER_VIEW)
+        step = self.time_bins / n_segments
+        step = max(1, int((step / self.hop_size) * self.hop_size ** 2))
+        return [(i, min(i + step, n), self._num_frames(min(i + step, n) - i)) for i in range(0, n, step)]
+
+    def _images(self, d_x, n, segments, transpose, cmap, ctx):
+        """one device call for all (start, length) segments: the uint8 buffer with the images back to back, and their shapes"""
+        W, hop = int(self.window_size), int(self.hop_size)
+        starts = np.array([s for s, _ in segments], dtype=np.int64)
+        lens = np.array([ln for _, ln in segments], dtype=np.int64)
+        frames = [self._num_frames(int(ln)) for ln in lens]
+        shapes = [((f, W, 4) if transpose else (W, f, 4)) for f in frames]
+        out = DeviceArray(ctx, (sum(frames) * W * 4,), np.uint8)
+        d_map = to_device(cmap, ctx)
+        d_w = self._window(ctx)
+        ctx.check(ctx.lib.urh_spectrogram_bgra(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr),
+                                               starts.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p), len(segments),
+                                               C.c_void_p(d_map.ptr), len(cmap), float(self.data_min), float(self.data_max),
+                                               int(bool(transpose)), C.c_void_p(out.ptr)))
+        return out, shapes
+
+    @staticmethod
+    def _split(out, shapes, on_device):
+        """the images of one buffer: DeviceArray views, or numpy views of one download"""
+        host = None if on_device else out.get()
+        off = 0
+        for shape in shapes:
+            size = shape[0] * shape[1] * 4
+            if on_device:
+                yield DeviceArray(out.ctx, shape, np.uint8, out.ptr + off, base=out)
+            else:
+                yield host[off: off + size].reshape(shape)
+            off += size
+
+    def create_spectrogram_image(self, sample_start: int = None, sample_end: int = None, step: int = None, transpose=False,
+                                 colormap=None):
+        """the uint8 BGRA array [W][frames][4] (transpose: [frames][W][4]) that the reference's create_image wraps in a QImage
+        (Spectrogram.py:164-181) of samples[sample_start:sample_end:step]; a DeviceArray when the samples are on the device"""
+        cmap = self._colormap(colormap)
+        ctx = _lib.default_context()
+        samples = self.samples
+        on_device = isinstance(samples, DeviceArray)
+        if on_device:
+            n = len(samples)
+            start, stop, st = slice(sample_start, sample_end, step).indices(n)
+            count = len(range(start, stop, st))
+            if st == 1:
+                d_x, seg = samples, (start, count)
+            else:   # a strided slice, gathered on the device
+                d_x = DeviceArray(ctx, (max(count, 1), 2), np.float32)
+                ctx.check(ctx.lib.urh_gather_samples(ctx.handle, C.c_void_p(samples.ptr), n, start, st, count, C.c_void_p(d_x.ptr)))
+                n, seg = count, (0, count)
+        else:
+            d_x, n = self._device_samples(samples[sample_start:sample_end:step], ctx)
+            seg = (0, n)
+        out, shapes = self._images(d_x, n, [seg], transpose, cmap, ctx)
+        return next(self._split(out, shapes, on_device))
+
+    def create_image_segments(self, colormap=None):
+        """the images of Spectrogram.py:183-190 (create_spectrogram_image(i, i + step) per segment), all from one device call"""
+        cmap = self._colormap(colormap)
+        bounds = self.segment_bounds()
+        if not bounds:
+            return
+        ctx = _lib.default_context()
+        d_x, n = self._device_samples(self.samples, ctx)   # uploaded once
+        out, shapes = self._images(d_x, n, [(s, e - s) for s, e, _ in bounds], False, cmap, ctx)
+        yield from self._split(out, shapes, isinstance(self.samples, DeviceArray))
+
+    # ---- FTA export (Spectrogram.py:118-154) ------------------------------------------------------------------------------------
+    @staticmethod
+    def fta_dtype(include_amplitude):
+        return np.dtype([("f", np.float64), ("t", np.uint32), ("a", np.float32)] if include_amplitude else [("f", np.float64), ("t", np.uint32)])
+
+    @staticmethod
+    def fta_check_times(frames, time_width, dtype):
+        """raise what the reference's loop raises at its first record whose time int(j * time_width) does not fit a uint32
+        (numpy's OverflowError; int() of NaN / inf raises ValueError / OverflowError itself), before any file is opened"""
+        with np.errstate(invalid="ignore", over="ignore"):
+            p = np.arange(frames, dtype=np.float64) * time_width
+            bad = ~np.isfinite(p) | (p >= 4294967296.0) | (p <= -1.0)
+        if bad.any():
+            j = int(np.argmax(bad))
+            rec = np.empty(1, dtype=dtype)
+            rec[0] = (0.0, int(j * time_width)) + ((0.0,) if len(dtype.names) == 3 else ())
+
+    def export_to_fta(self, sample_rate, filename: str, include_amplitude=False):
+        """Frequency (float64), Time (nanoseconds, uint32)[, Amplitude (float32)] records of every (bin, frame) cell, each repeated 3
+        (2) times, as the reference writes them (Spectrogram.py:118-154).  The records are generated on the device in bands of
+        FTA_BAND_BYTES and written while the next band is produced; the whole array never exists in memory."""
+        W = int(self.window_size)
+        n = len(self.samples)
+        frames = self._num_frames(n)
+        freqs = np.ascontiguousarray(np.fft.fftshift(np.fft.fftfreq(W, 1 / sample_rate)), dtype=np.float64)
+        time_width = 1e9 * ((n / sample_rate) / frames)
+        dtype = self.fta_dtype(include_amplitude)
+        self.fta_check_times(frames, time_width, dtype)
+        reps = 3 if include_amplitude else 2
+        row_bytes = frames * reps * dtype.itemsize
+        rows = max(1, min(W, FTA_BAND_BYTES // row_bytes))
+        bands = [(r0, min(rows, W - r0)) for r0 in range(0, W, rows)]
+        ctx = _lib.default_context()
+        d_db = self._run(self.samples, 1, keep=True)
+        d_f = to_device(freqs, ctx)
+        d_band = DeviceArray(ctx, (rows * row_bytes,), np.uint8)
+        hosts = [PinnedArray(rows * row_bytes, np.uint8, ctx) for _ in range(min(2, len(bands)))]
+
+        def produce(b):
+            r0, nr = bands[b]
+            ctx.check(ctx.lib.urh_fta_records(ctx.handle, C.c_void_p(d_db.ptr), frames, W, r0, nr, C.c_void_p(d_f.ptr), float(time_width),
+                                              int(bool(include_amplitude)), C.c_void_p(d_band.ptr), C.c_void_p(hosts[b % 2].ptr)))
+
+        try:
+            with open(filename, "wb") as fh:
+                produce(0)
+                for b in range(len(bands)):
+                    ctx.sync()   # band b is in hosts[b % 2]; nothing after it is queued yet
+                    if b + 1 < len(bands):
+                        produce(b + 1)
+                    fh.write(hosts[b % 2].array[: bands[b][1] * row_bytes])
+        finally:
+            ctx.sync()
+            for h in hosts:
+                h.free()
