@@ -303,6 +303,10 @@ int urh_timeline_fetch(urh_ctx* ctx, float* h_ms, char* h_names, int names_cap, 
 int urh_last_dense_ms(urh_ctx* ctx, float* ms);
 /* speculative Costas loop diagnostics of the last PSK demodulation: {chunks matched in O(1), chunks walked, samples stepped serially} */
 int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3);
+/* certificate of the last urh_demod_center_digitize(_host) call: {1 if the fine histogram of the demodulation pass decided the
+ * center (no histogram pass over qad) else 0, buckets of that histogram (0: not collected: sharded capture or
+ * $URH_B200_CENTER_NO_CERTIFY), U - L summed over the two deciding bins}.  See DESIGN.md §4.4.1. */
+int urh_center_certify_stats(urh_ctx* ctx, int64_t* h_out3);
 int64_t urh_costas_last_redone(urh_ctx* ctx);
 /* how the stitch pass of the last PSK demodulation resolved its super-chunks: {adopted from family A, adopted from family B,
  * chained by the stitch warp itself, segments per chunk}; super-chunk 0 of an unsharded capture is not counted.  The serial

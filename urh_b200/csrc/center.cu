@@ -410,8 +410,9 @@ __device__ __forceinline__ void hist_flush(HistCache& hc, unsigned int* s_hist, 
 
 // Tiles strictly between win[0] and win[1] lie entirely inside the rank window: every kept sample counts, no rank
 // bookkeeping, no prefix reads.  One warp per tile, grid-stride, eight 512-byte rows in flight per warp.
+// Tiles [t_first, t_end) by blocks blk of nblk (the callers pass the window's interior: win[0] + 1 .. win[1]).
 template <bool SMEM, bool FAST>
-__device__ __forceinline__ void hist_interior_body(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ win,
+__device__ __forceinline__ void hist_interior_body(const float* __restrict__ x, int64_t n, int64_t t_first, int64_t t_end, int blk, int nblk,
                                                    const float* __restrict__ g_fe, float scale, int nbins,
                                                    unsigned long long* __restrict__ hist, int edges_in_smem,
                                                    const int64_t* __restrict__ prefix) {
@@ -429,11 +430,10 @@ __device__ __forceinline__ void hist_interior_body(const float* __restrict__ x, 
     else hb.load(edges_in_smem ? s_fe : g_fe, scale, nbins);
     HistCache hc;
     hc.init();
-    const int64_t t_first = win[0] + 1, t_end = win[1];
-    const int64_t gw = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5), nw = (int64_t)gridDim.x * 8;
+    const int64_t gw = (int64_t)blk * 8 + (threadIdx.x >> 5), nw = (int64_t)nblk * 8;
     const bool vec = (((uintptr_t)x) & 15) == 0;
     const unsigned one = blockDim.x >> 8;   // 1 (256 threads), but not a compile-time constant: see hist_put
-    if (win[0] >= 0) {   // < 0: empty window
+    {
         for (int64_t t = t_first + gw; t < t_end; t += nw) {
             if (prefix[t + 1] == prefix[t]) continue;   // no kept sample in this tile (silence): nothing to count, nothing to read
             const int64_t base = t * URH_TILE;   // interior tiles are full tiles (t < last tile)
@@ -474,14 +474,15 @@ __global__ void __launch_bounds__(256, 4) k_hist_interior(const float* __restric
                                                       const float* __restrict__ g_fe, float scale, int nbins,
                                                       unsigned long long* __restrict__ hist, int edges_in_smem,
                                                       const int64_t* __restrict__ prefix) {
-    hist_interior_body<SMEM, FAST>(x, n, win, g_fe, scale, nbins, hist, edges_in_smem, prefix);
+    const int64_t w0 = win[0];   // < 0: empty window
+    hist_interior_body<SMEM, FAST>(x, n, w0 + 1, w0 >= 0 ? win[1] : 0, blockIdx.x, gridDim.x, g_fe, scale, nbins, hist, edges_in_smem, prefix);
 }
 
 // the window's first and last tile (win[0], win[1]; one block each): rank-exact, straight to the global histogram
 __device__ __forceinline__ void hist_window_ends_body(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
                                                       const int64_t* __restrict__ win, int64_t r0, int64_t r1,
                                                       const float* __restrict__ g_fe, float scale, int nbins,
-                                                      unsigned long long* __restrict__ hist) {
+                                                      unsigned long long* __restrict__ hist, unsigned long long* __restrict__ hist2 = nullptr) {
     __shared__ int s_pre[256];
     const int64_t t = win[blockIdx.x];
     if (t < 0 || (blockIdx.x == 1 && t == win[0])) return;
@@ -493,7 +494,10 @@ __device__ __forceinline__ void hist_window_ends_body(const float* __restrict__ 
     for (int j = 0; j < CEN_PER; j++) {
         const bool kept = v[j] > -4.0f;
         const int k = hb.bin_of<false>(v[j]);
-        if (k >= 0 && rank >= r0 && rank < r1) atomicAdd(&hist[k], 1ull);
+        if (k >= 0 && rank >= r0 && rank < r1) {
+            atomicAdd(&hist[k], 1ull);
+            if (hist2) atomicAdd(&hist2[k], 1ull);
+        }
         rank += kept ? 1 : 0;
     }
 }
@@ -588,7 +592,9 @@ struct __align__(16) CenterPlan {
     int fast;
     int state;                 // 0: no center; 1: center found / histogram to be built; 2: host path must decide
     unsigned int ticket;
-    int pad;
+    int certified;             // 1: k_center_certify decided the center from the fine histogram (no histogram pass over qad)
+    long long straddle;        // U - L of the two deciding bins (k_center_certify)
+    long long pad;
 };
 
 struct ScanKept {
@@ -618,6 +624,8 @@ __global__ void k_center_ranks(const int64_t* __restrict__ counts, int rank, int
     plan->lr0 = a; plan->lr1 = b;
     plan->ticket = 0u;
     plan->state = 1;
+    plan->certified = 0;
+    plan->straddle = 0;
 }
 
 // last tile t with prefix[t] <= r (prefix has ntiles + 1 entries, prefix[ntiles] = kept): the tile holding local rank r
@@ -710,9 +718,11 @@ __global__ void __launch_bounds__(256) k_center_window(const float* __restrict__
 }
 
 // Bin edges and the launch parameters of the histogram from the (rank-ordered) window partials of all shards.
-// parts: world entries (world == 1: &plan->local).  fe: CEN_MAX_BINS + 3 floats; hist: CEN_MAX_BINS counters (zeroed here).
+// parts: world entries (world == 1: &plan->local).  fe: CEN_MAX_BINS + 3 floats; hist, xhist (optional): CEN_MAX_BINS counters
+// (zeroed here).
 __global__ void __launch_bounds__(256) k_center_plan(const CenStats* __restrict__ parts, int world, CenterPlan* __restrict__ plan,
-                                                    float* __restrict__ fe, unsigned long long* __restrict__ hist) {
+                                                    float* __restrict__ fe, unsigned long long* __restrict__ hist,
+                                                    unsigned long long* __restrict__ xhist) {
     __shared__ int s_state;
     __shared__ long long s_nbins;
     __shared__ double s_hmin, s_edge1, s_delta;
@@ -770,7 +780,10 @@ __global__ void __launch_bounds__(256) k_center_plan(const CenStats* __restrict_
             fe[nbins + 1] = __double2float_rd(e);
             fe[nbins + 2] = fmaxf(__double2float_ru(s_hmin), nextafterf(-4.0f, 0.0f));
         }
-        if (k < nbins) hist[k] = 0ull;
+        if (k < nbins) {
+            hist[k] = 0ull;
+            if (xhist) xhist[k] = 0ull;
+        }
     }
 }
 
@@ -778,14 +791,152 @@ template <bool FAST>
 __global__ void __launch_bounds__(256, 3) k_hist_interior_dev(const float* __restrict__ x, int64_t n, const CenterPlan* __restrict__ plan,
                                                           const float* __restrict__ g_fe, unsigned long long* __restrict__ hist,
                                                           const int64_t* __restrict__ prefix) {
-    if (plan->state != 1 || (plan->fast != 0) != FAST) return;
-    hist_interior_body<true, FAST>(x, n, (const int64_t*)plan->win, g_fe, plan->scale, (int)plan->nbins, hist, 1, prefix);
+    if (plan->state != 1 || plan->certified || (plan->fast != 0) != FAST) return;
+    hist_interior_body<true, FAST>(x, n, plan->win[0] + 1, plan->win[1], blockIdx.x, gridDim.x, g_fe, plan->scale, (int)plan->nbins, hist, 1,
+                                   prefix);
 }
+
+// Slabs [*sf, *se) lie wholly among the window's interior tiles (win0, win1): their fine-histogram rows count in full.
+__device__ __forceinline__ void cen_full_slabs(int64_t win0, int64_t win1, int64_t slab_tiles, int64_t* sf, int64_t* se) {
+    *sf = (win0 + slab_tiles) / slab_tiles;   // first slab whose first tile is >= win0 + 1
+    *se = win1 / slab_tiles;                  // slabs below it end at or before win1
+}
+
+// Blocks 0 and 1: the window's first and last tile, rank-exactly, into hist (and xhist).  With a fine histogram (xhist != NULL)
+// blocks 2.. bin the interior tiles of the slabs the window covers only partly into xhist: the exact part of the certificate.
 __global__ void __launch_bounds__(256) k_hist_window_ends_dev(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
                                                              const CenterPlan* __restrict__ plan, const float* __restrict__ g_fe,
-                                                             unsigned long long* __restrict__ hist) {
+                                                             unsigned long long* __restrict__ hist, unsigned long long* __restrict__ xhist,
+                                                             int64_t slab_tiles) {
     if (plan->state != 1) return;
-    hist_window_ends_body(x, n, prefix, (const int64_t*)plan->win, plan->lr0, plan->lr1, g_fe, plan->scale, (int)plan->nbins, hist);
+    if (blockIdx.x < 2) {
+        hist_window_ends_body(x, n, prefix, (const int64_t*)plan->win, plan->lr0, plan->lr1, g_fe, plan->scale, (int)plan->nbins, hist, xhist);
+        return;
+    }
+    const int64_t w0 = plan->win[0], w1 = plan->win[1];
+    int64_t sf, se;
+    cen_full_slabs(w0, w1, slab_tiles, &sf, &se);
+    int64_t a_end = w1, b_begin = w1;   // no full slab: every interior tile is counted exactly
+    if (sf < se) { a_end = sf * slab_tiles; b_begin = se * slab_tiles; }
+    const int blk = blockIdx.x - 2, nblk = gridDim.x - 2, nbins = (int)plan->nbins;
+    const float scale = plan->scale;
+    if (plan->fast) {
+        hist_interior_body<true, true>(x, n, w0 + 1, a_end, blk, nblk, g_fe, scale, nbins, xhist, 1, prefix);
+        hist_interior_body<true, true>(x, n, b_begin, w1, blk, nblk, g_fe, scale, nbins, xhist, 1, prefix);
+    } else {
+        hist_interior_body<true, false>(x, n, w0 + 1, a_end, blk, nblk, g_fe, scale, nbins, xhist, 1, prefix);
+        hist_interior_body<true, false>(x, n, b_begin, w1, blk, nblk, g_fe, scale, nbins, xhist, 1, prefix);
+    }
+}
+
+// left edge of bin k exactly as np.arange forms it (k_center_pick, k_center_certify)
+__device__ __forceinline__ double cen_left_edge(const CenterPlan* plan, int k) {
+    return (k == 0) ? plan->hmin : (k == 1 ? plan->edge1 : __dadd_rn(plan->hmin, __dmul_rn((double)k, plan->delta)));
+}
+
+// ---- the certified peak pick (DESIGN.md §4.4.1) --------------------------------------------------------------------------
+// The window's count in bin k lies in [L_k, U_k]: xhist (exact) plus the fine-histogram buckets of the full slabs that lie wholly
+// inside the bin (L) or touch it (U).  A bucket lies wholly on one side of a float threshold t iff bucket(t) != bucket(pred(t))
+// (the bucket is monotone), so the bounds are exact.  Certified when two bins are peaks for every count vector within the bounds
+// and both exceed every other bin that could be a peak: then k_center_pick would pick exactly these two, whatever the counts.
+// Everything is strict, so numpy's order among equal counts never matters.  Otherwise nothing changes: the histogram pass runs.
+#define CERT_THREADS 512
+__global__ void __launch_bounds__(CERT_THREADS) k_center_certify(const UrhFine fine, CenterPlan* __restrict__ plan, const float* __restrict__ fe,
+                                                                 const unsigned long long* __restrict__ xhist, unsigned long long* __restrict__ lo,
+                                                                 unsigned long long* __restrict__ hi) {
+    __shared__ unsigned long long s_ge[URH_FINE_NB + 1];   // kept window samples of the full slabs in buckets >= b
+    __shared__ unsigned long long s_part[CERT_THREADS];
+    __shared__ unsigned char s_flag[CEN_MAX_BINS];         // 1: certainly a peak, 2: possibly a peak
+    __shared__ unsigned long long s_key[3];
+    __shared__ unsigned int s_certain;
+    if (plan->state != 1) return;
+    const int tid = threadIdx.x;
+    // bucket sums over the full slabs, then suffix sums (per thread, then across threads)
+    constexpr int PER = URH_FINE_NB / CERT_THREADS;
+    int64_t sf, se;
+    cen_full_slabs(plan->win[0], plan->win[1], fine.slab_tiles, &sf, &se);
+    unsigned long long b[PER], tot = 0;
+#pragma unroll
+    for (int j = 0; j < PER; j++) {
+        unsigned long long v = 0;
+        for (int64_t sl = sf; sl < se; sl++) v += fine.gh[sl * URH_FINE_NB + tid * PER + j];
+        b[j] = v;
+        tot += v;
+    }
+    s_part[tid] = tot;
+    if (tid < 3) s_key[tid] = 0ull;
+    if (tid == 0) s_certain = 0u;
+    __syncthreads();
+    for (int off = 1; off < CERT_THREADS; off <<= 1) {
+        const unsigned long long add = (tid + off < CERT_THREADS) ? s_part[tid + off] : 0ull;
+        __syncthreads();
+        s_part[tid] += add;
+        __syncthreads();
+    }
+    unsigned long long run = (tid + 1 < CERT_THREADS) ? s_part[tid + 1] : 0ull;
+#pragma unroll
+    for (int j = PER - 1; j >= 0; j--) {
+        run += b[j];
+        s_ge[tid * PER + j] = run;
+    }
+    if (tid == 0) s_ge[URH_FINE_NB] = 0ull;
+    __syncthreads();
+    // bounds of every bin: bin k = [max(fe[k], f_min), min(fe[k+1], succ(f_hi))) (the last bin: up to succ(f_hi)), as bin_of counts
+    const int nbins = (int)plan->nbins;
+    const float f_hi = fe[nbins + 1], f_min = fe[nbins + 2], top = nextafterf(f_hi, INFINITY);
+    auto ge = [&](float t, unsigned long long& glo, unsigned long long& ghi) {   // bounds of #(kept f >= t)
+        const int bt = urh_fine_bucket(t, fine.scale, fine.off);
+        const bool straddles = urh_fine_bucket(nextafterf(t, -INFINITY), fine.scale, fine.off) == bt;
+        ghi = s_ge[bt];
+        glo = straddles ? s_ge[bt + 1] : s_ge[bt];
+    };
+    for (int k = tid; k < nbins; k += CERT_THREADS) {
+        const float a = fmaxf(fe[k], f_min), e = (k == nbins - 1) ? top : fminf(fe[k + 1], top);
+        unsigned long long l = 0, u = 0;
+        if (a < e) {
+            unsigned long long alo, ahi, elo, ehi;
+            ge(a, alo, ahi);
+            ge(e, elo, ehi);
+            l = alo > ehi ? alo - ehi : 0ull;
+            u = ahi - elo;
+        }
+        lo[k] = xhist[k] + l;
+        hi[k] = xhist[k] + u;
+    }
+    __syncthreads();
+    int window = (int)(0.05 * (double)nbins) + 1;
+    if (window < 2) window = 2;
+    for (int k = tid; k < nbins; k += CERT_THREADS) {
+        const unsigned long long l = lo[k], u = hi[k];
+        bool certain = l > 0ull, possible = u > 0ull;
+        for (int d = -(window - 1); d < window && (certain || possible); d++) {
+            const int j = k + d;
+            if (d == 0 || j < 0 || j >= nbins) continue;
+            certain = certain && l > hi[j];
+            possible = possible && u > lo[j];
+        }
+        s_flag[k] = certain ? 1 : (possible ? 2 : 0);
+        if (certain) atomicAdd(&s_certain, 1u);
+    }
+    __syncthreads();
+    // the two certain peaks with the largest L (key: L, then the lower index), then the largest U of any other possible peak
+    for (int pass = 0; pass < 3; pass++) {
+        const long long p0 = pass > 0 ? (long long)(8191 - (s_key[0] & 8191)) : -1, p1 = pass > 1 ? (long long)(8191 - (s_key[1] & 8191)) : -1;
+        for (int k = tid; k < nbins; k += CERT_THREADS) {
+            if (k == p0 || k == p1) continue;
+            if (pass < 2 && s_flag[k] == 1) atomicMax(&s_key[pass], (lo[k] << 13) | (unsigned long long)(8191 - k));
+            if (pass == 2 && s_flag[k] != 0) atomicMax(&s_key[2], hi[k]);
+        }
+        __syncthreads();
+    }
+    if (tid != 0 || s_certain < 2u) return;
+    const int k1 = 8191 - (int)(s_key[0] & 8191), k2 = 8191 - (int)(s_key[1] & 8191);
+    plan->straddle = (long long)((hi[k1] - lo[k1]) + (hi[k2] - lo[k2]));
+    if (!(lo[k2] > s_key[2])) return;   // lo[k2] <= lo[k1]
+    const double c = __ddiv_rn(__dadd_rn(cen_left_edge(plan, k1), cen_left_edge(plan, k2)), 2.0);
+    plan->center = c;
+    plan->centerf = __double2float_rn(c);
+    plan->certified = 1;
 }
 
 // peak pick (one block).  y = hist[0..nbins)
@@ -793,7 +944,7 @@ __global__ void __launch_bounds__(256) k_center_pick(const unsigned long long* _
     __shared__ unsigned long long s_best[256];
     __shared__ int s_idx[256];
     __shared__ int s_cnt[256];
-    if (plan->state != 1) return;
+    if (plan->state != 1 || plan->certified) return;
     const int nbins = (int)plan->nbins;
     int window = (int)(0.05 * (double)nbins) + 1;
     if (window < 2) window = 2;
@@ -872,10 +1023,9 @@ __global__ void __launch_bounds__(256) k_center_pick(const unsigned long long* _
     if (threadIdx.x != 0) return;
     if (undecided) { plan->state = 2; return; }
     if (found == 0) { plan->state = 0; return; }
-    auto edge = [&](int k) { return (k == 0) ? plan->hmin : (k == 1 ? plan->edge1 : __dadd_rn(plan->hmin, __dmul_rn((double)k, plan->delta))); };
     double c;
-    if (found == 1) c = edge(top_idx[0]);
-    else c = __ddiv_rn(__dadd_rn(edge(top_idx[0]), edge(top_idx[1])), 2.0);
+    if (found == 1) c = cen_left_edge(plan, top_idx[0]);
+    else c = __ddiv_rn(__dadd_rn(cen_left_edge(plan, top_idx[0]), cen_left_edge(plan, top_idx[1])), 2.0);
     plan->center = c;
     plan->centerf = __double2float_rn(c);
     plan->state = 1;
@@ -889,8 +1039,10 @@ extern "C" int urh_nccl_allreduce_i64(urh_ctx* ctx, int64_t* d_buf, int64_t coun
 
 // The chain.  ts = the demodulator's tile table of d_qad (arena); *d_plan_out stays valid until the next arena reset.
 // Enqueues everything on the context stream; no synchronisation.  world > 1: the context's NCCL communicator.
+// fine != NULL (world == 1 only): the demodulator's fine histogram of d_qad; k_center_certify may then decide the center without
+// the histogram pass over qad.
 int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileStats* ts, int64_t max_size, int rank, int world,
-                     CenterPlan** d_plan_out) {
+                     const UrhFine* fine, CenterPlan** d_plan_out) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     int64_t* prefix;
     CenterPlan* plan;
@@ -899,6 +1051,7 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     unsigned long long* hist;
     int64_t* d_counts;
     CenStats* d_parts;
+    unsigned long long *xhist = nullptr, *cert_lo = nullptr, *cert_hi = nullptr;
     const int nb = ctx->sm_count * 2;
     URH_CHECK(urh_arena(ctx, (size_t)ntiles + 1, &prefix));
     URH_CHECK(urh_arena(ctx, 1, &plan));
@@ -907,6 +1060,11 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &hist));
     URH_CHECK(urh_arena(ctx, (size_t)world, &d_counts));
     URH_CHECK(urh_arena(ctx, (size_t)world, &d_parts));
+    if (fine) {
+        URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &xhist));
+        URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &cert_lo));
+        URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &cert_hi));
+    }
     ScanKept fk;
     fk.ts = ts; fk.prefix = prefix;
     URH_CHECK((urhts::scan<int64_t, CenAddI64, ScanKept>(ctx, ntiles, (int64_t)0, CenAddI64(), fk, prefix + ntiles)));
@@ -926,12 +1084,15 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
         URH_TL_MARK(ctx, "x2 window partials: done");
         parts = d_parts;
     }
-    URH_LAUNCH(ctx, k_center_plan, 1, 256, 0, parts, world, plan, fe, hist);
+    URH_LAUNCH(ctx, k_center_plan, 1, 256, 0, parts, world, plan, fe, hist, xhist);
     const size_t dyn = (size_t)CEN_MAX_BINS * 4 + (size_t)(CEN_MAX_BINS + 3) * 4;   // histogram + edge table, 48 KB
     const unsigned gs = (unsigned)min(urh_div_up(ntiles, 8), (int64_t)ctx->sm_count * 8);
+    // the window's cut tiles (and, with a fine histogram, the interior tiles of its cut slabs), then the certificate
+    URH_LAUNCH(ctx, k_hist_window_ends_dev, fine ? 2 + ctx->sm_count * 4 : 2, 256, fine ? dyn : 0, d_qad, n, (const int64_t*)prefix,
+               (const CenterPlan*)plan, (const float*)fe, hist, xhist, fine ? fine->slab_tiles : (int64_t)1);
+    if (fine) URH_LAUNCH(ctx, k_center_certify, 1, CERT_THREADS, 0, *fine, plan, (const float*)fe, (const unsigned long long*)xhist, cert_lo, cert_hi);
     URH_LAUNCH(ctx, (k_hist_interior_dev<true>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
     URH_LAUNCH(ctx, (k_hist_interior_dev<false>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
-    URH_LAUNCH(ctx, k_hist_window_ends_dev, 2, 256, 0, d_qad, n, (const int64_t*)prefix, (const CenterPlan*)plan, (const float*)fe, hist);
     const unsigned long long* hist_all = hist;
     if (world > 1) URH_TL_MARK(ctx, "x3 histogram sum: enter");
     if (world > 1) {
@@ -951,6 +1112,21 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     ctx->center_n = n;
     ctx->center_x = d_qad;
     *d_plan_out = plan;
+    return URH_OK;
+}
+
+// {certified, -, straddle mass} of a plan -> h_dst3 (pinned), on the stream
+int urh_center_plan_certify_stats(urh_ctx* ctx, const CenterPlan* plan, int64_t* h_dst3) {
+    h_dst3[0] = h_dst3[1] = h_dst3[2] = 0;
+    URH_CUDA(ctx, cudaMemcpyAsync(h_dst3, &plan->certified, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync(h_dst3 + 2, &plan->straddle, sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    return URH_OK;
+}
+
+// certificate of the last one-call step: {1 if the fine histogram decided the center (no histogram pass over qad) else 0,
+// buckets of the fine histogram (0: not collected), U - L summed over the two deciding bins}
+extern "C" int urh_center_certify_stats(urh_ctx* ctx, int64_t* h_out3) {
+    for (int i = 0; i < 3; i++) h_out3[i] = ctx->center_cert[i];
     return URH_OK;
 }
 

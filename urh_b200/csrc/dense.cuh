@@ -78,6 +78,56 @@ struct UrhStatAcc {
     }
 };
 
+// ---- fine histogram of the kept samples (one-call detect_center, DESIGN.md §4.4.1) -------------------
+// URH_FINE_NB buckets over a fixed grid per modulation: FSK [-4, 4) (scale 512, offset 2048), ASK [0, 1) (scale 4096, offset 0).
+// bucket(f) = floor(f * scale) + off clamped to [0, NB): exact and monotone in f, so every bucket is an interval of floats.
+// It costs one FFMA rounding toward -inf onto the integer grid of [2^23, 2^24) and two FMNMX (no float-to-int conversion, which
+// runs at a quarter of the FMA rate): the demodulation pass is close to its issue limit, so every instruction per sample counts.
+// Counts go to a per-block shared-memory histogram, flushed per SLAB (slab_tiles consecutive tiles, indexed by tile number).
+#define URH_FINE_NB 4096
+#define URH_FINE_SLABS 64
+struct UrhFine {
+    unsigned int* gh;   // [slabs][URH_FINE_NB]; nullptr: not collected
+    int64_t slab_tiles;
+    float scale, off;
+};
+__device__ __forceinline__ int urh_fine_bucket(float f, float scale, float off) {
+    // scale * f + off + 2^23 rounded down: for results in [2^23, 2^24) (float spacing 1) that is 2^23 + floor(f * scale) + off
+    // exactly (off is an integer); the clamp keeps the result inside that range (NaN never reaches here: not kept)
+    float t = __fmaf_rd(f, scale, off + 8388608.0f);
+    t = fminf(fmaxf(t, 8388608.0f), 8388608.0f + (float)(URH_FINE_NB - 1));
+    return __float_as_int(t) - 0x4B000000;
+}
+// kept (> -4, so never NaN) -> one count in the shared histogram, or straight into the global slab row when the warp's tile lies
+// in another slab than the block's first tile (g != nullptr: only blocks that straddle a slab boundary)
+__device__ __forceinline__ void urh_fine_add(float f, const UrhFine& fn, unsigned int* s, unsigned int* g) {
+    if (f > -4.0f) {
+        const int b = urh_fine_bucket(f, fn.scale, fn.off);
+        if (g) atomicAdd(g + b, 1u);
+        else atomicAdd(s + b, 1u);
+    }
+}
+// the global row of a warp's tile when it differs from the block's (see urh_fine_add)
+__device__ __forceinline__ unsigned int* urh_fine_row(const UrhFine& fn, int64_t tile, int64_t block_tile0) {
+    const int64_t slab = tile / fn.slab_tiles;
+    return (slab == block_tile0 / fn.slab_tiles) ? nullptr : fn.gh + slab * URH_FINE_NB;
+}
+__device__ __forceinline__ void urh_fine_zero(unsigned int* s) {
+    for (int w = threadIdx.x * 4; w < URH_FINE_NB; w += blockDim.x * 4) *(uint4*)(s + w) = make_uint4(0u, 0u, 0u, 0u);
+    __syncthreads();
+}
+__device__ __forceinline__ void urh_fine_flush(const UrhFine& fn, unsigned int* s, int64_t block_tile0) {
+    __syncthreads();
+    unsigned int* g = fn.gh + (block_tile0 / fn.slab_tiles) * URH_FINE_NB;
+    for (int w = threadIdx.x * 4; w < URH_FINE_NB; w += blockDim.x * 4) {
+        const uint4 v = *(const uint4*)(s + w);
+        if (v.x) atomicAdd(g + w, v.x);
+        if (v.y) atomicAdd(g + w + 1, v.y);
+        if (v.z) atomicAdd(g + w + 2, v.z);
+        if (v.w) atomicAdd(g + w + 3, v.w);
+    }
+}
+
 // ---- IQ sample access ------------------------------------------------------------------------------
 // (a + ib)(c + id) as std::complex<float> multiplies without -ffast-math (GCC): the naive product, and when both of its
 // parts are NaN, libgcc's __mulsc3 recovery of C99 Annex G (an infinite operand gives an infinite result, not NaN).  The

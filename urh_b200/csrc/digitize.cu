@@ -18,19 +18,15 @@
 // Dense kernels
 // =====================================================================================================
 
-// IQ source: demodulate (+ optionally write qad, + optionally digitize).
+// One tile of the IQ-source dense pass: demodulate (+ optionally write qad, + optionally digitize).
 template <int DT, int MOD, bool DIGITIZE>
-__global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32)
-k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, int vec_in,
-           int vec_out, const __grid_constant__ UrhClassify cls, int tol, UrhTileSummary* __restrict__ tiles,
-           uint32_t* __restrict__ staging, int stage_cap, int16_t* __restrict__ init_cls, int cls_of_zero,
-           int64_t tile_begin, int64_t tile_count, int has_halo, UrhTileStats* __restrict__ tile_stats) {
+__device__ __forceinline__ void dense_iq_tile(const void* __restrict__ iq, int64_t n, const UrhDemodParams& dp, float* __restrict__ qad_out,
+                                              int vec_in, int vec_out, const UrhClassify& cls, int tol, UrhTileSummary* __restrict__ tiles,
+                                              uint32_t* __restrict__ staging, int stage_cap, int16_t* __restrict__ init_cls, int cls_of_zero,
+                                              int64_t tile, int has_halo, UrhTileStats* __restrict__ tile_stats, const UrhFine& fine,
+                                              unsigned int* s_fine, unsigned int* g_fine) {
     const int lane = threadIdx.x & 31;
-    const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    if (tile_rel >= tile_count) return;
-    const int64_t tile = tile_begin + tile_rel;
     const int64_t tile_start = tile * URH_TILE;
-    if (tile_start >= n) return;
     const int tile_len = (int)((n - tile_start) < URH_TILE ? (n - tile_start) : URH_TILE);
     const int iters = (tile_len + 63) >> 6;
 
@@ -79,6 +75,10 @@ k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
         if (tile_stats) {
             if (v0) { acc.add(s0); acc.all_noise = acc.all_noise && (s0 == dp.noise_value); }
             if (v1) { acc.add(s1); acc.all_noise = acc.all_noise && (s1 == dp.noise_value); }
+            if (s_fine) {
+                if (v0) urh_fine_add(s0, fine, s_fine, g_fine);
+                if (v1) urh_fine_add(s1, fine, s_fine, g_fine);
+            }
         }
         if (qad_out) {
             if (v1 && vec_out) urh_stg_f2(qad_out + pos0, s0, s1);
@@ -98,24 +98,49 @@ k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
     if (DIGITIZE) rt.finish(tile_len, tiles + tile, lane);
 }
 
+// IQ source, one warp per tile; fine.gh: also the fine histogram of the kept samples (dynamic shared memory URH_FINE_NB words).
+template <int DT, int MOD, bool DIGITIZE>
+__global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32)
+k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, int vec_in,
+           int vec_out, const __grid_constant__ UrhClassify cls, int tol, UrhTileSummary* __restrict__ tiles,
+           uint32_t* __restrict__ staging, int stage_cap, int16_t* __restrict__ init_cls, int cls_of_zero,
+           int64_t tile_begin, int64_t tile_count, int has_halo, UrhTileStats* __restrict__ tile_stats, const UrhFine fine) {
+    extern __shared__ unsigned int s_fine[];   // [URH_FINE_NB] when fine.gh
+    const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    const int64_t block_tile0 = tile_begin + (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK;
+    if (fine.gh) urh_fine_zero(s_fine);
+    if (tile_rel < tile_count && (tile_begin + tile_rel) * URH_TILE < n)
+        dense_iq_tile<DT, MOD, DIGITIZE>(iq, n, dp, qad_out, vec_in, vec_out, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero,
+                                    tile_begin + tile_rel, has_halo, tile_stats, fine,
+                                    fine.gh ? s_fine : nullptr, fine.gh ? urh_fine_row(fine, tile_begin + tile_rel, block_tile0) : nullptr);
+    if (fine.gh) urh_fine_flush(fine, s_fine, block_tile0);
+}
+
 // Fast kernel: full, aligned, order-2 FSK tiles [tile_begin, tile_begin + tile_count), tile_begin >= 1
 // (fsk_fast.cuh: float2-paired math, same bits as the generic kernel).
 template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
 __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, URH_FAST_MIN_BLOCKS)
 k_fsk_fast(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
            float cls_noise, int tol, UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
-           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats) {
+           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats, const UrhFine fine) {
+    extern __shared__ unsigned int s_fine[];   // [URH_FINE_NB] when STATS and fine.gh
+    const bool fine_on = STATS && fine.gh;
     const int lane = threadIdx.x & 31;
     const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    if (tile_rel >= tile_count) return;
-    const int64_t tile = tile_begin + tile_rel;
-    UrhRunTracker rt;
-    if (DIGITIZE) rt.init(tol, staging + tile * (int64_t)stage_cap);
-    UrhOne one;
-    one.p = dp.one;
-    one.m = dp.mone;
-    urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
-                                                  STATS ? tile_stats + tile : nullptr, 0u, DIGITIZE ? tiles + tile : nullptr);
+    const int64_t block_tile0 = tile_begin + (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK;
+    if (fine_on) urh_fine_zero(s_fine);
+    if (tile_rel < tile_count) {
+        const int64_t tile = tile_begin + tile_rel;
+        UrhRunTracker rt;
+        if (DIGITIZE) rt.init(tol, staging + tile * (int64_t)stage_cap);
+        UrhOne one;
+        one.p = dp.one;
+        one.m = dp.mone;
+        urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
+                                                      STATS ? tile_stats + tile : nullptr, 0u, DIGITIZE ? tiles + tile : nullptr, fine,
+                                                      fine_on ? s_fine : nullptr, fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr);
+    }
+    if (fine_on) urh_fine_flush(fine, s_fine, block_tile0);
 }
 
 // The same kernel with the input staged through the shared-memory FIFO.
@@ -124,21 +149,28 @@ template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
 __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, (DT == URH_DT_F32) ? 5 : 4)   // (the integer variants spill at 48 registers)
 k_fsk_fifo(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
            float cls_noise, int tol, UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
-           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats) {
+           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats, const UrhFine fine) {
     __shared__ __align__(16) unsigned char s_fifo[URH_WARPS_PER_BLOCK][URH_FSK_FIFO + 1][64 * 2 * sizeof(typename UrhElem<DT>::type)];
+    extern __shared__ unsigned int s_fine[];   // [URH_FINE_NB] when STATS and fine.gh
+    const bool fine_on = STATS && fine.gh;
     const int lane = threadIdx.x & 31;
     const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    if (tile_rel >= tile_count) return;
-    const int64_t tile = tile_begin + tile_rel;
-    UrhRunTracker rt;
-    if (DIGITIZE) rt.init(tol, staging + tile * (int64_t)stage_cap);
-    UrhOne one;
-    one.p = dp.one;
-    one.m = dp.mone;
-    const uint32_t fifo = (uint32_t)__cvta_generic_to_shared(&s_fifo[threadIdx.x >> 5][0][0]);
-    urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS, URH_FSK_FIFO>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
-                                                                        STATS ? tile_stats + tile : nullptr, fifo,
-                                                                        DIGITIZE ? tiles + tile : nullptr);
+    const int64_t block_tile0 = tile_begin + (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK;
+    if (fine_on) urh_fine_zero(s_fine);
+    if (tile_rel < tile_count) {
+        const int64_t tile = tile_begin + tile_rel;
+        UrhRunTracker rt;
+        if (DIGITIZE) rt.init(tol, staging + tile * (int64_t)stage_cap);
+        UrhOne one;
+        one.p = dp.one;
+        one.m = dp.mone;
+        const uint32_t fifo = (uint32_t)__cvta_generic_to_shared(&s_fifo[threadIdx.x >> 5][0][0]);
+        urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS, URH_FSK_FIFO>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
+                                                                    STATS ? tile_stats + tile : nullptr, fifo,
+                                                                    DIGITIZE ? tiles + tile : nullptr, fine, fine_on ? s_fine : nullptr,
+                                                                    fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr);
+    }
+    if (fine_on) urh_fine_flush(fine, s_fine, block_tile0);
 }
 
 // =====================================================================================================
@@ -195,8 +227,10 @@ template <int DT, int MOD, bool DIG>
 static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const UrhDemodParams& dp, float* d_qad,
                              const UrhClassify& cls, int tol, UrhTileSummary* tiles, uint32_t* staging,
                              int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
-                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1) {
+                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
+                             const UrhFine& fine = UrhFine{}) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
+    const size_t fine_smem = fine.gh ? (size_t)URH_FINE_NB * sizeof(unsigned int) : 0;
     if (tile_hi < 0 || tile_hi > ntiles) tile_hi = ntiles;
     const int vec_in = iq_vec_aligned(d_iq, DT) ? 1 : 0;
     const int vec_out = (d_qad && ((uintptr_t)d_qad % 8) == 0) ? 1 : 0;
@@ -206,9 +240,9 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
         end = end > tile_hi ? tile_hi : end;
         const int64_t count = end - begin;
         if (count <= 0) return URH_OK;
-        URH_LAUNCH(ctx, (k_dense_iq<DT, MOD, DIG>), (unsigned)urh_div_up(count, URH_WARPS_PER_BLOCK), threads, 0, d_iq, n, dp,
+        URH_LAUNCH(ctx, (k_dense_iq<DT, MOD, DIG>), (unsigned)urh_div_up(count, URH_WARPS_PER_BLOCK), threads, fine_smem, d_iq, n, dp,
                    d_qad, vec_in, vec_out, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, begin, count, has_halo,
-                   tile_stats);
+                   tile_stats, fine);
         return URH_OK;
     };
     // FSK on aligned buffers with a binary digitizer: tiles 1 .. nfull-1 take the paired fast kernel
@@ -223,20 +257,20 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
             static const bool fifo = getenv("URH_B200_FSK_NO_FIFO") == nullptr;
             const bool ff = fifo;
             if (tile_stats && d_qad && !DIG) {
-                if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                   tiles, staging, stage_cap, fb, fe - fb, tile_stats);
-                else URH_LAUNCH(ctx, (k_fsk_fast<DT, false, true, true>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
-                                tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats);
+                if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
+                                   tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
+                else URH_LAUNCH(ctx, (k_fsk_fast<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
+                                tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
             } else if (d_qad) {
                 if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                   tiles, staging, stage_cap, fb, fe - fb, nullptr);
+                                   tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
                 else URH_LAUNCH(ctx, (k_fsk_fast<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                tiles, staging, stage_cap, fb, fe - fb, nullptr);
+                                tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
             } else {
                 if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                   tiles, staging, stage_cap, fb, fe - fb, nullptr);
+                                   tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
                 else URH_LAUNCH(ctx, (k_fsk_fast<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                tiles, staging, stage_cap, fb, fe - fb, nullptr);
+                                tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
             }
         }
         URH_CHECK(generic(0, 1));
@@ -252,13 +286,14 @@ template <int MOD, bool DIG>
 static int launch_dense_iq_m(urh_ctx* ctx, int dtype, const void* d_iq, int64_t n, const UrhDemodParams& dp,
                              float* d_qad, const UrhClassify& cls, int tol, UrhTileSummary* tiles,
                              uint32_t* staging, int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
-                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1) {
+                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
+                             const UrhFine& fine = UrhFine{}) {
     switch (dtype) {
-        case URH_DT_I8: return launch_dense_iq_t<URH_DT_I8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi);
-        case URH_DT_U8: return launch_dense_iq_t<URH_DT_U8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi);
-        case URH_DT_I16: return launch_dense_iq_t<URH_DT_I16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi);
-        case URH_DT_U16: return launch_dense_iq_t<URH_DT_U16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi);
-        case URH_DT_F32: return launch_dense_iq_t<URH_DT_F32, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi);
+        case URH_DT_I8: return launch_dense_iq_t<URH_DT_I8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
+        case URH_DT_U8: return launch_dense_iq_t<URH_DT_U8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
+        case URH_DT_I16: return launch_dense_iq_t<URH_DT_I16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
+        case URH_DT_U16: return launch_dense_iq_t<URH_DT_U16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
+        case URH_DT_F32: return launch_dense_iq_t<URH_DT_F32, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     }
 }
@@ -512,8 +547,9 @@ extern "C" int urh_shard_dense_qad(urh_ctx* ctx, const float* d_qad, int64_t n, 
 // ---- one-call paths: every stage enqueued on the context stream, ONE synchronisation at the end -----------------------------
 struct CenterPlan;
 int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileStats* ts, int64_t max_size, int rank, int world,
-                     CenterPlan** d_plan_out);   // center.cu
+                     const UrhFine* fine, CenterPlan** d_plan_out);   // center.cu
 int urh_center_plan_result(urh_ctx* ctx, const CenterPlan* plan, const float** d_centerf, const double** d_center, const int** d_state);
+int urh_center_plan_certify_stats(urh_ctx* ctx, const CenterPlan* plan, int64_t* h_dst3);
 
 // Sharded demod + digitize for a KNOWN center (SURVEY 8e): dense pass over this rank's shard, then the tile-level finish with
 // its three 16-byte exchanges on the stream (finish.cu).  d_qad_in != NULL: the shard is already demodulated, digitize from it.
@@ -591,6 +627,19 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     UrhTileStats* ts;
     URH_CHECK(urh_arena(ctx, (size_t)ntiles, &ts));
+    // fine histogram of the kept samples, per slab of tiles: lets detect_center certify its peaks without a histogram pass over qad
+    // (center.cu, k_center_certify).  Not collected for a sharded capture; $URH_B200_CENTER_NO_CERTIFY=1 forces the histogram pass.
+    const bool no_certify = getenv("URH_B200_CENTER_NO_CERTIFY") != nullptr;   // read per call: tests compare both paths
+    UrhFine fine = {};
+    if (!sharded && !no_certify) {
+        fine.slab_tiles = urh_div_up(ntiles, URH_FINE_SLABS);
+        if (fine.slab_tiles < URH_WARPS_PER_BLOCK) fine.slab_tiles = URH_WARPS_PER_BLOCK;   // a block straddles at most one slab edge
+        const int64_t nslabs = urh_div_up(ntiles, fine.slab_tiles);
+        URH_CHECK(urh_arena(ctx, (size_t)(nslabs * URH_FINE_NB), &fine.gh));
+        URH_CUDA(ctx, cudaMemsetAsync(fine.gh, 0, (size_t)(nslabs * URH_FINE_NB) * sizeof(unsigned int), ctx->stream));
+        fine.scale = (mod_type == URH_MOD_FSK) ? 512.0f : 4096.0f;
+        fine.off = (mod_type == URH_MOD_FSK) ? 2048.0f : 0.0f;
+    }
     // h_iq != NULL: the capture is in (pinned) host memory.  It is uploaded in chunks on the copy stream and every chunk is
     // demodulated as soon as it has landed, so the demodulation pass hides behind the PCIe transfer.
     const int64_t chunk_tiles = (h_iq && chunk_samples > 0) ? (chunk_samples >= URH_TILE ? chunk_samples / URH_TILE : 1) : ntiles;
@@ -607,12 +656,13 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
             URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev, 0));
         }
         if (mod_type == URH_MOD_ASK)
-            URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1)));
+            URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1, fine)));
         else
-            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1)));
+            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1, fine)));
     }
     CenterPlan* plan = nullptr;
-    URH_CHECK(urh_center_chain(ctx, d_qad_out, n, ts, max_size, sharded ? ctx->nccl_rank : 0, sharded ? ctx->nccl_world : 1, &plan));
+    URH_CHECK(urh_center_chain(ctx, d_qad_out, n, ts, max_size, sharded ? ctx->nccl_rank : 0, sharded ? ctx->nccl_world : 1,
+                               fine.gh ? &fine : nullptr, &plan));
     const float* d_centerf;
     const double* d_center;
     const int* d_state;
@@ -634,6 +684,7 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
                (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts);
     URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
     int64_t rows = 0;
     if (sharded)
         URH_CHECK(urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, &rows));
@@ -644,6 +695,9 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     int st = 0;
     memcpy(&st, ctx->h_mail + 41, sizeof(int));
     *center_state = st;
+    ctx->center_cert[0] = ctx->h_mail[42];
+    ctx->center_cert[1] = fine.gh ? URH_FINE_NB : 0;
+    ctx->center_cert[2] = ctx->h_mail[44];
     if (st != 1) {
         ctx->pulses_k = 0;
         rows = 0;
