@@ -186,6 +186,25 @@ int urh_gather_samples(urh_ctx* ctx, const float* d_x, int64_t n, int64_t start,
 int urh_fta_records(urh_ctx* ctx, const float* d_db, int64_t frames, int window_size, int64_t row0, int64_t nrows,
                     const double* d_freqs, double time_width, int include_amplitude, uint8_t* d_out, void* h_out);
 
+/* ---- signal views (path_creator.pyx; view.cu) ---------------------------------------------------------------------------------
+ * The source is sample d_src[i * stride], i < n, of dtype URH_DT_*: stride 1 for qad or a 1-D capture, 2 for one column of an
+ * (n, 2) capture (d_src then points at that column's first element).  Both need 0 <= start <= end <= n.
+ *
+ * path_creator.create_path (path_creator.pyx:19-69), spp = samples per pixel > 1: d_values[2k], d_values[2k + 1] = (min, max) of
+ * pixel k = samples [start + k * spp, min(start + (k + 1) * spp, end)), k < ceil((end - start) / spp), in the sample dtype, as the
+ * reference's walk from the pixel's first sample finds them (:50-59): strict < / > only, so the first of equal values wins, later
+ * NaNs are ignored and a NaN first sample is both outputs. */
+int urh_path_minmax(urh_ctx* ctx, const void* d_src, int dtype, int64_t stride, int64_t n, int64_t start, int64_t end, int64_t spp,
+                    void* d_values);
+/* The sub-path loop of create_path (:71-82) and array_to_QPath (:88-120) for every sub-path of one call, in one launch.
+ * h_bounds[2s], h_bounds[2s + 1] = the slice [lo, hi) of sub-path s into x / values, both within [0, L] (L = 2 * pixels when
+ * spp > 1, else end - start).  Sub-path s is written at d_out + h_offsets[s]: the big-endian stream {i4 n, n x {i4 1, f8 x, f8 y},
+ * i4 0, i4 0} with x = x0 + (i >> 1) * spp (or x0 + i when spp <= 1; x0 = start unless d_src holds only the visible range) and y = float64(-value) negated in the sample dtype;
+ * y comes from d_values when spp > 1 and straight from the samples otherwise (d_values may then be NULL).  An empty slice writes
+ * nothing.  h_offsets[count] = total bytes; with d_out = NULL only h_offsets is filled (no launch). */
+int urh_qpath_streams(urh_ctx* ctx, const void* d_src, int dtype, int64_t stride, int64_t n, int64_t start, int64_t end, int64_t spp,
+                      int64_t x0, const void* d_values, const int64_t* h_bounds, int count, uint8_t* d_out, int64_t* h_offsets);
+
 /* ---- sharded captures: one contiguous sample range per GPU (digitize.cu, nccl.cu; SURVEY 8e) ----------
  * urh_shard_dense      every rank: demodulate + classify its shard (d_iq[-1] = halo sample when has_halo);
  *                      h_summary = {last_cls, last_len, whole, init_cls}

@@ -156,6 +156,8 @@ SIGNATURES = {
     "urh_spectrogram_bgra": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, f32, f32, i32, vp]),
     "urh_gather_samples": (i32, [vp, vp, i64, i64, i64, i64, vp]),
     "urh_fta_records": (i32, [vp, vp, i64, i32, i64, i64, vp, C.c_double, i32, vp, vp]),
+    "urh_path_minmax": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, vp]),
+    "urh_qpath_streams": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, i64, vp, vp, i32, vp, vp]),
     "urh_modulate_stats": (i32, [vp, vp]),
     "urh_synth_psk": (i32, [vp, vp, i64, i64, i32, i32, C.c_double, f32, f32, C.c_uint64, i64, i64, i64]),
     "urh_synth_fsk": (i32, [vp, vp, i64, i64, i32, vp, vp, C.c_double, f32, f32, C.c_uint64, i64, i64, i64, i64, i64]),

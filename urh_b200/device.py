@@ -87,6 +87,32 @@ class DeviceArray:
         return self
 
 
+class DeviceColumn:
+    """A read-only 1-D view of column 0 (I) or 1 (Q) of an ``(n, 2)`` DeviceArray, without a copy.
+
+    What URH's scene code touches of its plot data (``len``, ``dtype``) and what ``path_creator.create_path`` reads on the
+    device: element i is ``ptr + i * stride * itemsize``."""
+
+    stride = 2
+    ndim = 1
+
+    def __init__(self, array: DeviceArray, column: int):
+        if array.ndim != 2 or array.shape[1] != 2 or column not in (0, 1):
+            raise ValueError("DeviceColumn needs an (n, 2) DeviceArray and column 0 or 1")
+        self.array = array
+        self.column = column
+        self.ctx = array.ctx
+        self.dtype = array.dtype
+        self.shape = (array.shape[0],)
+        self.ptr = array.ptr + column * array.dtype.itemsize
+
+    def __len__(self):
+        return self.shape[0]
+
+    def get(self) -> np.ndarray:
+        return np.ascontiguousarray(self.array.get()[:, self.column])
+
+
 def to_device(arr, ctx: _lib.Context = None) -> DeviceArray:
     if isinstance(arr, DeviceArray):
         return arr

@@ -12,6 +12,7 @@ _store = {}
 
 CONTINUOUS_BUFFER_SIZE_MB = 50  # settings.py:38
 SPECTRUM_BUFFER_SIZE = 2 ** 15  # settings.py:36
+PIXELS_PER_PATH = 5000  # settings.py:35; path_creator.create_path reads it at call time
 
 
 def read(key: str, default=None, type=None):

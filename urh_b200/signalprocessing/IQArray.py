@@ -122,6 +122,20 @@ class IQArray(object):
             self._device = to_device(np.ascontiguousarray(self.__data))
         return self._device
 
+    @property
+    def real_device(self):
+        """column I of `device()` as a DeviceColumn; unlike `real` it hands out no writable view, so the HBM copy stays cached"""
+        from ..device import DeviceColumn
+
+        return DeviceColumn(self.device(), 0)
+
+    @property
+    def imag_device(self):
+        """column Q of `device()` as a DeviceColumn (see `real_device`)"""
+        from ..device import DeviceColumn
+
+        return DeviceColumn(self.device(), 1)
+
     def own(self):
         """take a private copy of the samples: no outside view can reach them any more, so `device()` may cache again"""
         self.__data = np.array(self.__data, order="C")

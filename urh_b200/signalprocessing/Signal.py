@@ -283,6 +283,17 @@ class Signal(object):
             return np.zeros(0, dtype=np.float32)
 
     @property
+    def real_plot_data_device(self):
+        """`real_plot_data` resident in HBM (a DeviceColumn of `iq_array.device()`) for path_creator.create_path; reading it
+        leaves the IQArray's device copy cached, which `real_plot_data` does not"""
+        return self.iq_array.real_device
+
+    @property
+    def imag_plot_data_device(self):
+        """`imag_plot_data` resident in HBM (see `real_plot_data_device`)"""
+        return self.iq_array.imag_device
+
+    @property
     def changed(self) -> bool:
         return self.__changed
 
