@@ -156,6 +156,18 @@ int urh_convolve_c128(urh_ctx* ctx, const float* d_x, int64_t n, const double* d
 int urh_dc_correction(urh_ctx* ctx, const float* d_iq, int64_t n, float* d_out, int exact_order);
 /* the same for an integer capture: numpy promotes to float64 (exact integer column sums), d_out = double[n][2] */
 int urh_dc_correction_int(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double* d_out);
+/* The filters of one shard of a capture cut by contiguous sample range (urh_b200/dist.py).
+ * urh_fir_filter_shard: fir_filter (signal_functions.pyx:513-525, Filter.apply_fir_filter Filter.py:35-46) of a shard; has_history != 0
+ *   means d_x[-(m-1) .. -1] hold the previous shard's last m-1 samples and y equals urh_fir_filter of the whole capture from d_x[0] on.
+ * urh_dc_column_sums / urh_dc_subtract: Filter.dc_correction (Filter.py:31-33) split into per-shard column sums (h_sums: two host
+ *   doubles, undivided) and the subtraction of the global mean.  exact_order != 0: numpy's serial float32 chain continued from the two
+ *   accumulators h_carry (NULL: 0); otherwise the double sums of urh_dc_correction's reduction.
+ * urh_dc_int_column_sums / urh_dc_int_subtract: the same for an integer capture: exact int64 sums, d_out = double[n][2] = x - mean. */
+int urh_fir_filter_shard(urh_ctx* ctx, const float* d_x, int64_t n, int has_history, const float* d_taps, int m, float* d_y);
+int urh_dc_column_sums(urh_ctx* ctx, const float* d_iq, int64_t n, int exact_order, const float* h_carry, double* h_sums);
+int urh_dc_subtract(urh_ctx* ctx, const float* d_iq, int64_t n, float mean_i, float mean_q, float* d_out);
+int urh_dc_int_column_sums(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int64_t* h_sums);
+int urh_dc_int_subtract(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double mean_i, double mean_q, double* d_out);
 
 /* ---- spectrogram (spectrogram.cu; cuFFT for the FFT only) -------------------------------------------------
  * urh_stft replaces Spectrogram.stft (Spectrogram.py:94-116): complex128 [num_frames][window_size] = fft(frames*window)/W;

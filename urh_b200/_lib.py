@@ -97,6 +97,11 @@ SIGNATURES = {
     "urh_convolve_c128": (i32, [vp, vp, i64, vp, i32, i64, i64, vp]),
     "urh_dc_correction": (i32, [vp, vp, i64, vp, i32]),
     "urh_dc_correction_int": (i32, [vp, vp, i32, i64, vp]),
+    "urh_fir_filter_shard": (i32, [vp, vp, i64, i32, vp, i32, vp]),
+    "urh_dc_column_sums": (i32, [vp, vp, i64, i32, vp, vp]),
+    "urh_dc_subtract": (i32, [vp, vp, i64, f32, f32, vp]),
+    "urh_dc_int_column_sums": (i32, [vp, vp, i32, i64, vp]),
+    "urh_dc_int_subtract": (i32, [vp, vp, i32, i64, C.c_double, C.c_double, vp]),
     "urh_stft": (i32, [vp, vp, i64, i32, i32, vp, i64, vp]),
     "urh_spectrogram_db": (i32, [vp, vp, i64, i32, i32, vp, i64, vp]),
     "urh_shard_dense": (i32, [vp, vp, i32, i64, i32, f32, i32, f32, u16, u8, f32, vp, vp]),

@@ -46,6 +46,8 @@ __device__ __forceinline__ void fir_mbar_wait(uint64_t* bar, uint32_t phase) {
 }
 
 // Exact-order complex64 FIR.  smem: [taps M float2][tile FIR_TILE + M - 1 float2]
+// HISTORY: x[-(m-1) .. -1] hold real samples (the previous shard's tail) and are read instead of the zero initial state.
+template <bool HISTORY>
 __global__ void __launch_bounds__(FIR_THREADS) k_fir_exact(const float2* __restrict__ x, int64_t n, const float2* __restrict__ taps,
                                                             int m, float2* __restrict__ y) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -54,9 +56,9 @@ __global__ void __launch_bounds__(FIR_THREADS) k_fir_exact(const float2* __restr
     float2* s_x = s_taps + ((m + 1) & ~1);  // keep 16-byte alignment of the tile
     const int64_t tile0 = (int64_t)blockIdx.x * FIR_TILE;
     const int64_t first = tile0 - (m - 1);          // first input sample the tile needs (may be < 0)
-    const int64_t lo = first < 0 ? 0 : first;
+    const int64_t lo = (HISTORY || first >= 0) ? first : 0;
     const int64_t hi = min(tile0 + FIR_TILE, n);    // one past the last input sample
-    const int halo_missing = (int)(lo - first);     // zero initial state: samples before the capture are 0
+    const int halo_missing = (int)(lo - first);     // zero initial state: samples before the capture are 0 (none with HISTORY)
     for (int j = threadIdx.x; j < m; j += FIR_THREADS) s_taps[j] = taps[j];
     for (int j = threadIdx.x; j < halo_missing; j += FIR_THREADS) s_x[j] = make_float2(0.f, 0.f);
     // bulk-copy [lo, hi) into s_x + halo_missing: needs 16-byte aligned addresses and size
@@ -111,12 +113,26 @@ extern "C" int urh_fir_filter(urh_ctx* ctx, const float* d_x, int64_t n, const f
     }
     const size_t smem = (size_t)(((m + 1) & ~1) + FIR_TILE + m - 1 + 2) * sizeof(float2);
     if (smem > 200 * 1024) URH_FAIL(ctx, URH_ERR_INVALID, "fir_filter: %d taps exceed the shared-memory tile (max ~11000)", m);
-    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // NOTE on the reference's zero products: for the first m-1 outputs the reference simply has fewer terms; adding
     // the products of zero-padded samples (0*h = +-0) to a non-zero accumulator changes nothing, and the very first
     // term of every output is x[0]*h (k < m) or a real sample, so the sums are bit-identical except for the sign of
     // an all-zero result, which the reference (np.zeros start) also produces as +0 -> handled by starting at +0.
-    URH_LAUNCH(ctx, k_fir_exact, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
+    URH_LAUNCH(ctx, k_fir_exact<false>, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
+               (float2*)d_y);
+    return URH_OK;
+}
+
+// One shard of a capture cut by contiguous sample range: has_history != 0 means d_x[-(m-1) .. -1] hold the previous shard's last
+// m-1 samples, so y equals urh_fir_filter of the whole capture from this shard's first sample on (same products, same order).
+// has_history == 0 is urh_fir_filter itself (the first shard: zero initial state).
+extern "C" int urh_fir_filter_shard(urh_ctx* ctx, const float* d_x, int64_t n, int has_history, const float* d_taps, int m, float* d_y) {
+    if (!has_history || m <= 1) return urh_fir_filter(ctx, d_x, n, d_taps, m, d_y);
+    if (n <= 0) return URH_OK;
+    const size_t smem = (size_t)(((m + 1) & ~1) + FIR_TILE + m - 1 + 2) * sizeof(float2);
+    if (smem > 200 * 1024) URH_FAIL(ctx, URH_ERR_INVALID, "fir_filter_shard: %d taps exceed the shared-memory tile (max ~11000)", m);
+    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    URH_LAUNCH(ctx, k_fir_exact<true>, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
                (float2*)d_y);
     return URH_OK;
 }
@@ -214,10 +230,11 @@ extern "C" int urh_convolve_c128(urh_ctx* ctx, const float* d_x, int64_t n, cons
 // numpy's np.mean over axis 0 of a C-contiguous float32 (n,2) array accumulates each column naively in float32 in
 // row order (SURVEY H9).  exact != 0 reproduces that serial chain (one lane per column, the warp streams the data
 // through shared memory); exact == 0 uses a double reduction (accurate, NOT what the reference computes for large n).
-__global__ void __launch_bounds__(32) k_dc_mean_serial(const float2* __restrict__ x, int64_t n, float* __restrict__ mean) {
+// The serial chain of one warp: lane 0 returns acc + x[0].I + x[1].I + ... (each add rounded), lane 1 the same for Q; lanes 2..31
+// stream the next 1024-row chunk into shared memory meanwhile.
+__device__ __forceinline__ float dc_serial_chain(const float2* __restrict__ x, int64_t n, float acc) {
     __shared__ float2 buf[2][1024];
     const int lane = threadIdx.x;
-    float acc = 0.0f;  // lane 0: I column, lane 1: Q column
     const int64_t nchunks = (n + 1023) / 1024;
     for (int j = lane; j < 1024; j += 32) buf[0][j] = (j < n) ? x[j] : make_float2(0.f, 0.f);
     __syncwarp();
@@ -235,7 +252,19 @@ __global__ void __launch_bounds__(32) k_dc_mean_serial(const float2* __restrict_
         }
         __syncwarp();
     }
-    if (lane < 2) mean[lane] = __fdiv_rn(acc, (float)n);  // np.mean: sum / count in float32
+    return acc;
+}
+
+__global__ void __launch_bounds__(32) k_dc_mean_serial(const float2* __restrict__ x, int64_t n, float* __restrict__ mean) {
+    const float acc = dc_serial_chain(x, n, 0.0f);   // lane 0: I column, lane 1: Q column
+    if (threadIdx.x < 2) mean[threadIdx.x] = __fdiv_rn(acc, (float)n);  // np.mean: sum / count in float32
+}
+
+// the same chain continued from the accumulators (carry0, carry1) of the rows before x, returned undivided
+__global__ void __launch_bounds__(32) k_dc_sum_serial(const float2* __restrict__ x, int64_t n, float carry0, float carry1,
+                                                      double* __restrict__ sums) {
+    const float acc = dc_serial_chain(x, n, threadIdx.x == 0 ? carry0 : carry1);
+    if (threadIdx.x < 2) sums[threadIdx.x] = (double)acc;
 }
 
 __global__ void k_dc_mean_partial(const float2* __restrict__ x, int64_t n, double* __restrict__ part) {
@@ -259,6 +288,13 @@ __global__ void k_dc_mean_fold(const double* __restrict__ part, int nblocks, int
         double s = 0.0;
         for (int b = 0; b < nblocks; b++) s += part[2 * b + threadIdx.x];
         mean[threadIdx.x] = (float)(s / (double)n);
+    }
+}
+__global__ void k_dc_sum_fold(const double* __restrict__ part, int nblocks, double* __restrict__ sums) {
+    if (threadIdx.x < 2) {
+        double s = 0.0;
+        for (int b = 0; b < nblocks; b++) s += part[2 * b + threadIdx.x];
+        sums[threadIdx.x] = s;
     }
 }
 __global__ void k_dc_subtract(const float2* __restrict__ x, int64_t n, const float* __restrict__ mean, float2* __restrict__ y) {
@@ -289,6 +325,47 @@ extern "C" int urh_dc_correction(urh_ctx* ctx, const float* d_iq, int64_t n, flo
     return URH_OK;
 }
 
+// ---- DC correction in two steps, for a capture cut into shards: the column sums of each shard, then the subtraction of the global
+// mean.  exact_order != 0: the serial float32 chain of k_dc_mean_serial continued from h_carry (NULL: from 0), so that shards handed
+// over in row order reproduce urh_dc_correction's chain bit for bit; otherwise the double sums of k_dc_mean_partial / fold (the same
+// grid as urh_dc_correction).  h_sums: two host doubles, not divided by anything.
+extern "C" int urh_dc_column_sums(urh_ctx* ctx, const float* d_iq, int64_t n, int exact_order, const float* h_carry, double* h_sums) {
+    const float c0 = h_carry ? h_carry[0] : 0.0f, c1 = h_carry ? h_carry[1] : 0.0f;
+    if (n <= 0) {
+        h_sums[0] = exact_order ? (double)c0 : 0.0;
+        h_sums[1] = exact_order ? (double)c1 : 0.0;
+        return URH_OK;
+    }
+    urh_arena_reset(ctx);
+    double* sums;
+    URH_CHECK(urh_arena(ctx, 2, &sums));
+    if (exact_order) {
+        URH_LAUNCH(ctx, k_dc_sum_serial, 1, 32, 0, (const float2*)d_iq, n, c0, c1, sums);
+    } else {
+        const int nb = ctx->sm_count * 4;
+        double* part;
+        URH_CHECK(urh_arena(ctx, (size_t)nb * 2, &part));
+        URH_LAUNCH(ctx, k_dc_mean_partial, nb, 256, 0, (const float2*)d_iq, n, part);
+        URH_LAUNCH(ctx, k_dc_sum_fold, 1, 32, 0, part, nb, sums);
+    }
+    URH_CUDA(ctx, cudaMemcpyAsync(h_sums, sums, 2 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+
+// d_out = d_iq - (mean_i, mean_q), every subtraction rounded to float32 (k_dc_subtract)
+extern "C" int urh_dc_subtract(urh_ctx* ctx, const float* d_iq, int64_t n, float mean_i, float mean_q, float* d_out) {
+    if (n <= 0) return URH_OK;
+    urh_arena_reset(ctx);
+    float* mean;
+    URH_CHECK(urh_arena(ctx, 2, &mean));
+    const float h_mean[2] = {mean_i, mean_q};
+    URH_CUDA(ctx, cudaMemcpyAsync(mean, h_mean, sizeof(h_mean), cudaMemcpyHostToDevice, ctx->stream));
+    const unsigned grid = (unsigned)min(urh_div_up(n, 256), (int64_t)ctx->sm_count * 16);
+    URH_LAUNCH(ctx, k_dc_subtract, grid, 256, 0, (const float2*)d_iq, n, (const float*)mean, (float2*)d_out);
+    return URH_OK;
+}
+
 // ---- DC correction of an INTEGER capture: numpy promotes `x - np.mean(x, axis=0)` to float64; the column sums of integers
 // are exact (int64 here, float64 pairwise in numpy: both exact below 2^53), mean = sum / n in double, result double[n][2].
 template <typename T>
@@ -315,6 +392,13 @@ __global__ void k_dc_int_fold(const long long* __restrict__ part, int nblocks, i
         mean[threadIdx.x] = __ddiv_rn((double)s, (double)n);
     }
 }
+__global__ void k_dc_int_sum_fold(const long long* __restrict__ part, int nblocks, long long* __restrict__ sums) {
+    if (threadIdx.x < 2) {
+        long long s = 0;
+        for (int b = 0; b < nblocks; b++) s += part[2 * b + threadIdx.x];
+        sums[threadIdx.x] = s;
+    }
+}
 template <typename T>
 __global__ void k_dc_int_subtract(const T* __restrict__ x, int64_t n, const double* __restrict__ mean, double* __restrict__ y) {
     const double mr = mean[0], mi = mean[1];
@@ -337,6 +421,58 @@ static int dc_int(urh_ctx* ctx, const void* d_iq, int64_t n, double* d_out) {
     const unsigned grid = (unsigned)min(urh_div_up(n, 256), (int64_t)ctx->sm_count * 16);
     URH_LAUNCH(ctx, k_dc_int_subtract<T>, grid, 256, 0, (const T*)d_iq, n, (const double*)mean, d_out);
     return URH_OK;
+}
+
+// Integer captures in two steps: exact int64 column sums of a shard (h_sums: two host int64), then d_out = d_iq - mean in double.
+// Integer sums are exact, so the sums of the shards add up to the whole capture's sums in any order.
+template <typename T>
+static int dc_int_sums(urh_ctx* ctx, const void* d_iq, int64_t n, long long* h_sums) {
+    const int nb = ctx->sm_count * 4;
+    long long* part;
+    long long* sums;
+    URH_CHECK(urh_arena(ctx, (size_t)nb * 2, &part));
+    URH_CHECK(urh_arena(ctx, 2, &sums));
+    URH_LAUNCH(ctx, k_dc_int_partial<T>, nb, 256, 0, (const T*)d_iq, n, part);
+    URH_LAUNCH(ctx, k_dc_int_sum_fold, 1, 32, 0, (const long long*)part, nb, sums);
+    URH_CUDA(ctx, cudaMemcpyAsync(h_sums, sums, 2 * sizeof(long long), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+template <typename T>
+static int dc_int_apply(urh_ctx* ctx, const void* d_iq, int64_t n, double mean_i, double mean_q, double* d_out) {
+    double* mean;
+    URH_CHECK(urh_arena(ctx, 2, &mean));
+    const double h_mean[2] = {mean_i, mean_q};
+    URH_CUDA(ctx, cudaMemcpyAsync(mean, h_mean, sizeof(h_mean), cudaMemcpyHostToDevice, ctx->stream));
+    const unsigned grid = (unsigned)min(urh_div_up(n, 256), (int64_t)ctx->sm_count * 16);
+    URH_LAUNCH(ctx, k_dc_int_subtract<T>, grid, 256, 0, (const T*)d_iq, n, (const double*)mean, d_out);
+    return URH_OK;
+}
+
+extern "C" int urh_dc_int_column_sums(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int64_t* h_sums) {
+    h_sums[0] = h_sums[1] = 0;
+    if (n <= 0) return URH_OK;
+    urh_arena_reset(ctx);
+    long long* out = (long long*)h_sums;
+    switch (dtype) {
+        case URH_DT_I8: return dc_int_sums<int8_t>(ctx, d_iq, n, out);
+        case URH_DT_U8: return dc_int_sums<uint8_t>(ctx, d_iq, n, out);
+        case URH_DT_I16: return dc_int_sums<int16_t>(ctx, d_iq, n, out);
+        case URH_DT_U16: return dc_int_sums<uint16_t>(ctx, d_iq, n, out);
+        default: URH_FAIL(ctx, URH_ERR_DTYPE, "urh_dc_int_column_sums: integer capture expected");
+    }
+}
+
+extern "C" int urh_dc_int_subtract(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double mean_i, double mean_q, double* d_out) {
+    if (n <= 0) return URH_OK;
+    urh_arena_reset(ctx);
+    switch (dtype) {
+        case URH_DT_I8: return dc_int_apply<int8_t>(ctx, d_iq, n, mean_i, mean_q, d_out);
+        case URH_DT_U8: return dc_int_apply<uint8_t>(ctx, d_iq, n, mean_i, mean_q, d_out);
+        case URH_DT_I16: return dc_int_apply<int16_t>(ctx, d_iq, n, mean_i, mean_q, d_out);
+        case URH_DT_U16: return dc_int_apply<uint16_t>(ctx, d_iq, n, mean_i, mean_q, d_out);
+        default: URH_FAIL(ctx, URH_ERR_DTYPE, "urh_dc_int_subtract: integer capture expected");
+    }
 }
 
 extern "C" int urh_dc_correction_int(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double* d_out) {

@@ -14,12 +14,13 @@ Protocol of the sharded digitizer (exactness argument in DESIGN.md §6):
   4. gather the candidate tables on rank 0 (NCCL send/recv), which finishes exactly like the single-GPU path.
 """
 import ctypes as C
+import math
 import os
 
 import numpy as np
 
 from . import _lib
-from .device import DeviceArray
+from .device import DeviceArray, to_device
 
 
 # ---- pure host logic (unit-tested on CPU with gloo, tests/test_dist_cpu.py) -----------------------------------------
@@ -115,19 +116,26 @@ def init_p2p(ctx: _lib.Context, hx: HostExchange):
 
 
 class ShardBuffer(object):
-    """Device buffer [pad][halo][shard samples...]: the shard starts 256-byte aligned (full-line warp loads), the halo
-    sample sits right before it."""
+    """Device buffer [pad][halo][shard samples...][right]: the shard starts 256-byte aligned (full-line warp loads), the halo
+    samples sit right before it, the optional right halo (the next shard's first samples) right after it."""
 
-    def __init__(self, ctx, n_local, dtype=np.float32, halo=1):
+    def __init__(self, ctx, n_local, dtype=np.float32, halo=1, right=0):
         self.ctx = ctx
         self.n = int(n_local)
         self.dtype = np.dtype(dtype)
         self.halo_len = int(halo)
+        self.right_len = int(right)
         unit = 256 // (2 * self.dtype.itemsize)  # samples per 256 bytes
         self.pad = ((self.halo_len + unit - 1) // unit) * unit  # samples before the shard (keeps 256 B alignment)
-        self.buf = DeviceArray(ctx, (self.n + self.pad, 2), self.dtype)
-        self.shard = self.buf[self.pad:]
+        self.buf = DeviceArray(ctx, (self.n + self.pad + self.right_len, 2), self.dtype)
+        self.shard = self.buf[self.pad: self.pad + self.n]
         self.halo = self.buf[self.pad - self.halo_len: self.pad]
+        self.right = self.buf[self.pad + self.n: self.pad + self.n + self.right_len]
+
+    def window(self, left, right):
+        """the shard with `left` samples before it and `right` after it: [g0 - left, g1 + right) of the capture"""
+        assert 0 <= left <= self.halo_len and 0 <= right <= self.right_len
+        return self.buf[self.pad - left: self.pad + self.n + right]
 
 
 def exchange_halo(ctx, hx, sb: ShardBuffer):
@@ -653,3 +661,324 @@ def estimate_sharded(ctx, hx, sb: ShardBuffer, bounds, n_total, noise=None, modu
         tolerance = max(1, int(0.05 * bit_length))
     return {"modulation_type": "ASK" if modulation == "OOK" else modulation, "bit_length": bit_length, "center": center,
             "tolerance": int(tolerance), "noise": noise}
+
+
+# ---- filters and spectrogram over shards (DESIGN.md §6, "Filters and spectrogram over shards") -----------------------------------------
+# Every band-pass / FIR output and every spectrogram frame depends on its own input window only, with a fixed accumulation order, so a
+# rank that holds that window (its shard plus halos copied from its neighbours) computes the single-GPU words bit for bit.  The plans
+# are pure host logic, computed identically on every rank from `bounds`; they raise ValueError before any collective, so every rank
+# raises alike and none is left waiting inside NCCL.
+def _check_bounds(bounds):
+    bounds = [(int(a), int(b)) for a, b in bounds]
+    if not bounds or bounds[0][0] != 0 or any(b <= a for a, b in bounds) or any(bounds[q][1] != bounds[q + 1][0] for q in range(len(bounds) - 1)):
+        raise ValueError("bounds must cut the capture into contiguous, non-empty shards starting at sample 0")
+    return bounds
+
+
+def _check_halos(bounds, halos, what):
+    """halos[r] = (left, right): rank r - 1 supplies `left` samples and rank r + 1 `right` samples, from their own shards only"""
+    last = len(bounds) - 1
+    for r, (left, right) in enumerate(halos):
+        if left and (r == 0 or bounds[r - 1][1] - bounds[r - 1][0] < left):
+            raise ValueError("%s: shard %d (%d samples) is shorter than the %d-sample halo shard %d needs"
+                             % (what, r - 1, bounds[r - 1][1] - bounds[r - 1][0] if r else 0, left, r))
+        if right and (r == last or bounds[r + 1][1] - bounds[r + 1][0] < right):
+            raise ValueError("%s: shard %d (%d samples) is shorter than the %d-sample halo shard %d needs"
+                             % (what, r + 1, bounds[r + 1][1] - bounds[r + 1][0] if r < last else 0, right, r))
+
+
+def bandpass_plan(n_total, m, bounds):
+    """Filter.apply_bandpass_filter of an m-tap filter over a capture cut at `bounds` -> [(L, R, offset)] per rank: rank r convolves the
+    window x[g0 - L, g1 + R) with urh_convolve_c128 at `offset` for g1 - g0 outputs.  Both of the reference's branches (np.convolve
+    'same' and the centred FFT crop) give full_convolution[(m - 1) // 2 + k], k < N, for a filter no longer than the capture (odd on
+    the FFT branch); the inputs where the single-GPU function changes the length or returns nothing raise ValueError."""
+    bounds = _check_bounds(bounds)
+    n_total, m = int(n_total), int(m)
+    if n_total != bounds[-1][1]:
+        raise ValueError("bounds do not cover the %d-sample capture" % n_total)
+    if m < 1:
+        raise ValueError("band-pass: empty filter")
+    if n_total < m:
+        raise ValueError("band-pass: the capture (%d samples) is shorter than the %d-tap filter: np.convolve(..., 'same') returns %d samples"
+                         % (n_total, m, m))
+    if not m < 8 * math.log(math.sqrt(n_total)):   # Filter.apply_bandpass_filter's branch rule: the FFT convolution
+        if m <= 2:
+            raise ValueError("band-pass: the FFT convolution of a %d-tap filter returns an empty array" % m)
+        if m % 2 == 0:
+            raise ValueError("band-pass: the FFT convolution of an even %d-tap filter returns %d samples" % (m, n_total + 1))
+    half = (m - 1) // 2
+    last = len(bounds) - 1
+    plan = []
+    for r in range(len(bounds)):
+        left = 0 if r == 0 else m - 1 - half
+        right = 0 if r == last else half
+        plan.append((left, right, left + half))
+    _check_halos(bounds, [(left, right) for left, right, _ in plan], "band-pass")
+    return plan
+
+
+def fir_plan(n_total, m, bounds):
+    """Filter.apply_fir_filter (causal fir_filter) over a capture cut at `bounds` -> the history length per rank: rank r > 0 reads the
+    previous shard's last m - 1 samples instead of the zero initial state (urh_fir_filter_shard)."""
+    bounds = _check_bounds(bounds)
+    if int(n_total) != bounds[-1][1]:
+        raise ValueError("bounds do not cover the %d-sample capture" % n_total)
+    hist = [0 if r == 0 else max(0, int(m) - 1) for r in range(len(bounds))]
+    _check_halos(bounds, [(h, 0) for h in hist], "FIR")
+    return hist
+
+
+def frame_plan(n_total, window_size, hop, bounds):
+    """Spectrogram frames over a capture cut at `bounds` -> [(first_frame, frames, R)] per rank.  Frame f (of Spectrogram._num_frames)
+    belongs to the rank holding sample f * hop; R is what that rank's last frame reads past its shard (from the next one)."""
+    bounds = _check_bounds(bounds)
+    n_total, W, hop = int(n_total), int(window_size), int(hop)
+    if n_total != bounds[-1][1]:
+        raise ValueError("bounds do not cover the %d-sample capture" % n_total)
+    if W <= 0 or hop <= 0:
+        raise ValueError("spectrogram: bad window size %d / hop %d" % (W, hop))
+    frames = max(1, (max(n_total, W) - W) // hop + 1)
+    plan = []
+    for g0, g1 in bounds:
+        f0 = -(-g0 // hop)
+        f1 = min(frames, -(-g1 // hop))
+        nf = max(0, f1 - f0)
+        right = max(0, min(n_total, (f1 - 1) * hop + W) - g1) if nf else 0
+        plan.append((f0, nf, right))
+    _check_halos(bounds, [(0, right) for _, _, right in plan], "spectrogram")
+    return plan
+
+
+def segment_plan(n_total, window_size, hop, bounds, max_lines=None):
+    """The image segments of Spectrogram.create_image_segments over a capture cut at `bounds` -> (segments, owned, rights):
+    segments = Spectrogram.segment_bounds of the whole capture, owned[r] = indices of the segments that start in shard r (their tail
+    comes from the next shard), rights[r] = how far the last of them reaches past shard r."""
+    from .signalprocessing.Spectrogram import Spectrogram
+
+    bounds = _check_bounds(bounds)
+    n_total = int(n_total)
+    if n_total != bounds[-1][1]:
+        raise ValueError("bounds do not cover the %d-sample capture" % n_total)
+    if int(window_size) <= 0 or int(hop) <= 0:
+        raise ValueError("spectrogram: bad window size %d / hop %d" % (window_size, hop))
+    segments = Spectrogram.segment_bounds_of(n_total, int(window_size), int(hop),
+                                             Spectrogram.MAX_LINES_PER_VIEW if max_lines is None else int(max_lines))
+    owned = [[i for i, (s, _, _) in enumerate(segments) if g0 <= s < g1] for g0, g1 in bounds]
+    rights = [max([0] + [segments[i][1] - g1 for i in mine]) for mine, (_, g1) in zip(owned, bounds)]
+    _check_halos(bounds, [(0, right) for right in rights], "spectrogram images")
+    return segments, owned, rights
+
+
+def dc_exact_handover(rank, world, chain, allgather):
+    """The serial float32 column sums of a capture sharded over the ranks: rank r continues the chain from the two accumulators rank
+    r - 1 ended with (``chain(carry) -> float32[2]``), in rank order; ``allgather(float32[2]) -> [world, 2]``.  Every rank returns the
+    sums of the whole capture, bit for bit numpy's serial chain."""
+    carry = np.zeros(2, dtype=np.float32)
+    for turn in range(world):
+        mine = np.asarray(chain(carry), dtype=np.float32) if turn == rank else np.zeros(2, dtype=np.float32)
+        carry = np.asarray(allgather(mine), dtype=np.float32).reshape(world, 2)[turn].copy()
+    return carry
+
+
+def dc_fold_double(parts, n_total):
+    """float32 mean from per-rank double column sums [world, 2], added in rank order (the double regime of the DC correction)"""
+    s = np.zeros(2, dtype=np.float64)
+    for q in range(len(parts)):
+        s = s + np.asarray(parts[q], dtype=np.float64)
+    return (s / float(n_total)).astype(np.float32)
+
+
+def exchange_halos(ctx, hx, sb: ShardBuffer, halos=None):
+    """Rank r receives halos[r][0] samples of rank r - 1's tail into the samples right before its shard and halos[r][1] of rank r + 1's
+    head right after it: two grouped NCCL send/recv on the context stream, device to device.  ``halos``: [(left, right)] per rank, the
+    same on every rank (by default every rank's (halo_len, right_len))."""
+    rank, world = hx.rank, hx.world
+    if halos is None:
+        halos = hx.allgather((sb.halo_len, sb.right_len))
+    left = int(halos[rank][0]) if rank > 0 else 0
+    right = int(halos[rank][1]) if rank < world - 1 else 0
+    to_next = int(halos[rank + 1][0]) if rank + 1 < world else 0    # my tail -> rank + 1
+    to_prev = int(halos[rank - 1][1]) if rank > 0 else 0            # my head -> rank - 1
+    assert left <= sb.halo_len and right <= sb.right_len and to_next <= sb.n and to_prev <= sb.n
+    item = 2 * sb.dtype.itemsize
+    lib = ctx.lib
+    if to_next or left:
+        ctx.check(lib.urh_nccl_sendrecv(ctx.handle, C.c_void_p(sb.shard.ptr + (sb.n - to_next) * item), to_next * item, rank + 1 if to_next else -1,
+                                        C.c_void_p(sb.shard.ptr - left * item), left * item, rank - 1 if left else -1))
+    if to_prev or right:
+        ctx.check(lib.urh_nccl_sendrecv(ctx.handle, C.c_void_p(sb.shard.ptr), to_prev * item, rank - 1 if to_prev else -1,
+                                        C.c_void_p(sb.right.ptr), right * item, rank + 1 if right else -1))
+
+
+def _with_room(ctx, sb: ShardBuffer, left, right):
+    """`sb` if it has room for the halos, else a copy of its shard in a buffer that has"""
+    if sb.halo_len >= left and sb.right_len >= right:
+        return sb
+    out = ShardBuffer(ctx, sb.n, sb.dtype, halo=max(left, sb.halo_len), right=max(right, sb.right_len))
+    ctx.check(ctx.lib.urh_memcpy_d2d(ctx.handle, C.c_void_p(out.shard.ptr), C.c_void_p(sb.shard.ptr), sb.shard.nbytes))
+    return out
+
+
+def _output_halos(ctx, bounds, world, out_halo):
+    """the left halo of a filtered shard buffer: what the sharded demodulators read before the shard (default: the Costas warm-up)"""
+    h = costas_halo(ctx) if out_halo is None else int(out_halo)
+    halos = [(h if r else 0, 0) for r in range(world)]
+    _check_halos(bounds, halos, "filter output")
+    return h, halos
+
+
+def _float_shard(sb, what):
+    if sb.dtype != np.float32:
+        raise ValueError("%s: the shards must be complex64 samples (float32 (n, 2))" % what)
+
+
+def apply_bandpass_filter_sharded(ctx, hx, sb: ShardBuffer, bounds, f_low, f_high, filter_bw=0.08, out_halo=None) -> ShardBuffer:
+    """Filter.apply_bandpass_filter (Filter.py:84-101) of a capture sharded over the ranks, bit for bit the single-GPU result.  Rank r
+    receives the filter-length halos from its neighbours (``bandpass_plan``) and convolves its window; the output comes back as a
+    ShardBuffer whose left halo already holds the previous shard's filtered tail, so demod_center_digitize_distributed /
+    afp_demod_psk_sharded take it directly."""
+    from .signalprocessing.Filter import Filter
+
+    bounds = _check_bounds(bounds)
+    rank, world = hx.rank, hx.world
+    _float_shard(sb, "band-pass")
+    h = np.ascontiguousarray(Filter.bandpass_taps(f_low, f_high, filter_bw), dtype=np.complex128)
+    plan = bandpass_plan(bounds[-1][1], len(h), bounds)
+    out_h, out_halos = _output_halos(ctx, bounds, world, out_halo)
+    left, right, offset = plan[rank]
+    src = _with_room(ctx, sb, left, right)
+    exchange_halos(ctx, hx, src, [(a, b) for a, b, _ in plan])
+    win = src.window(left, right)
+    d_t = to_device(h.view(np.float64), ctx)
+    out = ShardBuffer(ctx, sb.n, np.float32, halo=out_h)
+    ctx.check(ctx.lib.urh_convolve_c128(ctx.handle, C.c_void_p(win.ptr), len(win), C.c_void_p(d_t.ptr), len(h), int(offset), sb.n,
+                                        C.c_void_p(out.shard.ptr)))
+    exchange_halos(ctx, hx, out, out_halos)
+    ctx.sync()
+    return out
+
+
+def fir_filter_sharded(ctx, hx, sb: ShardBuffer, bounds, taps, out_halo=None) -> ShardBuffer:
+    """Filter.apply_fir_filter (fir_filter, signal_functions.pyx:513-525) of a capture sharded over the ranks: rank r > 0 filters its
+    shard with the previous shard's last m - 1 samples as history (urh_fir_filter_shard), bit for bit the single-GPU result."""
+    bounds = _check_bounds(bounds)
+    rank, world = hx.rank, hx.world
+    _float_shard(sb, "FIR")
+    taps = np.ascontiguousarray(np.asarray(taps, dtype=np.complex64))
+    hist = fir_plan(bounds[-1][1], len(taps), bounds)
+    out_h, out_halos = _output_halos(ctx, bounds, world, out_halo)
+    src = _with_room(ctx, sb, hist[rank], 0)
+    exchange_halos(ctx, hx, src, [(a, 0) for a in hist])
+    d_t = to_device(taps.view(np.float32) if len(taps) else np.zeros(2, np.float32), ctx)
+    out = ShardBuffer(ctx, sb.n, np.float32, halo=out_h)
+    ctx.check(ctx.lib.urh_fir_filter_shard(ctx.handle, C.c_void_p(src.shard.ptr), sb.n, int(hist[rank] > 0), C.c_void_p(d_t.ptr), len(taps),
+                                           C.c_void_p(out.shard.ptr)))
+    exchange_halos(ctx, hx, out, out_halos)
+    ctx.sync()
+    return out
+
+
+def dc_correction_sharded(ctx, hx, sb: ShardBuffer, bounds, out_halo=None) -> ShardBuffer:
+    """Filter.dc_correction (Filter.py:31-33) of a capture sharded over the ranks.
+      float32, N <= Filter.EXACT_DC_MAX: numpy's serial float32 column chain handed from rank to rank (``dc_exact_handover``), then
+                 sum / N in float32 on every rank: bit for bit the single-GPU result;
+      float32, larger N: per-rank double column sums, all-gathered and added in rank order (``dc_fold_double``), mean = float32(sum / N);
+      integer captures: exact int64 column sums added over the ranks, mean = sum / N in double; a float64 result, bit for bit."""
+    from .signalprocessing.Filter import Filter
+
+    bounds = _check_bounds(bounds)
+    rank, world = hx.rank, hx.world
+    n_total = bounds[-1][1]
+    lib = ctx.lib
+    if sb.dtype == np.float32:
+        out_h, out_halos = _output_halos(ctx, bounds, world, out_halo)
+        if n_total <= Filter.EXACT_DC_MAX:
+            def chain(carry):
+                c = np.ascontiguousarray(carry, dtype=np.float32)
+                s = np.zeros(2, dtype=np.float64)
+                ctx.check(lib.urh_dc_column_sums(ctx.handle, C.c_void_p(sb.shard.ptr), sb.n, 1, c.ctypes.data_as(C.c_void_p),
+                                                 s.ctypes.data_as(C.c_void_p)))
+                return s.astype(np.float32)   # float32 accumulators carried in doubles: exact
+
+            def allgather(pair):
+                every = nccl_allgather_wide(ctx, world, np.ascontiguousarray(pair, dtype=np.float32).view(np.int64))
+                return np.ascontiguousarray(every).view(np.float32).reshape(world, 2)
+            mean = dc_exact_handover(rank, world, chain, allgather) / np.float32(n_total)
+        else:
+            s = np.zeros(2, dtype=np.float64)
+            ctx.check(lib.urh_dc_column_sums(ctx.handle, C.c_void_p(sb.shard.ptr), sb.n, 0, None, s.ctypes.data_as(C.c_void_p)))
+            every = nccl_allgather_wide(ctx, world, s.view(np.int64))
+            mean = dc_fold_double(np.ascontiguousarray(every).view(np.float64).reshape(world, 2), n_total)
+        out = ShardBuffer(ctx, sb.n, np.float32, halo=out_h)
+        ctx.check(lib.urh_dc_subtract(ctx.handle, C.c_void_p(sb.shard.ptr), sb.n, float(mean[0]), float(mean[1]), C.c_void_p(out.shard.ptr)))
+        exchange_halos(ctx, hx, out, out_halos)
+    elif sb.dtype in (np.int8, np.uint8, np.int16, np.uint16):
+        s = np.zeros(2, dtype=np.int64)
+        ctx.check(lib.urh_dc_int_column_sums(ctx.handle, C.c_void_p(sb.shard.ptr), _lib.dtype_code(sb.dtype), sb.n, s.ctypes.data_as(C.c_void_p)))
+        every = nccl_allgather_wide(ctx, world, s)
+        mean = [float(sum(int(v) for v in every[:, c])) / float(n_total) for c in (0, 1)]
+        out = ShardBuffer(ctx, sb.n, np.float64, halo=0)
+        ctx.check(lib.urh_dc_int_subtract(ctx.handle, C.c_void_p(sb.shard.ptr), _lib.dtype_code(sb.dtype), sb.n, mean[0], mean[1],
+                                          C.c_void_p(out.shard.ptr)))
+    else:
+        raise ValueError("dc_correction expects an (n, 2) capture of int8/uint8/int16/uint16/float32")
+    ctx.sync()
+    return out
+
+
+def filter_work_sharded(ctx, hx, sb: ShardBuffer, bounds, filt, out_halo=None) -> ShardBuffer:
+    """Filter.work (Filter.py:30-33) of a capture sharded over the ranks: the DC correction or the FIR filter of ``filt``"""
+    from .signalprocessing.Filter import FilterType
+
+    if filt.filter_type == FilterType.dc_correction:
+        return dc_correction_sharded(ctx, hx, sb, bounds, out_halo)
+    return fir_filter_sharded(ctx, hx, sb, bounds, filt.taps, out_halo)
+
+
+def spectrogram_db_sharded(ctx, hx, sb: ShardBuffer, bounds, window_size=1024, overlap_factor=0.5, window_function=np.hanning):
+    """Spectrogram.calculate_spectrogram (Spectrogram.py:156-162) of a capture sharded over the ranks -> (first_frame, DeviceArray
+    [frames, W]): the rows of the single-GPU dB map this rank owns (``frame_plan``), bit for bit."""
+    bounds = _check_bounds(bounds)
+    rank = hx.rank
+    _float_shard(sb, "spectrogram")
+    W = int(window_size)
+    hop = W - int(overlap_factor * W)
+    plan = frame_plan(bounds[-1][1], W, hop, bounds)
+    f0, nf, right = plan[rank]
+    src = _with_room(ctx, sb, 0, right)
+    exchange_halos(ctx, hx, src, [(0, r) for _, _, r in plan])
+    out = DeviceArray(ctx, (nf, W), np.float32)
+    if nf:
+        win = src.window(0, right)[f0 * hop - bounds[rank][0]:]
+        d_w = to_device(np.ascontiguousarray(window_function(W), dtype=np.float64), ctx)
+        ctx.check(ctx.lib.urh_spectrogram_db(ctx.handle, C.c_void_p(win.ptr), len(win), W, hop, C.c_void_p(d_w.ptr), nf, C.c_void_p(out.ptr)))
+    ctx.sync()
+    return f0, out
+
+
+def spectrogram_image_segments_sharded(ctx, hx, sb: ShardBuffer, bounds, window_size=1024, overlap_factor=0.5, window_function=np.hanning,
+                                       colormap=None, data_min=-140, data_max=10, transpose=False):
+    """Spectrogram.create_image_segments (Spectrogram.py:183-190) of a capture sharded over the ranks -> [(segment_index, image)] of the
+    segments that start in this rank's shard (``segment_plan``), each a uint8 DeviceArray [W][frames][4] (transpose: [frames][W][4], the
+    layout of create_spectrogram_image(start, end, transpose=True)), bit for bit the single-GPU images."""
+    from .signalprocessing.Spectrogram import Spectrogram
+
+    bounds = _check_bounds(bounds)
+    rank = hx.rank
+    _float_shard(sb, "spectrogram images")
+    cmap = Spectrogram._colormap(colormap)
+    spec = Spectrogram(None, window_size=int(window_size), overlap_factor=overlap_factor, window_function=window_function)
+    spec.data_min, spec.data_max = data_min, data_max
+    segments, owned, rights = segment_plan(bounds[-1][1], spec.window_size, spec.hop_size, bounds, spec.MAX_LINES_PER_VIEW)
+    right = rights[rank]
+    src = _with_room(ctx, sb, 0, right)
+    exchange_halos(ctx, hx, src, [(0, r) for r in rights])
+    mine = owned[rank]
+    if not mine:
+        ctx.sync()
+        return []
+    g0 = bounds[rank][0]
+    win = src.window(0, right)
+    out, shapes = spec._images(win, len(win), [(segments[i][0] - g0, segments[i][1] - segments[i][0]) for i in mine], transpose, cmap, ctx)
+    ctx.sync()
+    return list(zip(mine, spec._split(out, shapes, True)))

@@ -110,12 +110,17 @@ class Filter(object):
         return Filter._convolve_full_slice(x, h, too_much, n - 2 * too_much)
 
     @staticmethod
-    def apply_bandpass_filter(data, f_low, f_high, filter_bw=0.08):
+    def bandpass_taps(f_low, f_high, filter_bw=0.08):
+        """the taps apply_bandpass_filter designs: edges swapped into order and clamped to [-0.5, 0.5]"""
         if f_low > f_high:
             f_low, f_high = f_high, f_low
         f_low = max(-0.5, min(0.5, f_low))
         f_high = max(-0.5, min(0.5, f_high))
-        h = Filter.design_windowed_sinc_bandpass(f_low, f_high, filter_bw)
+        return Filter.design_windowed_sinc_bandpass(f_low, f_high, filter_bw)
+
+    @staticmethod
+    def apply_bandpass_filter(data, f_low, f_high, filter_bw=0.08):
+        h = Filter.bandpass_taps(f_low, f_high, filter_bw)
         if len(h) < 8 * math.log(math.sqrt(len(data))):
             # np.convolve(data, h, "same"): centred on the longer operand
             big, small = max(len(data), len(h)), min(len(data), len(h))

@@ -128,11 +128,19 @@ class Spectrogram(object):
 
     def segment_bounds(self):
         """[(start, end, frames)] of the slices create_image_segments renders (Spectrogram.py:183-190, the same float arithmetic)"""
-        n = len(self.samples)
-        n_segments = max(1, self.time_bins // self.MAX_LINES_PER_VIEW)
-        step = self.time_bins / n_segments
-        step = max(1, int((step / self.hop_size) * self.hop_size ** 2))
-        return [(i, min(i + step, n), self._num_frames(min(i + step, n) - i)) for i in range(0, n, step)]
+        return self.segment_bounds_of(len(self.samples), self.window_size, self.hop_size, self.MAX_LINES_PER_VIEW)
+
+    @staticmethod
+    def segment_bounds_of(n, window_size, hop_size, max_lines=MAX_LINES_PER_VIEW):
+        """segment_bounds of a capture of n samples, without the samples (a capture sharded over several GPUs)"""
+        time_bins = int(math.ceil(n / hop_size))
+        n_segments = max(1, time_bins // max_lines)
+        step = time_bins / n_segments
+        step = max(1, int((step / hop_size) * hop_size ** 2))
+
+        def frames(length):
+            return max(1, (max(length, window_size) - window_size) // hop_size + 1)
+        return [(i, min(i + step, n), frames(min(i + step, n) - i)) for i in range(0, n, step)]
 
     def _images(self, d_x, n, segments, transpose, cmap, ctx):
         """one device call for all (start, length) segments: the uint8 buffer with the images back to back, and their shapes"""
