@@ -254,6 +254,54 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
                                          int mod_type, uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size,
                                          int64_t chunk_samples, void* d_iq_scratch, float* d_qad_out, int64_t global_offset,
                                          int64_t n_total, double* center, int* center_state, int64_t* k);
+/* ---- streaming: host captures of any size through a ring of `ring` (2..8) device slots of chunk_samples each (digitize.cu,
+ * DESIGN.md §4.11).  chunk_samples <= 0: 2^24; it is rounded down to a multiple of 2048 (at least 2048).  Host buffers may be pinned
+ * (urh_host_alloc: copies overlap the kernels) or pageable, e.g. a memory-mapped file (correct, but each copy then blocks the host).
+ * Results are bit-identical to the resident entry points named below.  ASK / FSK only; PSK raises URH_ERR_INVALID.
+ * urh_afp_demod_stream: afp_demod (signal_functions.pyx:333-378) from host IQ into host qad h_qad[n].
+ * urh_grab_pulse_lens_stream: grab_pulse_lens (signal_functions.pyx:392-495) of qad[n], any bits_per_symbol; qad_on_device != 0: qad
+ *   is a device buffer (only the digitizer's work arrays are chunked).  Rows as urh_grab_pulse_lens (urh_fetch_pulses).
+ * urh_demod_digitize_stream: afp_demod + grab_pulse_lens for a known center in one pass over the IQ (urh_demod_digitize); h_qad_out
+ *   (may be NULL) receives qad.
+ * urh_demod_center_digitize_stream: urh_demod_center_digitize (afp_demod + AutoInterpretation.detect_center, AutoInterpretation.py:
+ *   226-277, + grab_pulse_lens) with the IQ streamed and qad resident in d_qad_out[n]; h_qad_out (may be NULL) mirrors it to the host.
+ *   center_state as urh_demod_center_digitize; on state 2 the tables of urh_center_window_stats / urh_center_histogram_tiles are
+ *   left for d_qad_out, and *kept = the number of kept samples (the input of the stepwise detect_center).
+ * urh_stream_footprint: device bytes a call needs, callable without a device.  entry = URH_STREAM_ENTRY_* | URH_STREAM_* flags;
+ *   URH_STREAM_RESIDENT gives the resident entry's bytes for the same capture instead.  rows: the pulse-table rows to budget for
+ *   (-1: the bound n / (tolerance + 1) + 3 that no capture exceeds; -2: the n / 64 + 1024 rows the resident call reserves up front).
+ * urh_stream_schedule: the order in which a call issues its copies and chunk computations, 6 int64 per op {kind (0 upload into
+ *   the slot, 1 compute, 2 download from the slot), chunk, slot, first sample, end sample, 1 if the upload carries the halo sample
+ *   first - 1}; host only.  flags: URH_STREAM_UPLOAD / DOWNLOAD / HALO.
+ * urh_stream_stats: {lowest free device memory seen inside the last streamed call (after each chunk and each chunk's finish and
+ *   while the pulse table grows; sampled only with urh_set_profiling on, else -1), chunks of its ring pass, the most bytes of
+ *   scratch-arena requests live at once during it}.
+ * urh_mem_get_info: cudaMemGetInfo on the context's device. */
+#define URH_STREAM_ENTRY_AFP_DEMOD 0
+#define URH_STREAM_ENTRY_GRAB_PULSE_LENS 1
+#define URH_STREAM_ENTRY_DEMOD_DIGITIZE 2
+#define URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE 3
+#define URH_STREAM_QAD_OUT 0x10       /* demod_digitize: qad also goes to the host */
+#define URH_STREAM_RESIDENT 0x20      /* footprint of the resident entry point */
+#define URH_STREAM_QAD_ON_DEVICE 0x40 /* grab_pulse_lens: qad is already on the device */
+#define URH_STREAM_UPLOAD 1
+#define URH_STREAM_DOWNLOAD 2
+#define URH_STREAM_HALO 4
+int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, int64_t chunk_samples,
+                         int ring, float* h_qad);
+int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qad_on_device, int64_t n, float center, uint16_t tolerance,
+                               int mod_type, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
+                               int64_t chunk_samples, int ring, int64_t* k);
+int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, float center,
+                              uint16_t tolerance, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
+                              int64_t chunk_samples, int ring, float* h_qad_out, int64_t* k);
+int urh_demod_center_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type,
+                                     uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size, int64_t chunk_samples, int ring,
+                                     float* d_qad_out, float* h_qad_out, double* center, int* center_state, int64_t* kept, int64_t* k);
+int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows, int64_t* bytes);
+int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
+int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3);
+int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
 int urh_shard_demod_center_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag,
                                     int mod_type, uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size,
                                     float* d_qad_out, int64_t global_offset, int64_t n_total, double* center,

@@ -18,6 +18,10 @@ ERR_CUDA, ERR_INVALID, ERR_DTYPE, ERR_NOMEM, ERR_MODULATION, ERR_NO_DEVICE = -1,
 
 DT_I8, DT_U8, DT_I16, DT_U16, DT_F32 = 0, 1, 2, 3, 4
 MOD_ASK, MOD_FSK, MOD_PSK, MOD_QAM, MOD_GFSK, MOD_OQPSK = 0, 1, 2, 3, 4, 5
+# streamed entry points (include/urh_b200.h)
+STREAM_AFP_DEMOD, STREAM_GRAB_PULSE_LENS, STREAM_DEMOD_DIGITIZE, STREAM_DEMOD_CENTER_DIGITIZE = 0, 1, 2, 3
+STREAM_QAD_OUT, STREAM_RESIDENT, STREAM_QAD_ON_DEVICE = 0x10, 0x20, 0x40
+STREAM_UPLOAD, STREAM_DOWNLOAD, STREAM_HALO = 1, 2, 4
 
 _DTYPE_CODE = {
     np.dtype(np.int8): DT_I8,
@@ -165,6 +169,15 @@ SIGNATURES = {
     "urh_qpath_streams": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, i64, vp, vp, i32, vp, vp]),
     "urh_modulate_stats": (i32, [vp, vp]),
     "urh_synth_psk": (i32, [vp, vp, i64, i64, i32, i32, C.c_double, f32, f32, C.c_uint64, i64, i64, i64]),
+    "urh_afp_demod_stream": (i32, [vp, vp, i32, i64, f32, i32, i64, i32, vp]),
+    "urh_grab_pulse_lens_stream": (i32, [vp, vp, i32, i64, f32, u16, i32, u32, u8, f32, i64, i32, C.POINTER(i64)]),
+    "urh_demod_digitize_stream": (i32, [vp, vp, i32, i64, f32, i32, f32, u16, u32, u8, f32, i64, i32, vp, C.POINTER(i64)]),
+    "urh_demod_center_digitize_stream": (i32, [vp, vp, i32, i64, f32, i32, u16, u32, i64, i64, i32, vp, vp, C.POINTER(C.c_double),
+                                               C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
+    "urh_stream_footprint": (i32, [i64, i32, i32, i64, i32, i32, i64, C.POINTER(i64)]),
+    "urh_stream_schedule": (i32, [i64, i64, i32, i32, vp, i64, C.POINTER(i64)]),
+    "urh_stream_stats": (i32, [vp, vp]),
+    "urh_mem_get_info": (i32, [vp, C.POINTER(szt), C.POINTER(szt)]),
     "urh_synth_fsk": (i32, [vp, vp, i64, i64, i32, vp, vp, C.c_double, f32, f32, C.c_uint64, i64, i64, i64, i64, i64]),
 }
 

@@ -96,6 +96,10 @@ struct urh_ctx {
     void* step_dev;
     // digitizer exchange state of a sharded capture (finish.cu)
     void* shard_fin;
+    // last streamed call (digitize.cu): lowest free device memory seen after a chunk, number of chunks
+    int64_t stream_free_low, stream_chunks;
+    size_t arena_live;   // bytes of the arena requests live since the last reset (released ones not counted)
+    size_t arena_peak;   // the most arena_live reached since the last reset
 };
 
 #define URH_CUDA(ctx, call)                                                                         \
@@ -146,7 +150,21 @@ static inline int urh_arena(urh_ctx* ctx, size_t count, T** out) {
     *out = (T*)p;
     return rc;
 }
+// bump position of the arena: work that repeats per chunk releases what it took (reuse is stream-ordered, as after a reset)
+struct UrhArenaMark {
+    size_t block, used, live;
+};
+static inline UrhArenaMark urh_arena_mark(const urh_ctx* ctx) { return UrhArenaMark{ctx->arena_block, ctx->arena_used, ctx->arena_live}; }
+static inline void urh_arena_release(urh_ctx* ctx, const UrhArenaMark& m) {
+    ctx->arena_block = m.block;
+    ctx->arena_used = m.used;
+    ctx->arena_live = m.live;
+}
 int urh_ensure_pulses(urh_ctx* ctx, size_t rows);
+// grow the pulse table to at least `rows`, keeping its first `keep` rows (a table that chunks are appended to)
+int urh_ensure_pulses_keep(urh_ctx* ctx, size_t rows, size_t keep);
+// streamed calls with profiling on (urh_set_profiling): lower ctx->stream_free_low to the device's free memory now (urh_stream_stats)
+void urh_stream_sample_free(urh_ctx* ctx);
 void urh_release_mod_plans(urh_ctx* ctx);  // modulation.cu
 int urh_ensure_stage(urh_ctx* ctx, size_t bytes);
 

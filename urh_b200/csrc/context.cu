@@ -48,6 +48,8 @@ extern "C" int urh_ctx_create(int device, urh_ctx** out) {
     for (int i = 0; i < 8; i++) ctx->p2p_peer[i] = nullptr;
     ctx->nccl_rank = 0;
     ctx->nccl_world = 1;
+    ctx->stream_free_low = -1;
+    ctx->stream_chunks = 0;
     if (cudaSetDevice(device) != cudaSuccess) {
         delete ctx;
         return URH_ERR_CUDA;
@@ -256,19 +258,27 @@ void urh_arena_reset(urh_ctx* ctx) {
     ctx->arena_block = 0;
     ctx->arena_used = 0;
     ctx->arena_need = 0;
+    ctx->arena_live = 0;
+    ctx->arena_peak = 0;
     ctx->center_prefix = nullptr;  // the detect_center tile table lived in the arena
     ctx->bits_valid = 0;           // so did the bit arrays
+}
+
+static void arena_note_peak(urh_ctx* ctx) {
+    if (ctx->arena_live > ctx->arena_peak) ctx->arena_peak = ctx->arena_live;
 }
 
 int urh_arena_alloc(urh_ctx* ctx, size_t bytes, void** out) {
     bytes = (bytes + 255) & ~(size_t)255;
     if (bytes == 0) bytes = 256;
     ctx->arena_need += bytes;
+    ctx->arena_live += bytes;
     while (ctx->arena_block < ctx->arena.size()) {
         urh_block& b = ctx->arena[ctx->arena_block];
         if (ctx->arena_used + bytes <= b.bytes) {
             *out = (char*)b.ptr + ctx->arena_used;
             ctx->arena_used += bytes;
+            arena_note_peak(ctx);
             return URH_OK;
         }
         ctx->arena_block++;
@@ -290,6 +300,7 @@ int urh_arena_alloc(urh_ctx* ctx, size_t bytes, void** out) {
     ctx->arena.push_back({p, want});
     ctx->arena_block = ctx->arena.size() - 1;
     ctx->arena_used = bytes;
+    arena_note_peak(ctx);
     *out = p;
     return URH_OK;
 }
@@ -306,6 +317,34 @@ int urh_ensure_pulses(urh_ctx* ctx, size_t rows) {
     size_t cap = rows + rows / 4;
     URH_CUDA(ctx, cudaMalloc((void**)&ctx->pulses, cap * 2 * sizeof(int64_t)));
     ctx->pulses_cap_rows = cap;
+    return URH_OK;
+}
+
+int urh_ensure_pulses_keep(urh_ctx* ctx, size_t rows, size_t keep) {
+    if (rows <= ctx->pulses_cap_rows) return URH_OK;
+    int64_t* p = nullptr;
+    URH_CUDA(ctx, cudaMalloc((void**)&p, rows * 2 * sizeof(int64_t)));
+    urh_stream_sample_free(ctx);   // the old and the new table coexist here
+    if (ctx->pulses) {
+        if (keep) URH_CUDA(ctx, cudaMemcpyAsync(p, ctx->pulses, keep * 2 * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        URH_CUDA(ctx, cudaFree(ctx->pulses));
+    }
+    ctx->pulses = p;
+    ctx->pulses_cap_rows = rows;
+    return URH_OK;
+}
+
+void urh_stream_sample_free(urh_ctx* ctx) {
+    if (!ctx->profiling) return;   // a driver call per chunk: only when measuring
+    size_t fr = 0, tot = 0;
+    if (cudaMemGetInfo(&fr, &tot) == cudaSuccess && (ctx->stream_free_low < 0 || (int64_t)fr < ctx->stream_free_low))
+        ctx->stream_free_low = (int64_t)fr;
+}
+
+extern "C" int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes) {
+    URH_CUDA(ctx, cudaSetDevice(ctx->device));
+    URH_CUDA(ctx, cudaMemGetInfo(free_bytes, total_bytes));
     return URH_OK;
 }
 

@@ -544,6 +544,313 @@ extern "C" int urh_shard_dense_qad(urh_ctx* ctx, const float* d_qad, int64_t n, 
     return URH_OK;
 }
 
+// ---- streaming through a ring of device slots (DESIGN.md §4.11) -----------------------------------------------------------------
+// A chunk is a whole number of tiles (the last one excepted), so every tile has the bounds and the arithmetic it has in the resident
+// call.  IQ kernels see the slot through a pointer shifted back by the chunk's first sample: they index the capture globally, their
+// tile range is the chunk's, and the halo sample (uploaded with the chunk) sits where the resident buffer holds it.
+int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
+                     int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
+                     int64_t rows_cap, int64_t* k);   // finish.cu
+
+#define URH_STREAM_MAX_RING 8
+#define URH_STREAM_PAD 256   // slot = [pad][halo][chunk]: the chunk starts 256 bytes in, the halo sample right before it
+enum { URH_OP_UPLOAD = 0, URH_OP_COMPUTE = 1, URH_OP_DOWNLOAD = 2 };
+
+static int64_t stream_chunk_samples(int64_t n, int64_t cs) {
+    if (cs <= 0) cs = (int64_t)1 << 24;
+    cs -= cs % URH_TILE;
+    if (cs < URH_TILE) cs = URH_TILE;
+    const int64_t whole = urh_div_up(n > 0 ? n : 1, URH_TILE) * URH_TILE;   // a capture shorter than a chunk: one slot of its size
+    return cs < whole ? cs : whole;
+}
+// rows one digitizer pass over n samples can produce: firings are >= tol + 1 samples apart, plus the head and the tail row
+static int64_t rows_bound(int64_t n, int tol) { return n / (tol + 1) + 3; }
+
+// Op semantics (the driver below and tests/test_stream_plan_cpu.py's model):
+//   upload(c, s)   copy stream 0: waits for the last compute recorded on slot s, copies, records "uploaded" on s
+//   compute(c, s)  compute stream: waits for "uploaded" on s (uploading calls) and for the last download recorded on s (downloading
+//                  calls), runs the chunk, records "computed" on s
+//   download(c, s) copy stream 1: waits for "computed" on s, copies qad out, records "downloaded" on s
+// Uploads run R - 1 chunks ahead: the upload of chunk c + R - 1 is issued before compute(c), into the slot compute(c - 1) released.
+extern "C" int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count) {
+    if (!count || n < 0 || ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
+    const int64_t cs = stream_chunk_samples(n, chunk_samples);
+    const int64_t chunks = urh_div_up(n, cs);
+    const bool up = flags & URH_STREAM_UPLOAD, down = flags & URH_STREAM_DOWNLOAD, halo = flags & URH_STREAM_HALO;
+    int64_t k = 0;
+    auto emit = [&](int64_t kind, int64_t c) {
+        if (h_ops && k < cap) {
+            int64_t* o = h_ops + 6 * k;
+            o[0] = kind; o[1] = c; o[2] = c % ring; o[3] = c * cs; o[4] = (c + 1) * cs < n ? (c + 1) * cs : n;
+            o[5] = (kind == URH_OP_UPLOAD && halo && c > 0) ? 1 : 0;
+        }
+        k++;
+    };
+    if (up)
+        for (int64_t c = 0; c < ring - 1 && c < chunks; c++) emit(URH_OP_UPLOAD, c);
+    for (int64_t c = 0; c < chunks; c++) {
+        if (up && c + ring - 1 < chunks) emit(URH_OP_UPLOAD, c + ring - 1);
+        emit(URH_OP_COMPUTE, c);
+        if (down) emit(URH_OP_DOWNLOAD, c);
+    }
+    *count = k;
+    return (h_ops && k > cap) ? URH_ERR_INVALID : URH_OK;
+}
+
+// Device bytes of the ring (one cudaMallocAsync block) and of the arena requests of a call; the one place these sizes live.
+struct StreamSizes {
+    int64_t cs;          // chunk samples
+    int64_t src_slot;    // bytes per source slot (0: no upload ring)
+    int64_t qad_slot;    // bytes per qad slot (0: no download ring)
+    int64_t ring_bytes;  // the ring block
+    int64_t arena;       // arena requests (tiles, staging, carries, finish, center tables)
+    int64_t scan_items;  // largest table a look-back scan of the call runs over
+    int64_t rows_chunk;  // bound of one chunk's rows
+};
+static int64_t r256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+static int64_t finish_arena_bytes(int64_t tiles, int64_t rows_cap, bool ask) {
+    return r256(tiles * (int64_t)sizeof(RunCarry)) + 2 * r256(tiles * 4) + 2 * r256(tiles * 8) + r256((32 + 8) * 8) +
+           (ask ? r256(rows_cap * 16) : 0);
+}
+static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_samples, int ring, int entry) {
+    StreamSizes z;
+    const int kind = entry & 0xf;
+    const bool resident = entry & URH_STREAM_RESIDENT;
+    const int64_t ntiles = urh_div_up(n, URH_TILE);
+    z.cs = resident ? ntiles * URH_TILE : stream_chunk_samples(n, chunk_samples);
+    const int64_t ct = z.cs / URH_TILE;
+    const int64_t cap = stage_cap_for(tol);
+    const bool iq = kind != URH_STREAM_ENTRY_GRAB_PULSE_LENS;
+    const bool digitize = kind != URH_STREAM_ENTRY_AFP_DEMOD;
+    z.rows_chunk = rows_bound(z.cs, tol);
+    if (resident) {   // what the resident entry allocates for a host capture: the capture and qad on the device, full-size tables
+        z.src_slot = iq ? n * urh_iq_bytes(dtype) : n * 4;
+        z.qad_slot = (kind == URH_STREAM_ENTRY_GRAB_PULSE_LENS) ? 0 : n * 4;
+        z.ring_bytes = r256(z.src_slot) + r256(z.qad_slot);
+    } else {
+        z.src_slot = (kind == URH_STREAM_ENTRY_GRAB_PULSE_LENS && (entry & URH_STREAM_QAD_ON_DEVICE)) ? 0
+                     : URH_STREAM_PAD + z.cs * (iq ? urh_iq_bytes(dtype) : 4);
+        const bool qad_ring = kind == URH_STREAM_ENTRY_AFP_DEMOD || (kind == URH_STREAM_ENTRY_DEMOD_DIGITIZE && (entry & URH_STREAM_QAD_OUT));
+        z.qad_slot = qad_ring ? z.cs * 4 : 0;
+        z.ring_bytes = ring * (r256(z.src_slot) + r256(z.qad_slot));
+        if (kind == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) z.ring_bytes += r256(n * 4);   // resident qad (the caller's buffer)
+    }
+    z.arena = 0;
+    z.scan_items = ct > z.rows_chunk ? ct : z.rows_chunk;
+    if (digitize) z.arena += r256(ct * (int64_t)sizeof(UrhTileSummary)) + r256(ct * cap * 4) + r256(16) + r256(sizeof(UrhChain)) +
+                             finish_arena_bytes(ct, z.rows_chunk, true);
+    if (kind == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) {   // tile statistics, fine histogram, center chain (center.cu)
+        z.arena += r256(ntiles * (int64_t)sizeof(UrhTileStats)) + r256((int64_t)URH_FINE_SLABS * URH_FINE_NB * 4) + r256((ntiles + 1) * 8) +
+                   ((int64_t)2 << 20);
+        if (ntiles > z.scan_items) z.scan_items = ntiles;
+    }
+    return z;
+}
+
+extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows,
+                                    int64_t* bytes) {
+    if (!bytes || n < 0 || tolerance < 0 || tolerance > 0xffff || (entry & 0xf) > URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) return URH_ERR_INVALID;
+    if (!(entry & URH_STREAM_RESIDENT) && (ring < 2 || ring > URH_STREAM_MAX_RING)) return URH_ERR_INVALID;
+    if ((entry & 0xf) != URH_STREAM_ENTRY_GRAB_PULSE_LENS && urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
+    const StreamSizes z = stream_sizes(n, dtype, tolerance, chunk_samples, ring, entry);
+    const bool digitize = (entry & 0xf) != URH_STREAM_ENTRY_AFP_DEMOD;
+    // rows -1: the bound no capture exceeds; -2: what the resident finish reserves up front (finish.cu: n / 64 + 1024)
+    const int64_t r = rows == -2 ? n / 64 + 1024 : (rows < 0 ? rows_bound(n, tolerance) : rows);
+    if (entry & URH_STREAM_RESIDENT) {
+        // capture + qad, full-size digitizer tables, the pulse table as urh_ensure_pulses sizes it (1.25 x rows)
+        const int64_t ntiles = urh_div_up(n, URH_TILE);
+        int64_t b = z.ring_bytes + ((int64_t)64 << 20);
+        if (digitize)
+            b += r256(ntiles * (int64_t)sizeof(UrhTileSummary)) + r256(ntiles * (int64_t)stage_cap_for(tolerance) * 4) +
+                 finish_arena_bytes(ntiles, r + r / 4, true) + 16 * (r + r / 4);
+        if ((entry & 0xf) == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE)
+            b += r256(ntiles * (int64_t)sizeof(UrhTileStats)) + r256((int64_t)URH_FINE_SLABS * URH_FINE_NB * 4) + r256((ntiles + 1) * 8);
+        *bytes = b;
+        return URH_OK;
+    }
+    int64_t b = z.ring_bytes;
+    // the arena grows in blocks of at least 64 MiB; a request that does not fit the current block's rest opens a new one, so new
+    // blocks hold at most twice the requests plus one block
+    b += 2 * z.arena + ((int64_t)64 << 20);
+    // look-back scan workspace (context.cu urhts::prepare): at least 8192 blocks, 256+ items each
+    const int64_t nb = 2 * (z.scan_items / 256 + 1);
+    b += 256 + (nb > 8192 ? nb : 8192) * (4 + 2 * 32);
+    // pulse table: grown with its rows kept (old and new table alive during the copy, the new one up to twice the old)
+    if (digitize) b += 3 * 16 * (r + z.rows_chunk);
+    *bytes = b;
+    return URH_OK;
+}
+
+extern "C" int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3) {
+    h_out3[0] = ctx->stream_free_low;
+    h_out3[1] = ctx->stream_chunks;
+    h_out3[2] = (int64_t)ctx->arena_peak;
+    return URH_OK;
+}
+
+// The ring of one streamed call: the block, its events, and the copy streams drained before the block is freed on every exit path.
+struct StreamRing {
+    urh_ctx* ctx = nullptr;
+    char* mem = nullptr;
+    cudaEvent_t ev[3][URH_STREAM_MAX_RING] = {};
+    int ring = 0;
+    int init(urh_ctx* c, int r, int64_t bytes) {
+        ctx = c;
+        ring = r;
+        ctx->stream_free_low = -1;
+        for (int k = 0; k < 3; k++)
+            for (int s = 0; s < r; s++) URH_CUDA(ctx, cudaEventCreateWithFlags(&ev[k][s], cudaEventDisableTiming));
+        if (bytes > 0) URH_CUDA(ctx, cudaMallocAsync((void**)&mem, (size_t)bytes, ctx->stream));
+        // the copy streams start after everything queued on the compute stream so far (the ring block included)
+        URH_CUDA(ctx, cudaEventRecord(ctx->ev_comp[0], ctx->stream));
+        URH_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream[0], ctx->ev_comp[0], 0));
+        URH_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream[1], ctx->ev_comp[0], 0));
+        return URH_OK;
+    }
+    ~StreamRing() {
+        if (!ctx) return;
+        cudaStreamSynchronize(ctx->copy_stream[0]);
+        cudaStreamSynchronize(ctx->copy_stream[1]);
+        if (mem) cudaFreeAsync(mem, ctx->stream);
+        cudaStreamSynchronize(ctx->stream);
+        for (int k = 0; k < 3; k++)
+            for (int s = 0; s < ring; s++)
+                if (ev[k][s]) cudaEventDestroy(ev[k][s]);
+    }
+};
+
+// Runs the schedule: compute(c, s0, s1, slot) enqueues chunk c's work on the compute stream (it may synchronise).  h_src: host source
+// of src_b bytes per sample uploaded into slots of src_slot bytes at d_src (NULL: the computation reads device data); h_qad: host
+// destination of the qad slots at d_qad (cs floats each; NULL: none).
+template <typename F>
+static int stream_run(urh_ctx* ctx, int64_t n, int64_t cs, StreamRing& R, const char* h_src, int src_b, bool halo, char* d_src,
+                      int64_t src_slot, float* h_qad, float* d_qad, F&& compute, bool qad_resident = false) {
+    const int flags = (h_src ? URH_STREAM_UPLOAD : 0) | (h_qad ? URH_STREAM_DOWNLOAD : 0) | (halo ? URH_STREAM_HALO : 0);
+    int64_t count = 0;
+    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, nullptr, 0, &count));
+    std::vector<int64_t> ops((size_t)(6 * count));
+    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, ops.data(), count, &count));
+    bool recorded[3][URH_STREAM_MAX_RING] = {};
+    ctx->stream_chunks = 0;
+    for (int64_t i = 0; i < count; i++) {
+        const int64_t* o = &ops[(size_t)(6 * i)];
+        const int kind = (int)o[0], s = (int)o[2];
+        const int64_t c = o[1], s0 = o[3], s1 = o[4], h = o[5];
+        if (kind == URH_OP_UPLOAD) {
+            cudaStream_t cp = ctx->copy_stream[0];
+            if (recorded[URH_OP_COMPUTE][s]) URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
+            URH_CUDA(ctx, cudaMemcpyAsync(d_src + s * src_slot + URH_STREAM_PAD - h * src_b, h_src + (s0 - h) * src_b,
+                                          (size_t)((s1 - s0 + h) * src_b), cudaMemcpyHostToDevice, cp));
+            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_UPLOAD][s], cp));
+        } else if (kind == URH_OP_COMPUTE) {
+            if (h_src) URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_UPLOAD][s], 0));
+            if (h_qad && !qad_resident && recorded[URH_OP_DOWNLOAD][s])
+                URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_DOWNLOAD][s], 0));
+            URH_CHECK(compute(c, s0, s1, s));
+            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_COMPUTE][s], ctx->stream));
+            urh_stream_sample_free(ctx);
+            ctx->stream_chunks++;
+        } else {
+            cudaStream_t cp = ctx->copy_stream[1];
+            URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
+            URH_CUDA(ctx, cudaMemcpyAsync(h_qad + s0, d_qad + (qad_resident ? s0 : (int64_t)s * cs), (size_t)(s1 - s0) * sizeof(float),
+                                          cudaMemcpyDeviceToHost, cp));
+            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_DOWNLOAD][s], cp));
+        }
+        recorded[kind][s] = true;
+    }
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream[1]));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+
+// Per-chunk digitizer state of a streamed call: tile table and staging of one chunk, the carries between chunks, the row count.
+struct StreamDigitizer {
+    UrhTileSummary* tiles;
+    uint32_t* staging;
+    int16_t* d_init;
+    UrhChain* chain;
+    int cap, tol;
+    bool is_ask;
+    uint32_t sps;
+    int64_t n, rows, rows_all;
+    UrhArenaMark mark;
+    int init(urh_ctx* ctx, int64_t n_total, int64_t cs, int tolerance, bool ask, uint32_t samples_per_symbol) {
+        n = n_total; tol = tolerance; is_ask = ask; sps = samples_per_symbol; rows = 0;
+        cap = stage_cap_for(tol);
+        rows_all = rows_bound(n, tol);
+        const int64_t ct = cs / URH_TILE;
+        URH_CHECK(urh_arena(ctx, (size_t)ct, &tiles));
+        URH_CHECK(urh_arena(ctx, (size_t)ct * cap, &staging));
+        URH_CHECK(urh_arena(ctx, 8, &d_init));
+        URH_CHECK(urh_arena(ctx, 1, &chain));
+        URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
+        mark = urh_arena_mark(ctx);
+        return URH_OK;
+    }
+    // the chunk [s0, s1) whose dense pass has filled tiles / staging
+    int finish(urh_ctx* ctx, int64_t s0, int64_t s1) {
+        const int64_t rc = rows_bound(s1 - s0, tol);
+        const int64_t need = rows + rc;
+        if (need > (int64_t)ctx->pulses_cap_rows) {
+            int64_t grow = 2 * (int64_t)ctx->pulses_cap_rows;
+            if (grow > rows_all + rc) grow = rows_all + rc;
+            URH_CHECK(urh_ensure_pulses_keep(ctx, (size_t)(grow > need ? grow : need), (size_t)rows));
+        }
+        urh_arena_release(ctx, mark);
+        int64_t kc = 0;
+        URH_CHECK(urh_finish_chunk(ctx, s1 - s0, tol, is_ask, sps, tiles, staging, cap, d_init, chain, s0, n, rows, rc, &kc));
+        urh_stream_sample_free(ctx);
+        rows += kc;
+        return URH_OK;
+    }
+};
+
+static int stream_check(urh_ctx* ctx, int64_t n, int ring, int mod_type, int dtype, bool iq) {
+    if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "streamed call: empty capture");
+    if (ring < 2 || ring > URH_STREAM_MAX_RING) URH_FAIL(ctx, URH_ERR_INVALID, "streamed call: ring of %d slots (2..%d)", ring, URH_STREAM_MAX_RING);
+    if (iq && (n <= 2 || (mod_type != URH_MOD_ASK && mod_type != URH_MOD_FSK)))
+        URH_FAIL(ctx, URH_ERR_INVALID, "streamed demodulation: ASK/FSK and n > 2 (PSK is a serial recurrence)");
+    if (iq && urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
+    return URH_OK;
+}
+
+// IQ chunk computation on slot `s`: the dense kernels over tiles [s0 / TILE, ceil(s1 / TILE)) of the whole capture.
+template <bool DIG>
+static int stream_dense_iq(urh_ctx* ctx, int dtype, int mod_type, const char* d_src, int64_t src_slot, int64_t n, const UrhDemodParams& dp,
+                           float* qad_global, const UrhClassify& cls, int tol, StreamDigitizer* dz, int64_t s0, int64_t s1, int s,
+                           UrhTileStats* ts = nullptr, const UrhFine& fine = UrhFine{}) {
+    const int b = urh_iq_bytes(dtype);
+    const void* iq = d_src + s * src_slot + URH_STREAM_PAD - s0 * b;   // sample i of the capture at iq + i * b for i in [s0 - 1, s1)
+    const int64_t t0 = s0 / URH_TILE, t1 = urh_div_up(s1, URH_TILE);
+    UrhTileSummary* tiles = dz ? dz->tiles - t0 : nullptr;
+    uint32_t* staging = dz ? dz->staging - t0 * dz->cap : nullptr;
+    const int cap = dz ? dz->cap : 0;
+    int16_t* init = dz ? dz->d_init : nullptr;
+    const int c0 = DIG ? host_classify(0.0f, cls) : 0;
+    if (mod_type == URH_MOD_ASK)
+        return launch_dense_iq_m<URH_MOD_ASK, DIG>(ctx, dtype, iq, n, dp, qad_global, cls, tol, tiles, staging, cap, init, c0, 0, ts, t0, t1, fine);
+    return launch_dense_iq_m<URH_MOD_FSK, DIG>(ctx, dtype, iq, n, dp, qad_global, cls, tol, tiles, staging, cap, init, c0, 0, ts, t0, t1, fine);
+}
+
+// Digitizer dense pass over qad [s0, s1) at x (local view: chunk-relative tiles; only chunk 0 sets the initial state).
+static int stream_dense_qad(urh_ctx* ctx, const float* x, int64_t s0, int64_t s1, const UrhClassify& cls, StreamDigitizer& dz,
+                            const float* d_thr0 = nullptr, const UrhTileStats* ts = nullptr) {
+    const int64_t nc = s1 - s0;
+    const unsigned grid = (unsigned)urh_div_up(urh_div_up(nc, URH_TILE), URH_WARPS_PER_BLOCK);
+    const int vec_in = (((uintptr_t)x % 8) == 0) ? 1 : 0;
+    int16_t* init = s0 == 0 ? dz.d_init : nullptr;
+    const int c0 = d_thr0 ? 0 : host_classify(0.0f, cls);
+    const UrhTileStats* tsc = ts ? ts + s0 / URH_TILE : nullptr;
+    if (cls.order == 2)
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, nc, vec_in, cls, dz.tol, dz.tiles, dz.staging,
+                   dz.cap, init, c0, d_thr0, tsc);
+    else
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, nc, vec_in, cls, dz.tol, dz.tiles, dz.staging,
+                   dz.cap, init, c0, d_thr0, tsc);
+    return URH_OK;
+}
+
 // ---- one-call paths: every stage enqueued on the context stream, ONE synchronisation at the end -----------------------------
 struct CenterPlan;
 int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileStats* ts, int64_t max_size, int rank, int world,
@@ -605,10 +912,19 @@ extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, con
 // *center_state: 0 = detect_center finds no center (None; *k = 0), 1 = *center is valid, 2 = the device could not decide
 // (a tie between histogram peaks whose order numpy's argsort defines, or more than 6000 bins): d_qad_out is valid, the
 // caller finishes through the stepwise entry points (urh_center_window_stats / urh_center_histogram_tiles / urh_grab_pulse_lens).
+// sc != NULL: the IQ is streamed from sc->h_iq through a ring (d_iq unused), qad stays resident in d_qad_out (mirrored to sc->h_qad),
+// and the digitizer runs chunk by chunk over it with chained finishes, so no table grows with n but the tile statistics.
+struct StreamCenter {
+    int ring;
+    int64_t chunk_samples;
+    const void* h_iq;
+    float* h_qad;
+    int64_t* kept;
+};
 static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag, int mod_type,
                                       uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size, float* d_qad_out, bool sharded,
                                       int64_t global_offset, int64_t n_total, double* center, int* center_state, int64_t* k,
-                                      const void* h_iq = nullptr, int64_t chunk_samples = 0) {
+                                      const void* h_iq = nullptr, int64_t chunk_samples = 0, const StreamCenter* sc = nullptr) {
     if (!k || !center || !center_state) return URH_ERR_INVALID;
     *k = 0;
     *center = 0.0;
@@ -644,8 +960,21 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     // demodulated as soon as it has landed, so the demodulation pass hides behind the PCIe transfer.
     const int64_t chunk_tiles = (h_iq && chunk_samples > 0) ? (chunk_samples >= URH_TILE ? chunk_samples / URH_TILE : 1) : ntiles;
     const size_t sample_bytes = (size_t)urh_iq_bytes(dtype);
+    StreamRing ring;
+    int64_t scs = 0;
+    if (sc) {
+        const StreamSizes z = stream_sizes(n, dtype, tolerance, sc->chunk_samples, sc->ring, URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE);
+        scs = z.cs;
+        URH_CHECK(ring.init(ctx, sc->ring, sc->ring * r256(z.src_slot)));
+        const int64_t slot = r256(z.src_slot);
+        URH_CHECK(stream_run(ctx, n, scs, ring, (const char*)sc->h_iq, urh_iq_bytes(dtype), true, ring.mem, slot, sc->h_qad, d_qad_out,
+                             [&](int64_t, int64_t s0, int64_t s1, int s) {
+                                 return stream_dense_iq<false>(ctx, dtype, mod_type, ring.mem, slot, n, dp, d_qad_out, cls, 0, nullptr, s0, s1, s,
+                                                               ts, fine);
+                             }, true));
+    }
     int chunk_no = 0;
-    for (int64_t t0 = 0; t0 < ntiles; t0 += chunk_tiles, chunk_no++) {
+    for (int64_t t0 = 0; t0 < (sc ? 0 : ntiles); t0 += chunk_tiles, chunk_no++) {
         const int64_t t1 = (t0 + chunk_tiles < ntiles) ? t0 + chunk_tiles : ntiles;
         if (h_iq) {
             const int64_t s0 = t0 * URH_TILE, s1 = (t1 * URH_TILE < n) ? t1 * URH_TILE : n;
@@ -671,25 +1000,48 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     cls.noise_value = urh_noise_value(mod_type);
     cls.order = 2;
     const int tol = tolerance;
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
-    URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
-    const int vec_in = (((uintptr_t)d_qad_out % 8) == 0) ? 1 : 0;
-    URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK), URH_WARPS_PER_BLOCK * 32, 0,
-               (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts);
-    URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
     int64_t rows = 0;
-    if (sharded)
-        URH_CHECK(urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, &rows));
-    else
-        URH_CHECK(urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, &rows));
+    if (sc) {
+        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
+        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 45, (const int64_t*)ctx->center_prefix + ntiles, sizeof(int64_t), cudaMemcpyDeviceToHost,
+                                      ctx->stream));
+        // the chunked digitizer synchronises per chunk anyway: learn the state first and digitize only when there is a center
+        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        int st0 = 0;
+        memcpy(&st0, ctx->h_mail + 41, sizeof(int));
+        if (st0 == 1) {
+            StreamDigitizer dz;
+            URH_CHECK(dz.init(ctx, n, scs, tol, mod_type == URH_MOD_ASK, samples_per_symbol));
+            for (int64_t s0 = 0; s0 < n; s0 += scs) {
+                const int64_t s1 = s0 + scs < n ? s0 + scs : n;
+                URH_CHECK(stream_dense_qad(ctx, d_qad_out + s0, s0, s1, cls, dz, d_centerf, ts));
+                URH_CHECK(dz.finish(ctx, s0, s1));
+            }
+            rows = dz.rows;
+        }
+        *sc->kept = ctx->h_mail[45];
+    } else {
+        const int cap = stage_cap_for(tol);
+        UrhTileSummary* tiles;
+        uint32_t* staging;
+        int16_t* d_init;
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
+        URH_CHECK(urh_arena(ctx, 8, &d_init));
+        URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
+        const int vec_in = (((uintptr_t)d_qad_out % 8) == 0) ? 1 : 0;
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK), URH_WARPS_PER_BLOCK * 32, 0,
+                   (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts);
+        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
+        if (sharded)
+            URH_CHECK(urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, &rows));
+        else
+            URH_CHECK(urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, &rows));
+    }
     // the finish synchronised the stream: the two scalars have landed
     memcpy(center, ctx->h_mail + 40, sizeof(double));
     int st = 0;
@@ -746,6 +1098,95 @@ extern "C" int urh_shard_demod_center_digitize(urh_ctx* ctx, const void* d_iq, i
                                                int* center_state, int64_t* k) {
     return demod_center_digitize_impl(ctx, d_iq, dtype, n, has_halo, noise_mag, mod_type, tolerance, samples_per_symbol, max_size, d_qad_out,
                                       true, global_offset, n_total, center, center_state, k);
+}
+
+// ---- streamed entry points (include/urh_b200.h) ------------------------------------------------------------------------------------
+extern "C" int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, int64_t chunk_samples,
+                                    int ring, float* h_qad) {
+    if (!h_iq || !h_qad) return URH_ERR_INVALID;
+    URH_CHECK(stream_check(ctx, n, ring, mod_type, dtype, true));
+    urh_arena_reset(ctx);
+    const StreamSizes z = stream_sizes(n, dtype, 0, chunk_samples, ring, URH_STREAM_ENTRY_AFP_DEMOD);
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, z.ring_bytes));
+    char* d_src = R.mem;
+    float* d_qad = (float*)(R.mem + ring * r256(z.src_slot));
+    const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
+    UrhClassify cls;
+    memset(&cls, 0, sizeof(cls));
+    return stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), true, d_src, r256(z.src_slot), h_qad, d_qad,
+                      [&](int64_t, int64_t s0, int64_t s1, int s) {
+                          return stream_dense_iq<false>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp, d_qad + s * z.cs - s0, cls, 0,
+                                                        nullptr, s0, s1, s);
+                      });
+}
+
+extern "C" int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qad_on_device, int64_t n, float center, uint16_t tolerance,
+                                          int mod_type, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
+                                          int64_t chunk_samples, int ring, int64_t* k) {
+    if (!k || !qad) return URH_ERR_INVALID;
+    *k = 0;
+    ctx->pulses_k = 0;
+    URH_CHECK(stream_check(ctx, n, ring, mod_type, 0, false));
+    urh_arena_reset(ctx);
+    UrhClassify cls;
+    URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
+    const StreamSizes z = stream_sizes(n, 0, tolerance, chunk_samples, ring,
+                                       URH_STREAM_ENTRY_GRAB_PULSE_LENS | (qad_on_device ? URH_STREAM_QAD_ON_DEVICE : 0));
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, z.ring_bytes));
+    StreamDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
+    char* d_src = R.mem;
+    URH_CHECK(stream_run(ctx, n, z.cs, R, qad_on_device ? nullptr : (const char*)qad, 4, false, d_src, r256(z.src_slot), nullptr, nullptr,
+                         [&](int64_t, int64_t s0, int64_t s1, int s) {
+                             const float* x = qad_on_device ? qad + s0 : (const float*)(d_src + s * r256(z.src_slot) + URH_STREAM_PAD);
+                             URH_CHECK(stream_dense_qad(ctx, x, s0, s1, cls, dz));
+                             return dz.finish(ctx, s0, s1);
+                         }));
+    *k = dz.rows;
+    return URH_OK;
+}
+
+extern "C" int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, float center,
+                                         uint16_t tolerance, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
+                                         int64_t chunk_samples, int ring, float* h_qad_out, int64_t* k) {
+    if (!k || !h_iq) return URH_ERR_INVALID;
+    *k = 0;
+    ctx->pulses_k = 0;
+    URH_CHECK(stream_check(ctx, n, ring, mod_type, dtype, true));
+    urh_arena_reset(ctx);
+    UrhClassify cls;
+    URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
+    const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
+    const StreamSizes z = stream_sizes(n, dtype, tolerance, chunk_samples, ring,
+                                       URH_STREAM_ENTRY_DEMOD_DIGITIZE | (h_qad_out ? URH_STREAM_QAD_OUT : 0));
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, z.ring_bytes));
+    StreamDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
+    char* d_src = R.mem;
+    float* d_qad = h_qad_out ? (float*)(R.mem + ring * r256(z.src_slot)) : nullptr;
+    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), true, d_src, r256(z.src_slot), h_qad_out, d_qad,
+                         [&](int64_t, int64_t s0, int64_t s1, int s) {
+                             URH_CHECK(stream_dense_iq<true>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp,
+                                                             d_qad ? d_qad + s * z.cs - s0 : nullptr, cls, tolerance, &dz, s0, s1, s));
+                             return dz.finish(ctx, s0, s1);
+                         }));
+    *k = dz.rows;
+    return URH_OK;
+}
+
+extern "C" int urh_demod_center_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type,
+                                                uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size, int64_t chunk_samples,
+                                                int ring, float* d_qad_out, float* h_qad_out, double* center, int* center_state,
+                                                int64_t* kept, int64_t* k) {
+    if (!h_iq || !d_qad_out || !kept) return URH_ERR_INVALID;
+    URH_CHECK(stream_check(ctx, n, ring, mod_type, dtype, true));
+    StreamCenter sc;
+    sc.ring = ring; sc.chunk_samples = chunk_samples; sc.h_iq = h_iq; sc.h_qad = h_qad_out; sc.kept = kept;
+    return demod_center_digitize_impl(ctx, nullptr, dtype, n, 0, noise_mag, mod_type, tolerance, samples_per_symbol, max_size, d_qad_out,
+                                      false, 0, n, center, center_state, k, nullptr, 0, &sc);
 }
 
 struct UrhShardState {

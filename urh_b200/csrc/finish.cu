@@ -152,7 +152,8 @@ __global__ void __launch_bounds__(256) k_finish_rows(const UrhTileSummary* __res
                                                     const int16_t* __restrict__ d_prev0, const int64_t* __restrict__ row_off,
                                                     const int64_t* __restrict__ prev_fired, const int64_t* __restrict__ d_xprev_fired,
                                                     int64_t ntiles, int64_t global_offset, int64_t n_total, int tol, int is_ask, int64_t sps,
-                                                    int emit_tail, int64_t* __restrict__ out, int64_t cap_rows, int64_t* __restrict__ d_out) {
+                                                    int emit_tail, int64_t row_base, int64_t* __restrict__ out, int64_t cap_rows,
+                                                    int64_t* __restrict__ d_out) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= ntiles) return;
     const UrhTileSummary s = tiles[t];
@@ -183,8 +184,8 @@ __global__ void __launch_bounds__(256) k_finish_rows(const UrhTileSummary* __res
     }
     if (t == ntiles - 1) {
         const int64_t fired = idx;
-        // tail row (pyx:485-493): appended only while fewer than n rows exist
-        if (emit_tail && (is_ask || fired < n_total)) {
+        // tail row (pyx:485-493): appended only while fewer than n rows exist (row_base: rows of the chunks before this one)
+        if (emit_tail && (is_ask || row_base + fired < n_total)) {
             if (idx < cap_rows) *((longlong2*)out + idx) = make_longlong2(prev, (pp >= 0) ? (n_total - 1 - pp) : (n_total - tol));
             idx++;
         }
@@ -194,6 +195,8 @@ __global__ void __launch_bounds__(256) k_finish_rows(const UrhTileSummary* __res
 }
 
 // ---- ASK: merge equal neighbours (pyx:475-476) -------------------------------------------------------------------------
+// A chained chunk (prev_last != nullptr) writes at out = table + row_base rows; a first row whose state equals the table's last
+// row (*prev_last) is a head of 0 and lands at out[-1], i.e. it is added to that row, as merge_shard_rows joins shard edges.
 struct ScanMergeRows {
     const int64_t* raw;    // (state, length) x rows, the tail row last when has_tail
     int64_t rows;
@@ -201,11 +204,16 @@ struct ScanMergeRows {
     int has_tail;
     int64_t* out;
     int64_t* d_k;
-    __device__ __forceinline__ int64_t load(int64_t r) const { return (r == 0 || raw[2 * r] != raw[2 * r - 2]) ? 1 : 0; }
+    const int64_t* prev_last;   // state of the row before out[0] (nullptr: none)
+    int64_t row_base;           // rows before out[0]
+    __device__ __forceinline__ int64_t load(int64_t r) const {
+        if (r == 0) return (prev_last && raw[0] == *prev_last) ? 0 : 1;
+        return raw[2 * r] != raw[2 * r - 2] ? 1 : 0;
+    }
     __device__ __forceinline__ void post(int64_t r, const int64_t& excl, const int64_t& head) const {
         const bool is_tail = has_tail && r == rows - 1;
         // the tail row is appended only while fewer than n (merged) rows exist (pyx:487)
-        if (is_tail && excl >= n_total) {
+        if (is_tail && row_base + excl >= n_total) {
             *d_k = excl;
             return;
         }
@@ -257,6 +265,25 @@ __global__ void k_fold_prev_fired(const int64_t* __restrict__ all, int rank, int
     *xprev = v;
 }
 
+// ---- chained chunks (streaming) -------------------------------------------------------------------------------------------------
+// Before chunk 0's finish: the digitizer's initial state becomes the "previous class"; nothing precedes the capture.
+__global__ void k_chain_start(const int16_t* __restrict__ d_init, UrhChain* __restrict__ chain) {
+    chain->run.len = 0; chain->run.cls = 0; chain->run.flags = 2 | 1;
+    chain->prev_fired = -1;
+    chain->last_state = INT64_MIN;
+    chain->prev_cls = *d_init;
+}
+// After a chunk's rows: fold its three scan totals into the chain, as k_fold_* fold the totals of the preceding ranks.
+__global__ void k_chain_advance(UrhChain* __restrict__ chain, const RunCarry* __restrict__ tot_run, const CandAgg* __restrict__ tot_cand,
+                                const FireAgg* __restrict__ tot_fire) {
+    chain->run = RunCarryOp()(chain->run, *tot_run);
+    if (tot_cand->last_cls != CLS_NONE) chain->prev_cls = (int16_t)tot_cand->last_cls;
+    if (tot_fire->last_pos >= 0) chain->prev_fired = tot_fire->last_pos;
+}
+__global__ void k_chain_last_row(UrhChain* __restrict__ chain, const int64_t* __restrict__ table, int64_t rows) {
+    if (rows > 0) chain->last_state = table[2 * (rows - 1)];
+}
+
 int urh_coll_allgather(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank);   // nccl.cu: mailboxes or NCCL
 extern "C" int urh_p2p_check(urh_ctx* ctx);
 
@@ -266,12 +293,17 @@ struct FinishShard {
     int64_t global_offset;      // first sample of this shard in the capture
     int64_t n_total;
     int emit_tail;
+    // chained chunk of a capture streamed through this GPU: the carries come from *chain instead of the other ranks, and the rows
+    // are appended to the pulse table after its first row_base rows (the caller has made room for rows_cap more)
+    UrhChain* chain;
+    int64_t row_base, rows_cap;
 };
 
 static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
                         int stage_cap, const int16_t* d_init, const FinishShard& sh, int64_t* k) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     const bool sharded = sh.world > 1;
+    UrhChain* chain = sh.chain;
     RunCarry* carry;
     int32_t *head_rel, *prev_cls;
     int64_t *row_off, *prev_fired, *d_small;
@@ -296,6 +328,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     int64_t* d_all2 = d_all1 + 4 * (sharded ? sh.world : 0);
     int64_t* d_all3 = d_all2 + 2 * (sharded ? sh.world : 0);
 
+    if (chain && sh.global_offset == 0) URH_LAUNCH(ctx, k_chain_start, 1, 1, 0, d_init, chain);
     RunCarry rc_ident;
     rc_ident.len = 0; rc_ident.cls = 0; rc_ident.flags = 2 | 1;
     ScanRunCarry fa;
@@ -309,12 +342,13 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
         URH_LAUNCH(ctx, k_fold_carry, 1, 1, 0, (const int64_t*)d_all1, sh.rank, d_xcarry);
     }
     ScanCandidates fb;
-    fb.tiles = tiles; fb.staging = staging; fb.stage_cap = stage_cap; fb.carry = carry; fb.xcarry = sharded ? d_xcarry : nullptr;
+    fb.tiles = tiles; fb.staging = staging; fb.stage_cap = stage_cap; fb.carry = carry;
+    fb.xcarry = sharded ? d_xcarry : (chain ? &chain->run : nullptr);
     fb.tol = tol; fb.head_rel = head_rel; fb.prev_cls = prev_cls;
     CandAgg ca_ident;
     ca_ident.cnt = 0; ca_ident.last_cls = CLS_NONE; ca_ident.pad = 0;
     URH_CHECK((urhts::scan<CandAgg, CandOp, ScanCandidates>(ctx, ntiles, ca_ident, CandOp(), fb, d_tot_cand)));
-    const int16_t* prev0 = d_init;
+    const int16_t* prev0 = chain ? &chain->prev_cls : d_init;
     if (sharded) {
         URH_TL_MARK(ctx, "x5 candidates: enter");
         URH_CHECK(urh_coll_allgather(ctx, d_tot_cand, d_all2, sizeof(CandAgg)));
@@ -328,7 +362,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     FireAgg fi_ident;
     fi_ident.fired = 0; fi_ident.last_pos = -1;
     URH_CHECK((urhts::scan<FireAgg, FireOp, ScanFirings, 4>(ctx, ntiles, fi_ident, FireOp(), fc, d_tot_fire)));   // heavy load(): thin blocks
-    const int64_t* xprev = d_small + 2;
+    const int64_t* xprev = chain ? &chain->prev_fired : d_small + 2;
     if (sharded) {
         URH_TL_MARK(ctx, "x6 firings: enter");
         URH_CHECK(urh_coll_allgather(ctx, d_tot_fire, d_all3, sizeof(FireAgg)));
@@ -340,23 +374,25 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     // rows: straight into the pulse buffer (ASK: into scratch, merged afterwards)
     int64_t cap_rows = (int64_t)ctx->pulses_cap_rows;
     const int64_t guess = n / 64 + 1024;
-    if (cap_rows < guess) {
+    if (!chain && cap_rows < guess) {
         URH_CHECK(urh_ensure_pulses(ctx, (size_t)guess));
         cap_rows = (int64_t)ctx->pulses_cap_rows;
     }
-    int64_t* raw = ctx->pulses;
-    int64_t raw_cap = cap_rows;
+    const int64_t row_base = chain ? sh.row_base : 0;
+    int64_t* raw = ctx->pulses + 2 * row_base;
+    int64_t raw_cap = chain ? sh.rows_cap : cap_rows;
     if (is_ask) URH_CHECK(urh_arena(ctx, (size_t)raw_cap * 2, &raw));
     int64_t got[2] = {0, 0};
     for (int attempt = 0; attempt < 2; attempt++) {
         URH_LAUNCH(ctx, k_finish_rows, (unsigned)urh_div_up(ntiles, 256), 256, 0, tiles, staging, stage_cap, (const int32_t*)head_rel,
                    (const int32_t*)prev_cls, prev0, (const int64_t*)row_off, (const int64_t*)prev_fired, xprev, ntiles, sh.global_offset,
-                   sh.n_total, tol, is_ask ? 1 : 0, (int64_t)sps, sh.emit_tail, raw, raw_cap, d_small);
+                   sh.n_total, tol, is_ask ? 1 : 0, (int64_t)sps, sh.emit_tail, row_base, raw, raw_cap, d_small);
         if (sharded && attempt == 0) URH_TL_MARK(ctx, "rows written");
         URH_CHECK(urh_read_i64(ctx, d_small, 2, got));
         if (sharded) URH_CHECK(urh_p2p_check(ctx));   // a mailbox exchange of this step (or of the center chain before it) timed out?
         if (got[0] <= raw_cap) break;
-        if (attempt == 1) URH_FAIL(ctx, URH_ERR_CUDA, "finish_tiles: row buffer overflow after regrowth");
+        // rows_cap bounds a chained chunk's rows (one per candidate plus the tail), so only the unchained table can overflow
+        if (attempt == 1 || chain) URH_FAIL(ctx, URH_ERR_CUDA, "finish_tiles: row buffer overflow after regrowth");
         // more rows than guessed: grow and repeat stage D only
         if (is_ask) {
             URH_CHECK(urh_arena(ctx, (size_t)got[0] * 2, &raw));
@@ -367,25 +403,44 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
             raw_cap = (int64_t)ctx->pulses_cap_rows;
         }
     }
+    if (chain) URH_LAUNCH(ctx, k_chain_advance, 1, 1, 0, chain, (const RunCarry*)d_tot_run, (const CandAgg*)d_tot_cand, (const FireAgg*)d_tot_fire);
     int64_t K = got[0];
     if (is_ask && K > 0) {
-        URH_CHECK(urh_ensure_pulses(ctx, (size_t)K));
-        URH_CUDA(ctx, cudaMemsetAsync(ctx->pulses, 0, (size_t)K * 2 * sizeof(int64_t), ctx->stream));
+        if (!chain) URH_CHECK(urh_ensure_pulses(ctx, (size_t)K));
+        int64_t* out = ctx->pulses + 2 * row_base;
+        URH_CUDA(ctx, cudaMemsetAsync(out, 0, (size_t)K * 2 * sizeof(int64_t), ctx->stream));
         ScanMergeRows fm;
-        fm.raw = raw; fm.rows = K; fm.n_total = sh.n_total; fm.has_tail = (sh.emit_tail && K > got[1]) ? 1 : 0; fm.out = ctx->pulses;
+        fm.raw = raw; fm.rows = K; fm.n_total = sh.n_total; fm.has_tail = (sh.emit_tail && K > got[1]) ? 1 : 0; fm.out = out;
         fm.d_k = d_small;
+        fm.prev_last = (chain && row_base > 0) ? &chain->last_state : nullptr;
+        fm.row_base = row_base;
         URH_CHECK((urhts::scan<int64_t, AddI64, ScanMergeRows>(ctx, K, (int64_t)0, AddI64(), fm, (int64_t*)nullptr)));
         URH_CHECK(urh_read_i64(ctx, d_small, 1, &K));
+        if (chain) URH_LAUNCH(ctx, k_chain_last_row, 1, 1, 0, chain, (const int64_t*)ctx->pulses, row_base + K);
     }
-    ctx->pulses_k = K;
+    ctx->pulses_k = row_base + K;
     *k = K;
     return URH_OK;
+}
+
+// One chunk of a capture streamed through this GPU (digitize.cu): the same stages as a shard, with the three carries taken from
+// and folded into *chain (device memory) instead of exchanged between ranks.  *k = rows this chunk added to the pulse table
+// (a first row that continues the table's last row is merged into it).
+int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
+                     int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
+                     int64_t rows_cap, int64_t* k) {
+    FinishShard sh;
+    sh.rank = 0; sh.world = 1; sh.global_offset = global_offset; sh.n_total = n_total;
+    sh.emit_tail = (global_offset + n == n_total) ? 1 : 0;
+    sh.chain = chain; sh.row_base = row_base; sh.rows_cap = rows_cap;
+    return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
 }
 
 int urh_finish_local(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
                      int stage_cap, const int16_t* d_init, int64_t* k) {
     FinishShard sh;
     sh.rank = 0; sh.world = 1; sh.global_offset = 0; sh.n_total = n; sh.emit_tail = 1;
+    sh.chain = nullptr; sh.row_base = 0; sh.rows_cap = 0;
     return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
 }
 
@@ -397,5 +452,6 @@ int urh_finish_shard(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps
     FinishShard sh;
     sh.rank = ctx->nccl_rank; sh.world = ctx->nccl_world; sh.global_offset = global_offset; sh.n_total = n_total;
     sh.emit_tail = (ctx->nccl_rank == ctx->nccl_world - 1) ? 1 : 0;
+    sh.chain = nullptr; sh.row_base = 0; sh.rows_cap = 0;
     return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
 }

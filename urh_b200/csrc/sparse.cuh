@@ -28,6 +28,16 @@ struct RunCarryOp {
 };
 
 
+// Chunks of one capture digitized one after another on the same GPU (streaming, finish.cu): what the finish of chunk c needs from
+// the chunks before it, left in device memory by their finishes.  The same three totals a shard receives from its predecessors.
+struct __align__(16) UrhChain {
+    RunCarry run;          // the run that ends at the end of the preceding chunks (identity before chunk 0)
+    int64_t prev_fired;    // position of the last firing in the preceding chunks (-1: none)
+    int64_t last_state;    // state of the last row in the pulse table (ASK merge across the chunk edge)
+    int16_t prev_cls;      // class of the last candidate of the preceding chunks (chunk 0: the digitizer's initial state)
+    int16_t pad[7];
+};
+
 struct UrhCandidates {
     int64_t count;   // number of candidates (host copy)
     int64_t* pos;    // device: absolute sample index run_start + tolerance

@@ -1,5 +1,6 @@
 """CUDA drop-in for ``urh.cythonext.signal_functions`` (reference: src/urh/cythonext/signal_functions.pyx)."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -29,6 +30,46 @@ def _check_iq(samples):
     return samples
 
 
+# ---- captures larger than device memory -------------------------------------------------------------------------------
+# A host capture whose resident footprint exceeds the device budget goes through a ring of STREAM_RING device slots of
+# STREAM_CHUNK samples (urh_*_stream, DESIGN.md §4.11); the results are bit-identical.  Pinned host memory (PinnedArray) lets the
+# copies overlap the kernels; a pageable array or np.memmap works too, but then every copy blocks the calling thread.
+STREAM_CHUNK = 1 << 24
+STREAM_RING = 2
+
+
+def stream_footprint(n: int, dtype, tolerance: int, entry: int, chunk_samples: int = STREAM_CHUNK, ring: int = STREAM_RING,
+                     rows: int = -1) -> int:
+    """device bytes a streamed call (or, with _lib.STREAM_RESIDENT in entry, the resident call) needs; no device involved.
+    rows: pulse-table rows to budget for (-1: the bound no capture exceeds, -2: the resident call's up-front reservation)"""
+    out = C.c_int64(0)
+    rc = _lib.load_library().urh_stream_footprint(int(n), _lib.dtype_code(dtype) if dtype is not None else _lib.DT_F32, int(tolerance),
+                                                  int(chunk_samples), int(ring), int(entry), int(rows), C.byref(out))
+    if rc != _lib.URH_OK:
+        raise ValueError("urh_stream_footprint: invalid arguments")
+    return out.value
+
+
+def device_budget(ctx) -> int:
+    """free device memory less a margin; $URH_B200_DEVICE_BUDGET (bytes, read per call) lowers it"""
+    free, total = C.c_size_t(0), C.c_size_t(0)
+    ctx.check(ctx.lib.urh_mem_get_info(ctx.handle, C.byref(free), C.byref(total)))
+    budget = free.value - max(1 << 29, total.value // 32)
+    env = os.environ.get("URH_B200_DEVICE_BUDGET")
+    if env:
+        budget = min(budget, int(env))
+    return budget
+
+
+def use_stream(n: int, dtype, tolerance: int, entry: int, budget: int) -> bool:
+    """stream when the resident call's footprint (with the pulse rows it reserves up front, rows = -2) exceeds the budget"""
+    return stream_footprint(n, dtype, tolerance, entry | _lib.STREAM_RESIDENT, rows=-2) > budget
+
+
+def _host_ptr(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
 def afp_demod(samples, noise_mag: float, mod_type: str, mod_order: int, costas_loop_bandwidth: float = 0.1):
     """signal_functions.pyx:333-378.  Returns float32[n] (numpy for numpy input, DeviceArray for device input)."""
     samples = _check_iq(samples)
@@ -37,9 +78,15 @@ def afp_demod(samples, noise_mag: float, mod_type: str, mod_order: int, costas_l
     n = len(samples)
     if n == 0:
         return DeviceArray(ctx, (0,), np.float32) if on_device else np.zeros(0, dtype=np.float32)
+    code = _lib.demod_mod_code(mod_type)
+    if (not on_device and n > 2 and code in (_lib.MOD_ASK, _lib.MOD_FSK)
+            and use_stream(n, samples.dtype, 0, _lib.STREAM_AFP_DEMOD, device_budget(ctx))):
+        host = np.empty(n, dtype=np.float32)
+        ctx.check(ctx.lib.urh_afp_demod_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag), code,
+                                               STREAM_CHUNK, STREAM_RING, _host_ptr(host)))
+        return host
     d_iq = samples if on_device else to_device(samples, ctx)
     out = DeviceArray(ctx, (n,), np.float32)
-    code = _lib.demod_mod_code(mod_type)
     ctx.check(
         ctx.lib.urh_afp_demod(
             ctx.handle, C.c_void_p(d_iq.ptr), _lib.dtype_code(d_iq.dtype), n, float(noise_mag), code if code >= 0 else 99,
@@ -89,9 +136,14 @@ def grab_pulse_lens(samples, center: float, tolerance: int, modulation_type: str
     n = len(samples)
     if n == 0:
         return np.zeros((0, 2), dtype=np.int64)
-    d = samples if on_device else to_device(samples, ctx)
     k = C.c_int64(0)
     code = _lib.demod_mod_code(modulation_type)
+    if not on_device and use_stream(n, None, tolerance, _lib.STREAM_GRAB_PULSE_LENS, device_budget(ctx)):
+        ctx.check(ctx.lib.urh_grab_pulse_lens_stream(ctx.handle, _host_ptr(samples), 0, n, float(center), int(tolerance),
+                                                     code if code >= 0 else 99, int(samples_per_symbol), int(bits_per_symbol),
+                                                     float(center_spacing), STREAM_CHUNK, STREAM_RING, C.byref(k)))
+        return _fetch_pulses(ctx, k.value)
+    d = samples if on_device else to_device(samples, ctx)
     ctx.check(
         ctx.lib.urh_grab_pulse_lens(
             ctx.handle, C.c_void_p(d.ptr), n, float(center), int(tolerance), code if code >= 0 else 99,
@@ -111,10 +163,19 @@ def demod_digitize(samples, noise_mag: float, mod_type: str, center: float, tole
     n = len(samples)
     if n == 0:
         return (np.zeros(0, np.float32) if return_qad else None), np.zeros((0, 2), dtype=np.int64)
-    d_iq = samples if on_device else to_device(samples, ctx)
-    qad = DeviceArray(ctx, (n,), np.float32) if return_qad else None
     k = C.c_int64(0)
     code = _lib.demod_mod_code(mod_type)
+    entry = _lib.STREAM_DEMOD_DIGITIZE | (_lib.STREAM_QAD_OUT if return_qad else 0)
+    if (not on_device and n > 2 and code in (_lib.MOD_ASK, _lib.MOD_FSK)
+            and use_stream(n, samples.dtype, tolerance, entry, device_budget(ctx))):
+        host = np.empty(n, dtype=np.float32) if return_qad else None
+        ctx.check(ctx.lib.urh_demod_digitize_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag), code,
+                                                    float(center), int(tolerance), int(samples_per_symbol), int(bits_per_symbol),
+                                                    float(center_spacing), STREAM_CHUNK, STREAM_RING,
+                                                    _host_ptr(host) if host is not None else None, C.byref(k)))
+        return host, _fetch_pulses(ctx, k.value)
+    d_iq = samples if on_device else to_device(samples, ctx)
+    qad = DeviceArray(ctx, (n,), np.float32) if return_qad else None
     ctx.check(
         ctx.lib.urh_demod_digitize(
             ctx.handle, C.c_void_p(d_iq.ptr), _lib.dtype_code(d_iq.dtype), n, float(noise_mag), code if code >= 0 else 99,
@@ -154,6 +215,9 @@ def demod_center_digitize(samples, noise_mag: float, mod_type: str, tolerance: i
             ctx.check(ctx.lib.urh_demod_center_digitize(ctx.handle, C.c_void_p(d_iq.ptr), _lib.dtype_code(d_iq.dtype), n, float(noise_mag),
                                                         code, int(tolerance), int(samples_per_symbol), -1 if max_size is None else int(max_size),
                                                         C.c_void_p(qad.ptr), C.byref(center), C.byref(state), C.byref(k)))
+        elif scratch is None and use_stream(n, samples.dtype, tolerance, _lib.STREAM_DEMOD_CENTER_DIGITIZE, device_budget(ctx)):
+            return _demod_center_digitize_stream(ctx, samples, noise_mag, code, tolerance, samples_per_symbol, max_size, qad, return_qad,
+                                                 rows_out)
         else:
             host = np.ascontiguousarray(samples)
             d_iq = scratch if scratch is not None else DeviceArray(ctx, host.shape, host.dtype)
@@ -176,6 +240,38 @@ def demod_center_digitize(samples, noise_mag: float, mod_type: str, tolerance: i
     if return_qad:
         return center, rows, (qad if on_device else qad.get())
     return center, rows
+
+
+def _demod_center_digitize_stream(ctx, samples, noise_mag, code, tolerance, samples_per_symbol, max_size, qad, return_qad, rows_out):
+    """demod_center_digitize for a host capture that does not fit: IQ streamed, qad resident (and mirrored to the host with
+    return_qad).  A center the device must not decide (state 2) is finished stepwise from the resident qad and the demodulator's
+    tile table, as demod_detect_center would, with the digitizer streamed over the resident qad."""
+    from urh_b200.ainterpretation import AutoInterpretation as AI
+    n = len(samples)
+    host = np.empty(n, dtype=np.float32) if return_qad else None
+    center, state, kept, k = C.c_double(0.0), C.c_int(0), C.c_int64(0), C.c_int64(0)
+    ctx.check(ctx.lib.urh_demod_center_digitize_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag),
+                                                       code, int(tolerance), int(samples_per_symbol), -1 if max_size is None else int(max_size),
+                                                       STREAM_CHUNK, STREAM_RING, C.c_void_p(qad.ptr),
+                                                       _host_ptr(host) if host is not None else None, C.byref(center), C.byref(state),
+                                                       C.byref(kept), C.byref(k)))
+    if state.value == 2:
+        r0, r1 = AI.center_rank_window(kept.value, max_size)
+        w = np.zeros(5, dtype=np.float64)
+        ctx.check(ctx.lib.urh_center_window_stats(ctx.handle, C.c_void_p(qad.ptr), n, r0, r1, w.ctypes.data_as(C.c_void_p)))
+        st = AI.center_stats_from_window(kept.value, r0, r1, w)
+        c = AI._center_from_stats(ctx, qad, n, st, ctx.lib.urh_center_histogram_tiles)
+        rows = np.zeros((0, 2), dtype=np.int64)
+        if c is not None:
+            ctx.check(ctx.lib.urh_grab_pulse_lens_stream(ctx.handle, C.c_void_p(qad.ptr), 1, n, float(c), int(tolerance), code,
+                                                         int(samples_per_symbol), 1, 0.1, STREAM_CHUNK, STREAM_RING, C.byref(k)))
+            rows = _fetch_pulses(ctx, k.value, rows_out)
+    else:
+        c = float(center.value) if state.value == 1 else None
+        rows = _fetch_pulses(ctx, k.value, rows_out) if c is not None else np.zeros((0, 2), dtype=np.int64)
+    if return_qad:
+        return c, rows, host
+    return c, rows
 
 
 def ppseq_to_bits(ppseq, samples_per_symbol: int, bits_per_symbol: int = 1, write_bit_sample_pos: bool = True,

@@ -47,7 +47,9 @@ class ProtocolAnalyzer(object):
         self.messages = []
         if signal is None:
             return
-        qad = signal.qad_device if hasattr(signal, "qad_device") else signal.qad
+        qad = signal.qad_device if hasattr(signal, "qad_device") else None
+        if qad is None:   # no device copy (or one that would not fit): grab_pulse_lens streams the host qad when it must
+            qad = signal.qad
         ppseq = signal_functions.grab_pulse_lens(
             qad, signal.center, signal.tolerance, signal.modulation_type, signal.samples_per_symbol,
             signal.bits_per_symbol, signal.center_spacing)

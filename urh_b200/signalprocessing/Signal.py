@@ -13,7 +13,7 @@ import wave
 
 import numpy as np
 
-from .. import settings
+from .. import _lib, settings
 from ..ainterpretation import AutoInterpretation
 from ..cythonext import signal_functions
 from .Filter import Filter
@@ -251,11 +251,15 @@ class Signal(object):
     # ---- demodulation ---------------------------------------------------------------------------------------------------
     @property
     def qad_device(self):
-        """demodulated samples resident in HBM (DeviceArray); feeds grab_pulse_lens without another upload"""
+        """demodulated samples resident in HBM (DeviceArray); feeds grab_pulse_lens without another upload.  None when the
+        digitizer over a resident qad would not fit the device budget: grab_pulse_lens then streams the host qad."""
         q = self.qad  # demodulates on the GPU if necessary (and keeps the device copy)
         if self._qad_dev is None or len(self._qad_dev) != len(q):
             from ..device import to_device
 
+            if signal_functions.use_stream(len(q), None, self.tolerance, _lib.STREAM_GRAB_PULSE_LENS,
+                                           signal_functions.device_budget(_lib.default_context())):
+                return None
             self._qad_dev = to_device(np.ascontiguousarray(q, dtype=np.float32))
         return self._qad_dev
 
@@ -307,8 +311,25 @@ class Signal(object):
         return signal_functions.afp_demod(self.iq_array.device(), self.noise_threshold, self.modulation_type,
                                           self.modulation_order, self.costas_loop_bandwidth)
 
+    def _host_capture_too_large(self):
+        """the host capture when demodulating it resident would exceed the device budget and it can be streamed instead (ASK /
+        FSK; a capture already on the device fits), else None"""
+        iq = self.iq_array
+        if self.modulation_type not in ("ASK", "FSK") or iq._device is not None or len(iq) <= 2:
+            return None
+        host = iq._peek()
+        if not signal_functions.use_stream(len(host), host.dtype, 0, _lib.STREAM_AFP_DEMOD,
+                                           signal_functions.device_budget(_lib.default_context())):
+            return None
+        return host
+
     def quad_demod(self):
         if self.noise_threshold < self.max_magnitude:
+            host = self._host_capture_too_large()
+            if host is not None:   # streamed through the device: qad comes back to the host, nothing stays resident
+                self._qad_dev = None
+                return signal_functions.afp_demod(host, self.noise_threshold, self.modulation_type, self.modulation_order,
+                                                  self.costas_loop_bandwidth)
             self._qad_dev = self._quad_demod_device()
             return self._qad_dev.get()
         return np.zeros(2, dtype=np.float32)
