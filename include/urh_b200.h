@@ -386,6 +386,11 @@ int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3);
  * center (no histogram pass over qad) else 0, buckets of that histogram (0: not collected: sharded capture or
  * $URH_B200_CENTER_NO_CERTIFY), U - L summed over the two deciding bins}.  See DESIGN.md §4.4.1. */
 int urh_center_certify_stats(urh_ctx* ctx, int64_t* h_out3);
+/* speculative digitizing of the last urh_demod_center_digitize call (resident float32 FSK on one GPU): {tiles the demodulation
+ * pass digitized at its threshold guess, of those the tiles the qad digitizer did not read again (their margin proved the classes
+ * at the detected center, or the tile is silent), tiles it digitized again from qad}.  All zero when nothing was speculated:
+ * another dtype, modulation or entry point, or $URH_B200_NO_SPECULATE.  See DESIGN.md §4.4.1. */
+int urh_speculate_stats(urh_ctx* ctx, int64_t* h_out3);
 int64_t urh_costas_last_redone(urh_ctx* ctx);
 /* how the stitch pass of the last PSK demodulation resolved its super-chunks: {adopted from family A, adopted from family B,
  * chained by the stitch warp itself, segments per chunk}; super-chunk 0 of an unsharded capture is not counted.  The serial

@@ -158,6 +158,7 @@ SIGNATURES = {
     "urh_costas_shard_adopt": (i32, [vp, i32, vp]),
     "urh_costas_stats": (i32, [vp, vp]),
     "urh_center_certify_stats": (i32, [vp, vp]),
+    "urh_speculate_stats": (i32, [vp, vp]),
     "urh_costas_last_redone": (i64, [vp]),
     "urh_costas_stitch_stats": (i32, [vp, vp]),
     "urh_selftest_packed_div": (i32, [vp, C.c_uint64, i64, C.POINTER(i64), C.POINTER(i64)]),

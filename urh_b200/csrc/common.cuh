@@ -77,6 +77,7 @@ struct urh_ctx {
     int64_t center_n;
     void* center_prefix;  // tile rank prefix left by urh_afp_demod_stats for urh_center_histogram_tiles (arena)
     int64_t center_cert[3];  // urh_center_certify_stats of the last one-call step
+    int64_t spec_stats[3];   // urh_speculate_stats of the last one-call step
     void* nccl_comm;
     void* nccl_stage;
     void* nccl_hstage;  // pinned twin of nccl_stage

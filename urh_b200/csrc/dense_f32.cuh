@@ -37,6 +37,17 @@ struct SrcCenter {  // get_plateau_lengths: -1/1 around center (auto_interpretat
     template <typename T> __device__ __forceinline__ static bool above(T s, float thr0) { return !(s <= (T)thr0); }
 };
 
+// Speculative digitizing of the detect-center step (DESIGN.md §4.4.1): the demodulation pass digitized tiles [lo, hi) at the
+// guess *tg and left margin[t] = min over tile t of fl(|s - t_g|).  At the real threshold c a kept sample changes class only if it
+// lies in (t_g, c] or (c, t_g]; rounding is monotone, so then fl(|s - t_g|) <= fl(|c - t_g|).  margin[t] > fl(|c - t_g|) therefore
+// proves every class of tile t unchanged, and the summary and staging the pass wrote are exactly the ones this kernel would write.
+struct UrhSpec {
+    const float* tg;
+    float* margin;
+    int64_t lo, hi;          // lo == hi: nothing speculated
+    unsigned int* redone;    // speculated tiles that failed the proof and were digitized again
+};
+
 template <typename T> struct UrhVec2;
 template <> struct UrhVec2<float> { typedef float2 type; };
 template <> struct UrhVec2<double> { typedef double2 type; };
@@ -46,7 +57,7 @@ __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32)
 k_dense_f32(const T* __restrict__ x, int64_t n, int vec_in, const __grid_constant__ UrhClassify cls, int tol,
             UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
             int16_t* __restrict__ init_cls, int cls_of_zero, const float* __restrict__ d_thr0 = nullptr,
-            const UrhTileStats* __restrict__ tile_stats = nullptr) {
+            const UrhTileStats* __restrict__ tile_stats = nullptr, const UrhSpec spec = UrhSpec{}) {
     // d_thr0: the (binary) threshold lives in device memory (center detected on the device); then cls_of_zero is derived here
     const float thr0 = d_thr0 ? *d_thr0 : cls.thr[0];
     if (d_thr0) cls_of_zero = (0.0f <= thr0) ? 0 : 1;
@@ -65,6 +76,11 @@ k_dense_f32(const T* __restrict__ x, int64_t n, int vec_in, const __grid_constan
             if (tile_start == 0 && init_cls) *init_cls = (int16_t)-1;
         }
         return;
+    }
+    // the demodulation pass digitized the tile at the guess t_g: keep its result when the margin proves the classes (UrhSpec)
+    if (tile >= spec.lo && tile < spec.hi) {
+        if (spec.margin[tile] > fabsf(__fsub_rn(thr0, *spec.tg))) return;
+        if (lane == 0) atomicAdd(spec.redone, 1u);
     }
     UrhRunTracker rt;
     rt.init(tol, staging + tile * (int64_t)stage_cap);

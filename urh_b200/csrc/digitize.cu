@@ -144,15 +144,18 @@ k_fsk_fast(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
 }
 
 // The same kernel with the input staged through the shared-memory FIFO.
+// DIGITIZE and STATS: the speculative pass of the detect-center step; the threshold is the guess *d_thr0, margin[tile] its proof.
 #define URH_FSK_FIFO 3
 template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
 __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, (DT == URH_DT_F32) ? 5 : 4)   // (the integer variants spill at 48 registers)
 k_fsk_fifo(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
            float cls_noise, int tol, UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
-           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats, const UrhFine fine) {
+           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats, const UrhFine fine,
+           const float* __restrict__ d_thr0 = nullptr, float* __restrict__ margin = nullptr) {
     __shared__ __align__(16) unsigned char s_fifo[URH_WARPS_PER_BLOCK][URH_FSK_FIFO + 1][64 * 2 * sizeof(typename UrhElem<DT>::type)];
     extern __shared__ unsigned int s_fine[];   // [URH_FINE_NB] when STATS and fine.gh
     const bool fine_on = STATS && fine.gh;
+    if (DIGITIZE && STATS) thr0 = *d_thr0;
     const int lane = threadIdx.x & 31;
     const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
     const int64_t block_tile0 = tile_begin + (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK;
@@ -168,9 +171,77 @@ k_fsk_fifo(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
         urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS, URH_FSK_FIFO>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
                                                                     STATS ? tile_stats + tile : nullptr, fifo,
                                                                     DIGITIZE ? tiles + tile : nullptr, fine, fine_on ? s_fine : nullptr,
-                                                                    fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr);
+                                                                    fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr,
+                                                                    (DIGITIZE && STATS) ? margin + tile : nullptr);
     }
     if (fine_on) urh_fine_flush(fine, s_fine, block_tile0);
+}
+
+// Threshold guess t_g of the speculative detect-center step (float32 FSK captures, DESIGN.md §4.4.1).  One block demodulates
+// URH_GUESS_SAMPLES samples spread evenly over the capture (the same noise gate, plain atan2f), histograms the kept ones over
+// URH_GUESS_BINS bins spanning their [min, max], and takes the midpoint of the two most populated local maxima - the rule
+// k_center_pick applies to the capture's histogram.  The mean of the kept samples would not do: with one symbol dominating it sits
+// next to that symbol's level.  One peak: its bin; none: the middle of the range.  Only the step's speed depends on the guess.
+// forced != 0 replaces the guess by forced_tg ($URH_B200_SPECULATE_GUESS).  Also zeroes the redo counter.
+#define URH_GUESS_SAMPLES 16384
+#define URH_GUESS_BINS 128
+#define URH_GUESS_THREADS 1024
+__global__ void __launch_bounds__(URH_GUESS_THREADS) k_speculate_guess(const float2* __restrict__ iq, int64_t n, float noise_sqrd, int forced,
+                                                                      float forced_tg, float* __restrict__ d_tg, unsigned int* __restrict__ redone) {
+    constexpr int PER = URH_GUESS_SAMPLES / URH_GUESS_THREADS;
+    __shared__ unsigned int s_hist[URH_GUESS_BINS];
+    __shared__ float s_mn[32], s_mx[32];
+    if (forced) {
+        if (threadIdx.x == 0) { *d_tg = forced_tg; *redone = 0u; }
+        return;
+    }
+    for (int b = threadIdx.x; b < URH_GUESS_BINS; b += blockDim.x) s_hist[b] = 0u;
+    float v[PER];
+    float mn = INFINITY, mx = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < PER; k++) {
+        const int64_t i = 1 + (int64_t)(k * URH_GUESS_THREADS + threadIdx.x) * (n - 1) / URH_GUESS_SAMPLES;   // 1 .. n - 1
+        const float2 p = iq[i - 1], c = iq[i];
+        v[k] = NAN;   // gated
+        if (!(c.x * c.x + c.y * c.y <= noise_sqrd)) {
+            v[k] = atan2f(p.x * c.y - p.y * c.x, p.x * c.x + p.y * c.y);
+            mn = fminf(mn, v[k]);
+            mx = fmaxf(mx, v[k]);
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        mn = fminf(mn, __shfl_xor_sync(URH_FULL_MASK, mn, off));
+        mx = fmaxf(mx, __shfl_xor_sync(URH_FULL_MASK, mx, off));
+    }
+    if ((threadIdx.x & 31) == 0) { s_mn[threadIdx.x >> 5] = mn; s_mx[threadIdx.x >> 5] = mx; }
+    __syncthreads();
+    mn = INFINITY; mx = -INFINITY;
+    for (int w = 0; w < URH_GUESS_THREADS / 32; w++) { mn = fminf(mn, s_mn[w]); mx = fmaxf(mx, s_mx[w]); }
+    const float width = (mx - mn) / URH_GUESS_BINS;   // mn > mx (nothing kept) or width 0: no histogram
+    if (width > 0.0f) {
+#pragma unroll
+        for (int k = 0; k < PER; k++)
+            if (!isnan(v[k])) atomicAdd(&s_hist[min((int)((v[k] - mn) / width), URH_GUESS_BINS - 1)], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    *redone = 0u;
+    if (!(mn <= mx)) { *d_tg = 0.0f; return; }
+    if (!(width > 0.0f)) { *d_tg = mn; return; }
+    constexpr int WINDOW = (int)(0.05 * URH_GUESS_BINS) + 1;
+    int top[2] = {-1, -1};
+    for (int b = 0; b < URH_GUESS_BINS; b++) {
+        const unsigned int y = s_hist[b];
+        bool peak = y > 0u;
+        for (int d = 1; d < WINDOW && peak; d++)
+            peak = y > (b + d < URH_GUESS_BINS ? s_hist[b + d] : 0u) && y > (b - d >= 0 ? s_hist[b - d] : 0u);
+        if (!peak) continue;
+        if (top[0] < 0 || y > s_hist[top[0]]) { top[1] = top[0]; top[0] = b; }
+        else if (top[1] < 0 || y > s_hist[top[1]]) top[1] = b;
+    }
+    if (top[0] < 0) *d_tg = 0.5f * (mn + mx);
+    else if (top[1] < 0) *d_tg = mn + ((float)top[0] + 0.5f) * width;
+    else *d_tg = mn + (0.5f * (float)(top[0] + top[1]) + 0.5f) * width;
 }
 
 // =====================================================================================================
@@ -223,12 +294,14 @@ static bool iq_vec_aligned(const void* p, int dtype) { return ((uintptr_t)p % (2
 
 // tile_lo / tile_hi: restrict the pass to tiles [tile_lo, tile_hi) (chunked ingest: a chunk is demodulated as soon as its
 // upload has landed); tile_hi < 0 = all tiles.
+// spec != NULL (float32 FSK, tile statistics, no DIG): the fast kernel's tiles are also digitized at the guess spec->tg into
+// tiles / staging (tol, stage_cap), with their margins; spec->lo / hi is set to that tile range (UrhSpec).
 template <int DT, int MOD, bool DIG>
 static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const UrhDemodParams& dp, float* d_qad,
                              const UrhClassify& cls, int tol, UrhTileSummary* tiles, uint32_t* staging,
                              int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
                              UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
-                             const UrhFine& fine = UrhFine{}) {
+                             const UrhFine& fine = UrhFine{}, UrhSpec* spec = nullptr) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     const size_t fine_smem = fine.gh ? (size_t)URH_FINE_NB * sizeof(unsigned int) : 0;
     if (tile_hi < 0 || tile_hi > ntiles) tile_hi = ntiles;
@@ -256,7 +329,18 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
             // the variant that stages its input through the shared-memory FIFO (URH_B200_FSK_NO_FIFO selects the register-fed loop)
             static const bool fifo = getenv("URH_B200_FSK_NO_FIFO") == nullptr;
             const bool ff = fifo;
-            if (tile_stats && d_qad && !DIG) {
+            bool speculated = false;
+            if constexpr (DT == URH_DT_F32 && MOD == URH_MOD_FSK && !DIG) {
+                if (spec && ff && tile_stats && d_qad) {
+                    URH_LAUNCH(ctx, (k_fsk_fifo<DT, true, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, 0.0f, dp.noise_value,
+                               tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine, (const float*)spec->tg, spec->margin);
+                    spec->lo = fb;
+                    spec->hi = fe;
+                    speculated = true;
+                }
+            }
+            if (speculated) {
+            } else if (tile_stats && d_qad && !DIG) {
                 if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
                                    tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
                 else URH_LAUNCH(ctx, (k_fsk_fast<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
@@ -287,13 +371,13 @@ static int launch_dense_iq_m(urh_ctx* ctx, int dtype, const void* d_iq, int64_t 
                              float* d_qad, const UrhClassify& cls, int tol, UrhTileSummary* tiles,
                              uint32_t* staging, int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
                              UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
-                             const UrhFine& fine = UrhFine{}) {
+                             const UrhFine& fine = UrhFine{}, UrhSpec* spec = nullptr) {
     switch (dtype) {
         case URH_DT_I8: return launch_dense_iq_t<URH_DT_I8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
         case URH_DT_U8: return launch_dense_iq_t<URH_DT_U8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
         case URH_DT_I16: return launch_dense_iq_t<URH_DT_I16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
         case URH_DT_U16: return launch_dense_iq_t<URH_DT_U16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
-        case URH_DT_F32: return launch_dense_iq_t<URH_DT_F32, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
+        case URH_DT_F32: return launch_dense_iq_t<URH_DT_F32, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine, spec);
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     }
 }
@@ -973,6 +1057,35 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
                                                                ts, fine);
                              }, true));
     }
+    // the digitizer's tables, filled by the qad digitizer after the center chain, and by the speculative pass before it
+    cls.noise_value = urh_noise_value(mod_type);
+    cls.order = 2;
+    const int tol = tolerance;
+    const int cap = stage_cap_for(tol);
+    UrhTileSummary* tiles = nullptr;
+    uint32_t* staging = nullptr;
+    int16_t* d_init = nullptr;
+    if (!sc) {
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
+        URH_CHECK(urh_arena(ctx, 8, &d_init));
+    }
+    // speculative digitizing (UrhSpec, DESIGN.md §4.4.1): the pass digitizes its fast tiles at a guessed threshold, the qad digitizer
+    // re-reads only the tiles whose margin does not prove the classes at the detected center.  The resident single-GPU float32 FSK
+    // step only; $URH_B200_NO_SPECULATE=1 turns it off, $URH_B200_SPECULATE_GUESS=<float> replaces the guess (read per call).
+    const bool speculate = !sharded && !h_iq && !sc && mod_type == URH_MOD_FSK && dtype == URH_DT_F32 &&
+                           getenv("URH_B200_NO_SPECULATE") == nullptr;
+    UrhSpec spec = {};
+    if (speculate) {
+        float* tg;
+        URH_CHECK(urh_arena(ctx, 1, &tg));
+        URH_CHECK(urh_arena(ctx, 1, &spec.redone));
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &spec.margin));
+        spec.tg = tg;
+        const char* forced = getenv("URH_B200_SPECULATE_GUESS");
+        URH_LAUNCH(ctx, k_speculate_guess, 1, URH_GUESS_THREADS, 0, (const float2*)d_iq, n, dp.noise_sqrd, forced ? 1 : 0,
+                   forced ? strtof(forced, nullptr) : 0.0f, tg, spec.redone);
+    }
     int chunk_no = 0;
     for (int64_t t0 = 0; t0 < (sc ? 0 : ntiles); t0 += chunk_tiles, chunk_no++) {
         const int64_t t1 = (t0 + chunk_tiles < ntiles) ? t0 + chunk_tiles : ntiles;
@@ -987,7 +1100,8 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
         if (mod_type == URH_MOD_ASK)
             URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1, fine)));
         else
-            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1, fine)));
+            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, nullptr, 0, has_halo,
+                                                             ts, t0, t1, fine, speculate ? &spec : nullptr)));
     }
     CenterPlan* plan = nullptr;
     URH_CHECK(urh_center_chain(ctx, d_qad_out, n, ts, max_size, sharded ? ctx->nccl_rank : 0, sharded ? ctx->nccl_world : 1,
@@ -997,9 +1111,6 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     const int* d_state;
     urh_center_plan_result(ctx, plan, &d_centerf, &d_center, &d_state);
     // digitizer pass over qad, threshold read from device memory
-    cls.noise_value = urh_noise_value(mod_type);
-    cls.order = 2;
-    const int tol = tolerance;
     int64_t rows = 0;
     if (sc) {
         URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1023,20 +1134,15 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
         }
         *sc->kept = ctx->h_mail[45];
     } else {
-        const int cap = stage_cap_for(tol);
-        UrhTileSummary* tiles;
-        uint32_t* staging;
-        int16_t* d_init;
-        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-        URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-        URH_CHECK(urh_arena(ctx, 8, &d_init));
         URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
         const int vec_in = (((uintptr_t)d_qad_out % 8) == 0) ? 1 : 0;
         URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK), URH_WARPS_PER_BLOCK * 32, 0,
-                   (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts);
+                   (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts, spec);
         URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
+        ctx->h_mail[46] = 0;
+        if (speculate) URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 46, spec.redone, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
         if (sharded)
             URH_CHECK(urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, &rows));
         else
@@ -1050,11 +1156,20 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     ctx->center_cert[0] = ctx->h_mail[42];
     ctx->center_cert[1] = fine.gh ? URH_FINE_NB : 0;
     ctx->center_cert[2] = ctx->h_mail[44];
+    const int64_t redone = (spec.hi > spec.lo) ? ctx->h_mail[46] : 0;
+    ctx->spec_stats[0] = spec.hi - spec.lo;
+    ctx->spec_stats[1] = spec.hi - spec.lo - redone;
+    ctx->spec_stats[2] = redone;
     if (st != 1) {
         ctx->pulses_k = 0;
         rows = 0;
     }
     *k = rows;
+    return URH_OK;
+}
+
+extern "C" int urh_speculate_stats(urh_ctx* ctx, int64_t* h_out3) {
+    for (int i = 0; i < 3; i++) h_out3[i] = ctx->spec_stats[i];
     return URH_OK;
 }
 
