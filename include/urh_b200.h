@@ -257,7 +257,8 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
 /* ---- streaming: host captures of any size through a ring of `ring` (2..8) device slots of chunk_samples each (digitize.cu,
  * DESIGN.md §4.11).  chunk_samples <= 0: 2^24; it is rounded down to a multiple of 2048 (at least 2048).  Host buffers may be pinned
  * (urh_host_alloc: copies overlap the kernels) or pageable, e.g. a memory-mapped file (correct, but each copy then blocks the host).
- * Results are bit-identical to the resident entry points named below.  ASK / FSK only; PSK raises URH_ERR_INVALID.
+ * Results are bit-identical to the resident entry points named below.  ASK / FSK only; PSK raises URH_ERR_INVALID (PSK has entry
+ * points of its own, below).
  * urh_afp_demod_stream: afp_demod (signal_functions.pyx:333-378) from host IQ into host qad h_qad[n].
  * urh_grab_pulse_lens_stream: grab_pulse_lens (signal_functions.pyx:392-495) of qad[n], any bits_per_symbol; qad_on_device != 0: qad
  *   is a device buffer (only the digitizer's work arrays are chunked).  Rows as urh_grab_pulse_lens (urh_fetch_pulses).
@@ -267,8 +268,15 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
  *   226-277, + grab_pulse_lens) with the IQ streamed and qad resident in d_qad_out[n]; h_qad_out (may be NULL) mirrors it to the host.
  *   center_state as urh_demod_center_digitize; on state 2 the tables of urh_center_window_stats / urh_center_histogram_tiles are
  *   left for d_qad_out, and *kept = the number of kept samples (the input of the stepwise detect_center).
+ * urh_afp_demod_psk_stream: urh_afp_demod(..., URH_MOD_PSK, mod_order, costas_loop_bandwidth, ...) from host IQ into host qad h_qad[n].
+ *   The Costas loop runs chunk by chunk, each chunk continued from the loop state the preceding one left on the device.
+ * urh_demod_digitize_psk_stream: urh_demod_digitize for PSK (the Costas loop of order 1 << bits_per_symbol at loop bandwidth 0.1, then
+ *   grab_pulse_lens) with the Costas loop streamed as above and the digitizer run on each chunk's qad; h_qad_out (may be NULL)
+ *   receives qad.  After either PSK call urh_costas_stats / urh_costas_stitch_stats hold sums over its chunks.
  * urh_stream_footprint: device bytes a call needs, callable without a device.  entry = URH_STREAM_ENTRY_* | URH_STREAM_* flags;
- *   URH_STREAM_RESIDENT gives the resident entry's bytes for the same capture instead.  rows: the pulse-table rows to budget for
+ *   URH_STREAM_RESIDENT gives the resident entry's bytes for the same capture instead.  PSK (AFP_DEMOD and DEMOD_DIGITIZE entries):
+ *   URH_STREAM_PSK for a Costas loop of order 2 (also a bound for orders 1 and 3, which run the serial kernel), with
+ *   URH_STREAM_PSK4 for order 4 or more.  rows: the pulse-table rows to budget for
  *   (-1: the bound n / (tolerance + 1) + 3 that no capture exceeds; -2: the n / 64 + 1024 rows the resident call reserves up front).
  * urh_stream_schedule: the order in which a call issues its copies and chunk computations, 6 int64 per op {kind (0 upload into
  *   the slot, 1 compute, 2 download from the slot), chunk, slot, first sample, end sample, 1 if the upload carries the halo sample
@@ -284,6 +292,8 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
 #define URH_STREAM_QAD_OUT 0x10       /* demod_digitize: qad also goes to the host */
 #define URH_STREAM_RESIDENT 0x20      /* footprint of the resident entry point */
 #define URH_STREAM_QAD_ON_DEVICE 0x40 /* grab_pulse_lens: qad is already on the device */
+#define URH_STREAM_PSK 0x80           /* the PSK entry points (Costas loop of order 2) */
+#define URH_STREAM_PSK4 0x100         /* with URH_STREAM_PSK: Costas loop of order 4 */
 #define URH_STREAM_UPLOAD 1
 #define URH_STREAM_DOWNLOAD 2
 #define URH_STREAM_HALO 4
@@ -298,6 +308,11 @@ int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t
 int urh_demod_center_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type,
                                      uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size, int64_t chunk_samples, int ring,
                                      float* d_qad_out, float* h_qad_out, double* center, int* center_state, int64_t* kept, int64_t* k);
+int urh_afp_demod_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_order,
+                             float costas_loop_bandwidth, int64_t chunk_samples, int ring, float* h_qad);
+int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, float center, uint16_t tolerance,
+                                  uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing, int64_t chunk_samples,
+                                  int ring, float* h_qad_out, int64_t* k);
 int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows, int64_t* bytes);
 int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
 int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3);
@@ -380,7 +395,8 @@ int urh_set_profiling(urh_ctx* ctx, int enabled);
  * read) returns the milliseconds from the first mark to each mark and the '\n'-separated names; *count = number of marks (<= 32). */
 int urh_timeline_fetch(urh_ctx* ctx, float* h_ms, char* h_names, int names_cap, int* count);
 int urh_last_dense_ms(urh_ctx* ctx, float* ms);
-/* speculative Costas loop diagnostics of the last PSK demodulation: {chunks matched in O(1), chunks walked, samples stepped serially} */
+/* speculative Costas loop diagnostics of the last PSK demodulation: {chunks matched in O(1), chunks walked, samples stepped serially}
+ * (after a streamed PSK call: sums over its ring chunks) */
 int urh_costas_stats(urh_ctx* ctx, int64_t* h_out3);
 /* certificate of the last urh_demod_center_digitize(_host) call: {1 if the fine histogram of the demodulation pass decided the
  * center (no histogram pass over qad) else 0, buckets of that histogram (0: not collected: sharded capture or
@@ -394,7 +410,9 @@ int urh_speculate_stats(urh_ctx* ctx, int64_t* h_out3);
 int64_t urh_costas_last_redone(urh_ctx* ctx);
 /* how the stitch pass of the last PSK demodulation resolved its super-chunks: {adopted from family A, adopted from family B,
  * chained by the stitch warp itself, segments per chunk}; super-chunk 0 of an unsharded capture is not counted.  The serial
- * kernel (captures shorter than 8192 samples) zeroes these and urh_costas_stats and reports segs = 0.
+ * kernel (captures shorter than 8192 samples) zeroes these and urh_costas_stats and reports segs = 0.  After a streamed PSK call
+ * (urh_*_psk_stream) the counters are sums over its ring chunks (each ring chunk's super-chunk 0 not counted; chunks that ran the
+ * serial kernel add nothing) and segs is the layout of the first ring chunk that took the speculative path (0: none did).
  * $URH_B200_COSTAS_SEGS = 2, 4, 8 or 16 forces the speculative path's chunk layout (the result does not depend on it). */
 int urh_costas_stitch_stats(urh_ctx* ctx, int64_t* h_out4);
 /* paired (float2) division used by the FSK fast path vs __fdiv_rn on `count` random operand pairs */

@@ -21,6 +21,7 @@ MOD_ASK, MOD_FSK, MOD_PSK, MOD_QAM, MOD_GFSK, MOD_OQPSK = 0, 1, 2, 3, 4, 5
 # streamed entry points (include/urh_b200.h)
 STREAM_AFP_DEMOD, STREAM_GRAB_PULSE_LENS, STREAM_DEMOD_DIGITIZE, STREAM_DEMOD_CENTER_DIGITIZE = 0, 1, 2, 3
 STREAM_QAD_OUT, STREAM_RESIDENT, STREAM_QAD_ON_DEVICE = 0x10, 0x20, 0x40
+STREAM_PSK, STREAM_PSK4 = 0x80, 0x100
 STREAM_UPLOAD, STREAM_DOWNLOAD, STREAM_HALO = 1, 2, 4
 
 _DTYPE_CODE = {
@@ -175,6 +176,8 @@ SIGNATURES = {
     "urh_demod_digitize_stream": (i32, [vp, vp, i32, i64, f32, i32, f32, u16, u32, u8, f32, i64, i32, vp, C.POINTER(i64)]),
     "urh_demod_center_digitize_stream": (i32, [vp, vp, i32, i64, f32, i32, u16, u32, i64, i64, i32, vp, vp, C.POINTER(C.c_double),
                                                C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
+    "urh_afp_demod_psk_stream": (i32, [vp, vp, i32, i64, f32, i32, f32, i64, i32, vp]),
+    "urh_demod_digitize_psk_stream": (i32, [vp, vp, i32, i64, f32, f32, u16, u32, u8, f32, i64, i32, vp, C.POINTER(i64)]),
     "urh_stream_footprint": (i32, [i64, i32, i32, i64, i32, i32, i64, C.POINTER(i64)]),
     "urh_stream_schedule": (i32, [i64, i64, i32, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_stats": (i32, [vp, vp]),

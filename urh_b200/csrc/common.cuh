@@ -169,6 +169,19 @@ void urh_stream_sample_free(urh_ctx* ctx);
 void urh_release_mod_plans(urh_ctx* ctx);  // modulation.cu
 int urh_ensure_stage(urh_ctx* ctx, size_t bytes);
 
+// Costas loop of a streamed PSK capture across its ring chunks (costas_spec.cu; arena memory taken before the chunks' mark):
+// two {freq, phase} state slots, the summed stitch counters, the chunk layout of the first speculative chunk (0: none)
+struct UrhCostasStream {
+    float* state;
+    int64_t* acc;
+    int segs;
+};
+int urh_costas_stream_begin(urh_ctx* ctx, UrhCostasStream* S);
+int urh_costas_stream_chunk(urh_ctx* ctx, UrhCostasStream* S, int64_t c, const void* d_iq, int dtype, int64_t n, float noise_sqrd,
+                            int loop_order, float bandwidth, float* d_out);
+int urh_costas_stream_end(urh_ctx* ctx, const UrhCostasStream* S);
+int64_t urh_costas_arena_bytes(int64_t n, int loop_order);
+
 // read back `count` int64 scalars from device (synchronises the ctx stream)
 int urh_read_i64(urh_ctx* ctx, const int64_t* d_src, int count, int64_t* h_out);
 

@@ -17,9 +17,12 @@ struct CostasParams {
     int order;
 };
 
+// st_in (NULL: the loop's initial state {0, 1.5}) / st_out: {freq, phase} before / after the n samples on the device (the ring chunks
+// of a streamed capture carry the state this way); cap_start: sample 0 is the capture's first (the reference skips it)
 template <int DT>
 __global__ void __launch_bounds__(32) k_costas(const void* __restrict__ iq, int64_t n, CostasParams P,
-                                               float* __restrict__ out, int write_first) {
+                                               float* __restrict__ out, int write_first, const float* __restrict__ st_in,
+                                               float* __restrict__ st_out, int cap_start) {
     __shared__ float s_re[2][COSTAS_CHUNK];
     __shared__ float s_im[2][COSTAS_CHUNK];
     __shared__ float s_out[2][COSTAS_CHUNK];
@@ -27,6 +30,10 @@ __global__ void __launch_bounds__(32) k_costas(const void* __restrict__ iq, int6
     const E* p = (const E*)iq;
     const int lane = threadIdx.x;
     float freq = 0.0f, phase = 1.5f;
+    if (st_in) {
+        freq = st_in[0];
+        phase = st_in[1];
+    }
     const double two_pi_d = 2 * M_PI;  // the reference compares/adjusts the float phase in double
     const int64_t nchunks = (n + COSTAS_CHUNK - 1) / COSTAS_CHUNK;
 
@@ -51,7 +58,7 @@ __global__ void __launch_bounds__(32) k_costas(const void* __restrict__ iq, int6
         const int len = (int)((n - base) < COSTAS_CHUNK ? (n - base) : COSTAS_CHUNK);
         if (lane == 0) {
             for (int j = 0; j < len; j++) {
-                if (base + j == 0) continue;  // the reference loop starts at i = 1 (pyx:289)
+                if (cap_start && base + j == 0) continue;  // the reference loop starts at i = 1 (pyx:289)
                 const float re = s_re[buf][j], im = s_im[buf][j];
                 if (__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im)) <= P.noise_sqrd) {
                     s_out[buf][j] = -4.0f;
@@ -108,15 +115,20 @@ __global__ void __launch_bounds__(32) k_costas(const void* __restrict__ iq, int6
         }
         __syncwarp();
         for (int j = lane; j < len; j += 32) {
-            if (base + j == 0 && !write_first) continue;
-            out[base + j] = (base + j == 0) ? 0.0f : s_out[buf][j];
+            const bool first = cap_start && base + j == 0;
+            if (first && !write_first) continue;
+            out[base + j] = first ? 0.0f : s_out[buf][j];
         }
         __syncwarp();
+    }
+    if (lane == 0 && st_out) {
+        st_out[0] = freq;
+        st_out[1] = phase;
     }
 }
 
 int urh_costas_demod_serial(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float noise_sqrd, int loop_order,
-                            float bandwidth, float* d_out) {
+                            float bandwidth, float* d_out, const float* d_st_in, float* d_st_out, int cap_start) {
     // signal_functions.pyx:252-287
     CostasParams P;
     const float damping = (float)(sqrt(2.0) / 2.0);
@@ -144,11 +156,11 @@ int urh_costas_demod_serial(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n
     for (int i = 0; i < 4; i++) ctx->costas_stitch[i] = 0;
     // result[0] is uninitialised in the reference (np.empty, pyx:265); we define it as 0.
     switch (dtype) {
-        case URH_DT_I8: URH_LAUNCH(ctx, k_costas<URH_DT_I8>, 1, 32, 0, d_iq, n, P, d_out, 1); break;
-        case URH_DT_U8: URH_LAUNCH(ctx, k_costas<URH_DT_U8>, 1, 32, 0, d_iq, n, P, d_out, 1); break;
-        case URH_DT_I16: URH_LAUNCH(ctx, k_costas<URH_DT_I16>, 1, 32, 0, d_iq, n, P, d_out, 1); break;
-        case URH_DT_U16: URH_LAUNCH(ctx, k_costas<URH_DT_U16>, 1, 32, 0, d_iq, n, P, d_out, 1); break;
-        default: URH_LAUNCH(ctx, k_costas<URH_DT_F32>, 1, 32, 0, d_iq, n, P, d_out, 1); break;
+        case URH_DT_I8: URH_LAUNCH(ctx, k_costas<URH_DT_I8>, 1, 32, 0, d_iq, n, P, d_out, 1, d_st_in, d_st_out, cap_start); break;
+        case URH_DT_U8: URH_LAUNCH(ctx, k_costas<URH_DT_U8>, 1, 32, 0, d_iq, n, P, d_out, 1, d_st_in, d_st_out, cap_start); break;
+        case URH_DT_I16: URH_LAUNCH(ctx, k_costas<URH_DT_I16>, 1, 32, 0, d_iq, n, P, d_out, 1, d_st_in, d_st_out, cap_start); break;
+        case URH_DT_U16: URH_LAUNCH(ctx, k_costas<URH_DT_U16>, 1, 32, 0, d_iq, n, P, d_out, 1, d_st_in, d_st_out, cap_start); break;
+        default: URH_LAUNCH(ctx, k_costas<URH_DT_F32>, 1, 32, 0, d_iq, n, P, d_out, 1, d_st_in, d_st_out, cap_start); break;
     }
     return URH_OK;
 }

@@ -26,6 +26,14 @@
 #define CS_WARM 1024
 #define CS_MAXBR 4
 #define CS_STATS 6              // per stitch hypothesis: {O(1) chunks, walked chunks, samples stepped, self-chained, A, B}
+// How a run starts (the `start` argument of the kernels below):
+//   CS_EXACT  the true incoming loop state is known: chunk 0 has one exact run (from *st0, or the loop's initial {0, 1.5} when
+//             st0 is NULL) and super-chunk 0 one chain;
+//   CS_CAP    sample 0 is the capture's first sample: result[0] is not computed (written as 0) and warm-ups clip at index 1.
+// A resident capture (and the first shard of a sharded one) has both, later shards neither, and the ring chunks c > 0 of a streamed
+// capture only CS_EXACT: their incoming state is the preceding chunk's end state, left on the device.
+#define CS_EXACT 1
+#define CS_CAP 2
 
 struct CsParams {
     float noise_sqrd, alpha, beta, scale, shift;
@@ -117,7 +125,8 @@ __device__ __forceinline__ int cs_run(const void* iq, int64_t a, int64_t b, CsSt
 template <int DT>
 __global__ void __launch_bounds__(128) k_cs_speculate(const void* __restrict__ iq, int64_t n, CsParams P, int64_t nchunks,
                                                       float* __restrict__ cand, CsState* __restrict__ ckpt,
-                                                      int* __restrict__ nonnoise, int* __restrict__ chunk_cnt, int first_shard) {
+                                                      int* __restrict__ nonnoise, int* __restrict__ chunk_cnt, int start,
+                                                      const CsState* __restrict__ st0) {
     const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int k = blockIdx.y;
     if (c >= nchunks) return;
@@ -130,13 +139,16 @@ __global__ void __launch_bounds__(128) k_cs_speculate(const void* __restrict__ i
     s.phase = (float)(1.5 + (double)k * (2.0 * M_PI / (double)P.order));
     if ((double)s.phase > 2.0 * M_PI) s.phase = (float)((double)s.phase - 2.0 * M_PI);
     float o;
-    if (c == 0 && first_shard) {
-        if (k != 0) return;  // chunk 0 of the capture starts from the true initial state: one exact run only
-        s.phase = 1.5f;
+    if (c == 0 && (start & CS_EXACT)) {
+        if (k != 0) return;  // chunk 0 starts from the true incoming state: one exact run only
+        if (st0) s = *st0;
+        else s.phase = 1.5f;
     } else {
-        // later shards of a sharded capture have CS_WARM halo samples stored in front of iq (negative indices)
+        // later shards of a sharded capture have CS_WARM halo samples stored in front of iq (negative indices); an exact start
+        // has none and clips the warm-up at its first sample
         int64_t w0 = p0 - CS_WARM;
-        if (first_shard && w0 < 1) w0 = 1;
+        const int64_t lo = (start & CS_CAP) ? 1 : 0;
+        if ((start & CS_EXACT) && w0 < lo) w0 = lo;
         cs_run<DT, false>(iq, w0, p0, s, P, nullptr, 0);
     }
     ck[0] = s;
@@ -144,7 +156,7 @@ __global__ void __launch_bounds__(128) k_cs_speculate(const void* __restrict__ i
     for (int j = 0; j < P.segs; j++) {
         const int64_t a = p0 + (int64_t)j * CS_SEG;
         int64_t a0 = a;
-        if (a0 == 0 && first_shard) { out[0] = 0.0f; a0 = 1; }  // the reference loop starts at i = 1 (result[0] undefined -> 0)
+        if (a0 == 0 && (start & CS_CAP)) { out[0] = 0.0f; a0 = 1; }  // the reference loop starts at i = 1 (result[0] undefined -> 0)
         const int64_t b0 = min(a + (int64_t)CS_SEG, n);
         const int cnt = cs_run<DT, true>(iq, a0, b0, s, P, out, 0);
         ck[j + 1] = s;
@@ -179,7 +191,7 @@ struct CsTables {
 template <int DT>
 __device__ CsState cs_chain(const void* __restrict__ iq, int64_t n, const CsParams& P, int64_t nchunks, int nbr,
                             const CsState* __restrict__ ckpt, const int* __restrict__ nonnoise, const int* __restrict__ chunk_cnt,
-                            uint8_t* __restrict__ src, CsState* __restrict__ segst, int first_shard, int64_t lo, int64_t hi, CsState st,
+                            uint8_t* __restrict__ src, CsState* __restrict__ segst, int cap_start, int64_t lo, int64_t hi, CsState st,
                             int64_t* acc) {
     const int lane = threadIdx.x & 31;
     int64_t fast = 0, slow = 0, stepped = 0;
@@ -250,12 +262,12 @@ __device__ CsState cs_chain(const void* __restrict__ iq, int64_t n, const CsPara
                 for (int g = 0; g < CS_SEG / 32; g++) {
                     const int64_t i = a + g * 32 + lane;
                     sre[g] = 0.f; sim[g] = 0.f;
-                    if (i < n && !(i == 0 && first_shard)) cs_load<DT>(iq, i, sre[g], sim[g]);
+                    if (i < n && !(i == 0 && cap_start)) cs_load<DT>(iq, i, sre[g], sim[g]);
                 }
 #pragma unroll
                 for (int g = 0; g < CS_SEG / 32; g++) {
                     const int64_t i = a + g * 32 + lane;
-                    const bool live = (i < n && !(i == 0 && first_shard)) &&
+                    const bool live = (i < n && !(i == 0 && cap_start)) &&
                                       !(__fadd_rn(__fmul_rn(sre[g], sre[g]), __fmul_rn(sim[g], sim[g])) <= P.noise_sqrd);
                     smask[g] = __ballot_sync(URH_FULL_MASK, live);
                 }
@@ -307,7 +319,7 @@ __device__ CsState cs_chain(const void* __restrict__ iq, int64_t n, const CsPara
 template <int DT>
 __global__ void __launch_bounds__(128) k_cs_chains(const void* __restrict__ iq, int64_t n, CsParams P, int64_t nchunks, int nbr,
                                                   const CsState* __restrict__ ckpt, const int* __restrict__ nonnoise,
-                                                  const int* __restrict__ chunk_cnt, CsTables T, int first_shard, int64_t nsuper,
+                                                  const int* __restrict__ chunk_cnt, CsTables T, int start, int64_t nsuper,
                                                   int family, const int64_t* __restrict__ prev_live, const CsState* __restrict__ end_a,
                                                   CsState* __restrict__ sup_end, int64_t* __restrict__ sup_acc) {
     const int lane = threadIdx.x & 31;
@@ -322,8 +334,8 @@ __global__ void __launch_bounds__(128) k_cs_chains(const void* __restrict__ iq, 
     uint8_t* src = T.src + (int64_t)(family * nbr + k) * T.nseg;
     CsState* segst = T.segst + (int64_t)(family * nbr + k) * T.nseg;
     if (family == 0) {
-        if (w == 0 && first_shard) {
-            // the capture's first chunk is the one exact run (candidate 0 started from the loop's true initial state)
+        if (w == 0 && (start & CS_EXACT)) {
+            // the run's first chunk is the one exact run (candidate 0 started from the true incoming state)
             if (k != 0) {
                 if (lane == 0) sup_end[w * nbr + k].freq = sup_end[w * nbr + k].phase = __int_as_float(0x7fc00000);
                 return;
@@ -336,13 +348,13 @@ __global__ void __launch_bounds__(128) k_cs_chains(const void* __restrict__ iq, 
         }
     } else {
         const int64_t p = prev_live[w];
-        if (p < 0 || (p == 0 && first_shard && k != 0)) {   // nothing to inherit (family A of super-chunk 0 has one chain only)
+        if (p < 0 || (p == 0 && (start & CS_EXACT) && k != 0)) {   // nothing to inherit (family A of super-chunk 0 has one chain only)
             if (lane == 0) sup_end[w * nbr + k].freq = sup_end[w * nbr + k].phase = __int_as_float(0x7fc00000);
             return;
         }
         st = end_a[p * nbr + k];
     }
-    st = cs_chain<DT>(iq, n, P, nchunks, nbr, ckpt, nonnoise, chunk_cnt, src, segst, first_shard, lo, hi, st, acc);
+    st = cs_chain<DT>(iq, n, P, nchunks, nbr, ckpt, nonnoise, chunk_cnt, src, segst, start & CS_CAP, lo, hi, st, acc);
     if (lane == 0) {
         sup_end[w * nbr + k] = st;
         sup_acc[(w * nbr + k) * 3 + 0] = acc[0];
@@ -373,14 +385,16 @@ __global__ void k_cs_prev_live(const int64_t* __restrict__ live, int64_t nsuper,
 template <int DT>
 __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, int64_t n, CsParams P, int64_t nchunks, int nbr,
                                                   const CsState* __restrict__ ckpt, const int* __restrict__ nonnoise,
-                                                  const int* __restrict__ chunk_cnt, CsTables T, int first_shard, int64_t nsuper,
+                                                  const int* __restrict__ chunk_cnt, CsTables T, int start, int64_t nsuper,
                                                   const int64_t* __restrict__ prev_live, const CsState* __restrict__ end_a,
                                                   const CsState* __restrict__ end_b, const int64_t* __restrict__ acc_a,
                                                   const int64_t* __restrict__ acc_b, uint8_t* __restrict__ chosen,
-                                                  int64_t* __restrict__ stats, CsState st_in, CsState* __restrict__ st_out, int hyp_mode) {
+                                                  int64_t* __restrict__ stats, CsState st_in, CsState* __restrict__ st_out, int hyp_mode,
+                                                  int accumulate) {
     // hyp_mode (later shards of a sharded capture): block h hops under the HYPOTHESIS that the shard starts in candidate h's
     // start state (true whenever the preceding shard ends locked); each hypothesis has its own chosen[] row, counters, end
     // state and self-run table, so all of them run concurrently and independently of the preceding shard.
+    // accumulate: add the counters to stats[] instead of overwriting them (the ring chunks of a streamed capture sum them).
     const int lane = threadIdx.x;
     const int h = blockIdx.x;
     chosen += (int64_t)h * nsuper;
@@ -392,7 +406,7 @@ __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, i
     CsState st = st_in;
     if (hyp_mode) st = ckpt[((int64_t)h * nchunks) * (P.segs + 1)];
     int64_t w = 0;
-    if (first_shard) {
+    if (start & CS_EXACT) {
         if (lane == 0) chosen[0] = 0;
         st = end_a[0];
         for (int q = 0; q < 3; q++) acc[q] += acc_a[q];
@@ -431,17 +445,13 @@ __global__ void __launch_bounds__(32) k_cs_stitch(const void* __restrict__ iq, i
             if (lane == 0) chosen[w] = (uint8_t)self_family;
             redone++;
             st = cs_chain<DT>(iq, n, P, nchunks, nbr, ckpt, nonnoise, chunk_cnt, T.src + (int64_t)self_family * T.nseg,
-                              T.segst + (int64_t)self_family * T.nseg, first_shard, lo, min(nchunks, lo + T.sup), st, acc);
+                              T.segst + (int64_t)self_family * T.nseg, start & CS_CAP, lo, min(nchunks, lo + T.sup), st, acc);
         }
     }
     if (lane == 0 && st_out) *st_out = st;
     if (lane == 0 && stats) {
-        stats[0] = acc[0];
-        stats[1] = acc[1];
-        stats[2] = acc[2];
-        stats[3] = redone;
-        stats[4] = adopted_a;
-        stats[5] = adopted_b;
+        const int64_t v[CS_STATS] = {acc[0], acc[1], acc[2], redone, adopted_a, adopted_b};
+        for (int q = 0; q < CS_STATS; q++) stats[q] = (accumulate ? stats[q] : 0) + v[q];
     }
 }
 
@@ -460,7 +470,7 @@ __global__ void k_cs_assemble(const float* __restrict__ cand, int64_t n, CsTable
 // pass 4: the stepped segments (one warp each): recompute the samples from the recorded state
 template <int DT>
 __global__ void __launch_bounds__(128) k_cs_fix(const void* __restrict__ iq, int64_t n, CsParams P, CsTables T, const uint8_t* __restrict__ chosen,
-                                               int first_shard, float* __restrict__ out) {
+                                               int cap_start, float* __restrict__ out) {
     const int lane = threadIdx.x & 31;
     const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t seg = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; seg < T.nseg; seg += nw) {
@@ -473,11 +483,11 @@ __global__ void __launch_bounds__(128) k_cs_fix(const void* __restrict__ iq, int
             const int64_t i = a + g * 32 + lane;
             float re = 0.f, im = 0.f;
             bool live = false;
-            if (i < n && !(i == 0 && first_shard)) {
+            if (i < n && !(i == 0 && cap_start)) {
                 cs_load<DT>(iq, i, re, im);
                 live = !(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im)) <= P.noise_sqrd);
                 if (!live) out[i] = -4.0f;
-            } else if (i == 0 && first_shard) {
+            } else if (i == 0 && cap_start) {
                 out[0] = 0.0f;
             }
             unsigned mask = __ballot_sync(URH_FULL_MASK, live);
@@ -496,7 +506,8 @@ __global__ void __launch_bounds__(128) k_cs_fix(const void* __restrict__ iq, int
 }
 
 int urh_costas_demod_serial(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float noise_sqrd, int loop_order,
-                            float bandwidth, float* d_out);  // costas.cu
+                            float bandwidth, float* d_out, const float* d_st_in = nullptr, float* d_st_out = nullptr,
+                            int cap_start = 1);  // costas.cu
 
 static int cs_params(urh_ctx* ctx, CsParams* P, int dtype, float noise_sqrd, int order, float bandwidth) {
     const float damping = (float)(sqrt(2.0) / 2.0);
@@ -523,7 +534,9 @@ static int cs_params(urh_ctx* ctx, CsParams* P, int dtype, float noise_sqrd, int
 struct CsRun {
     CsParams P;
     const void* iq;
-    int dtype, nbr, first_shard;
+    int dtype, nbr, start;   // start: CS_EXACT | CS_CAP
+    const CsState* st0 = nullptr;   // exact start: the incoming state on the device (NULL: the loop's initial state)
+    int accumulate = 0;             // the stitch adds its counters to stats[] (streamed chunks); cs_finish does not read them
     int64_t n, nchunks;
     float* cand;
     CsState* ckpt;
@@ -551,8 +564,8 @@ struct CsRun {
         default: URH_LAUNCH(ctx, KERNEL<URH_DT_F32>, __VA_ARGS__); break;              \
     }
 
+// the caller resets the arena (or releases a mark) before: every table below is a fresh arena request
 static int cs_speculate(urh_ctx* ctx, CsRun& R) {
-    urh_arena_reset(ctx);
     // enough independent chains to fill the GPU: shrink the chunk for short captures (more warm-up overhead)
     int segs = 16;
     while (segs > 2 && (R.n / (segs * CS_SEG)) * R.P.order < (int64_t)ctx->sm_count * 1024) segs >>= 1;
@@ -573,7 +586,7 @@ static int cs_speculate(urh_ctx* ctx, CsRun& R) {
     R.T.sup = (int)max((int64_t)CS_SUP_MIN, urh_div_up((int64_t)131072, (int64_t)R.P.chunk));
     R.nsuper = urh_div_up(R.nchunks, R.T.sup);
     // table families: nbr x A, nbr x B, then one self-run table per stitch hypothesis (a single one when unsharded)
-    const int self_tables = R.first_shard ? 1 : R.nbr;
+    const int self_tables = (R.start & CS_EXACT) ? 1 : R.nbr;
     URH_CHECK(urh_arena(ctx, (size_t)(2 * R.nbr + self_tables) * R.T.nseg, &R.T.src));
     URH_CHECK(urh_arena(ctx, (size_t)(2 * R.nbr + self_tables) * R.T.nseg, &R.T.segst));
     URH_CHECK(urh_arena(ctx, (size_t)2 * R.nsuper * R.nbr, &R.sup_end));
@@ -586,16 +599,16 @@ static int cs_speculate(urh_ctx* ctx, CsRun& R) {
     URH_CHECK(urh_arena(ctx, (size_t)2 * self_tables, &R.st_out));
     R.adopted = 0;
     const dim3 grid((unsigned)urh_div_up(R.nchunks, 128), (unsigned)R.nbr);
-    CS_DISPATCH(R, k_cs_speculate, grid, 128, 0, R.iq, R.n, R.P, R.nchunks, R.cand, R.ckpt, R.nonnoise, R.chunk_cnt, R.first_shard);
+    CS_DISPATCH(R, k_cs_speculate, grid, 128, 0, R.iq, R.n, R.P, R.nchunks, R.cand, R.ckpt, R.nonnoise, R.chunk_cnt, R.start, R.st0);
     // pass 2a: the chains of every super-chunk under every assumption (independent of the true incoming state)
     const int64_t per = R.nsuper * R.nbr;
     URH_CUDA(ctx, cudaMemsetAsync(R.sup_acc, 0, (size_t)2 * per * 3 * sizeof(int64_t), ctx->stream));
     URH_LAUNCH(ctx, k_cs_live, (unsigned)urh_div_up(R.nsuper, 128), 128, 0, R.chunk_cnt, R.nchunks, R.nsuper, R.T.sup, R.live);
     URH_LAUNCH(ctx, k_cs_prev_live, 1, 32, 0, (const int64_t*)R.live, R.nsuper, R.prev_live);
     const unsigned gc = (unsigned)urh_div_up(per * 32, 128);
-    CS_DISPATCH(R, k_cs_chains, gc, 128, 0, R.iq, R.n, R.P, R.nchunks, R.nbr, R.ckpt, R.nonnoise, R.chunk_cnt, R.T, R.first_shard, R.nsuper, 0,
+    CS_DISPATCH(R, k_cs_chains, gc, 128, 0, R.iq, R.n, R.P, R.nchunks, R.nbr, R.ckpt, R.nonnoise, R.chunk_cnt, R.T, R.start, R.nsuper, 0,
                 (const int64_t*)R.prev_live, (const CsState*)R.sup_end, R.sup_end, R.sup_acc);
-    CS_DISPATCH(R, k_cs_chains, gc, 128, 0, R.iq, R.n, R.P, R.nchunks, R.nbr, R.ckpt, R.nonnoise, R.chunk_cnt, R.T, R.first_shard, R.nsuper, 1,
+    CS_DISPATCH(R, k_cs_chains, gc, 128, 0, R.iq, R.n, R.P, R.nchunks, R.nbr, R.ckpt, R.nonnoise, R.chunk_cnt, R.T, R.start, R.nsuper, 1,
                 (const int64_t*)R.prev_live, (const CsState*)R.sup_end, R.sup_end + per, R.sup_acc + per * 3);
     return URH_OK;
 }
@@ -606,7 +619,8 @@ static int cs_finish(urh_ctx* ctx, CsRun& R, float* h_state_out) {
     const unsigned ga = (unsigned)min(urh_div_up(R.n, 256), (int64_t)ctx->sm_count * 32);
     URH_LAUNCH(ctx, k_cs_assemble, ga, 256, 0, R.cand, R.n, R.T, R.P.segs, chosen, R.out);
     CS_DISPATCH(R, k_cs_fix, (unsigned)min(urh_div_up(R.T.nseg * 32, 128), (int64_t)ctx->sm_count * 16), 128, 0, R.iq, R.n, R.P, R.T, chosen,
-                R.first_shard, R.out);
+                R.start & CS_CAP, R.out);
+    if (R.accumulate) return URH_OK;   // streamed: the counters stay on the device until urh_costas_stream_end
     int64_t st6[CS_STATS];
     URH_CHECK(urh_read_i64(ctx, R.stats + CS_STATS * R.adopted, CS_STATS, st6));
     for (int i = 0; i < 3; i++) ctx->costas_stats[i] = st6[i];
@@ -625,8 +639,9 @@ static int cs_finish(urh_ctx* ctx, CsRun& R, float* h_state_out) {
 static int cs_stitch(urh_ctx* ctx, CsRun& R, CsState st_in, int hypotheses) {
     const int64_t per = R.nsuper * R.nbr;
     CS_DISPATCH(R, k_cs_stitch, hypotheses > 0 ? hypotheses : 1, 32, 0, R.iq, R.n, R.P, R.nchunks, R.nbr, R.ckpt, R.nonnoise, R.chunk_cnt, R.T,
-                R.first_shard, R.nsuper, (const int64_t*)R.prev_live, (const CsState*)R.sup_end, (const CsState*)(R.sup_end + per),
-                (const int64_t*)R.sup_acc, (const int64_t*)(R.sup_acc + per * 3), R.chosen, R.stats, st_in, R.st_out, hypotheses > 0 ? 1 : 0);
+                R.start, R.nsuper, (const int64_t*)R.prev_live, (const CsState*)R.sup_end, (const CsState*)(R.sup_end + per),
+                (const int64_t*)R.sup_acc, (const int64_t*)(R.sup_acc + per * 3), R.chosen, R.stats, st_in, R.st_out, hypotheses > 0 ? 1 : 0,
+                R.accumulate);
     return URH_OK;
 }
 
@@ -643,11 +658,92 @@ int urh_costas_demod(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float
         return urh_costas_demod_serial(ctx, d_iq, dtype, n, noise_sqrd, loop_order, bandwidth, d_out);
     CsRun R;
     URH_CHECK(cs_params(ctx, &R.P, dtype, noise_sqrd, order, bandwidth));
-    R.iq = d_iq; R.dtype = dtype; R.n = n; R.first_shard = 1; R.out = d_out;
+    R.iq = d_iq; R.dtype = dtype; R.n = n; R.start = CS_EXACT | CS_CAP; R.out = d_out;
+    urh_arena_reset(ctx);
     URH_CHECK(cs_speculate(ctx, R));
     CsState none;
     none.freq = 0.f; none.phase = 1.5f;
     return cs_resolve(ctx, R, none, nullptr);
+}
+
+// Device bytes cs_speculate requests for n samples at loop order `order` (0 for the serial kernel), the largest over the chunk
+// layouts: $URH_B200_COSTAS_SEGS may force any of them.  Exact start (one self-run table).  urh_stream_footprint's PSK term.
+int64_t urh_costas_arena_bytes(int64_t n, int loop_order) {
+    const int order = loop_order > 4 ? 4 : loop_order;
+    if (n < 4 * 512 * 4 || (order != 2 && order != 4)) return 0;
+    auto r = [](int64_t b) { return b > 0 ? (b + 255) & ~(int64_t)255 : (int64_t)256; };
+    int64_t most = 0;
+    for (int segs = 2; segs <= CS_MAX_SEGS; segs <<= 1) {
+        const int64_t chunk = (int64_t)segs * CS_SEG, nchunks = urh_div_up(n, chunk), nseg = nchunks * segs;
+        const int64_t sup = max((int64_t)CS_SUP_MIN, urh_div_up((int64_t)131072, chunk)), nsuper = urh_div_up(nchunks, sup);
+        const int64_t nbr = order, fam = 2 * nbr + 1;
+        const int64_t b = r(nbr * n * 4) + r(nbr * nchunks * (segs + 1) * (int64_t)sizeof(CsState)) + r(nseg * 4) + r(fam * nseg) +
+                          r(fam * nseg * (int64_t)sizeof(CsState)) + r(2 * nsuper * nbr * (int64_t)sizeof(CsState)) +
+                          r(2 * nsuper * nbr * 3 * 8) + 2 * r(nsuper * 8) + r(nsuper) + r(nchunks * 4) + r(CS_STATS * 8) +
+                          r(2 * (int64_t)sizeof(CsState));
+        most = b > most ? b : most;
+    }
+    return most;
+}
+
+// ---- PSK captures streamed through a ring of device slots (digitize.cu, DESIGN.md §4.3) --------------------------------------------
+// The ring chunks run one after the other on the compute stream, so the exact loop state at every chunk edge is on the device when
+// the next chunk starts: chunk c > 0 is an exact start (no capture start), its incoming state the one chunk c - 1 left.  Chunk c reads
+// state slot c & 1 and writes slot (c + 1) & 1.  The stitch counters add up in S->acc; nothing is read back per chunk.
+__global__ void k_cs_stream_init(CsState* st, int64_t* acc) {
+    if (threadIdx.x == 0) {
+        st[0].freq = 0.0f;
+        st[0].phase = 1.5f;
+    }
+    if (threadIdx.x < CS_STATS) acc[threadIdx.x] = 0;
+}
+
+int urh_costas_stream_begin(urh_ctx* ctx, UrhCostasStream* S) {
+    CsState* st;
+    URH_CHECK(urh_arena(ctx, 2, &st));
+    URH_CHECK(urh_arena(ctx, CS_STATS, &S->acc));
+    S->state = (float*)st;
+    S->segs = 0;
+    URH_LAUNCH(ctx, k_cs_stream_init, 1, 32, 0, st, S->acc);
+    return URH_OK;
+}
+
+// ring chunk c: n samples at d_iq (the chunk's first sample at index 0) -> d_out[n]; enqueued only
+int urh_costas_stream_chunk(urh_ctx* ctx, UrhCostasStream* S, int64_t c, const void* d_iq, int dtype, int64_t n, float noise_sqrd,
+                            int loop_order, float bandwidth, float* d_out) {
+    CsState* st = (CsState*)S->state;
+    CsState* st_in = st + (c & 1);
+    CsState* st_out = st + ((c + 1) & 1);
+    const int order = loop_order > 4 ? 4 : loop_order;
+    if (n < 4 * 512 * 4 || (order != 2 && order != 4))
+        return urh_costas_demod_serial(ctx, d_iq, dtype, n, noise_sqrd, loop_order, bandwidth, d_out, (const float*)st_in, (float*)st_out,
+                                       c == 0);
+    CsRun R;
+    URH_CHECK(cs_params(ctx, &R.P, dtype, noise_sqrd, order, bandwidth));
+    R.iq = d_iq; R.dtype = dtype; R.n = n; R.start = CS_EXACT | (c == 0 ? CS_CAP : 0); R.st0 = st_in; R.out = d_out;
+    URH_CHECK(cs_speculate(ctx, R));
+    R.stats = S->acc;
+    R.st_out = st_out;
+    R.accumulate = 1;
+    if (S->segs == 0) S->segs = R.P.segs;
+    CsState none;
+    none.freq = 0.f; none.phase = 1.5f;   // unused: an exact start takes its state from st0
+    URH_CHECK(cs_stitch(ctx, R, none, 0));
+    R.adopted = 0;
+    return cs_finish(ctx, R, nullptr);
+}
+
+// after the last chunk: the summed counters become urh_costas_stats / urh_costas_stitch_stats (one read-back per call)
+int urh_costas_stream_end(urh_ctx* ctx, const UrhCostasStream* S) {
+    int64_t st6[CS_STATS];
+    URH_CHECK(urh_read_i64(ctx, S->acc, CS_STATS, st6));
+    for (int i = 0; i < 3; i++) ctx->costas_stats[i] = st6[i];
+    ctx->costas_redone = st6[3];
+    ctx->costas_stitch[0] = st6[4];
+    ctx->costas_stitch[1] = st6[5];
+    ctx->costas_stitch[2] = st6[3];
+    ctx->costas_stitch[3] = S->segs;
+    return URH_OK;
 }
 
 // ---- PSK captures sharded over GPUs: pass 1 runs concurrently on every rank, the chain is handed from rank to rank ----
@@ -666,7 +762,10 @@ extern "C" int urh_costas_shard_speculate(urh_ctx* ctx, const void* d_iq, int dt
     volatile float sq = nm * nm;
     CsRun& R = g_shard_run;
     URH_CHECK(cs_params(ctx, &R.P, dtype, sq, order, bandwidth));
-    R.iq = d_iq; R.dtype = dtype; R.n = n; R.first_shard = first_shard ? 1 : 0; R.out = d_out;
+    R.iq = d_iq; R.dtype = dtype; R.n = n; R.start = first_shard ? (CS_EXACT | CS_CAP) : 0; R.out = d_out;
+    R.st0 = nullptr;
+    R.accumulate = 0;
+    urh_arena_reset(ctx);
     return cs_speculate(ctx, R);
 }
 
@@ -682,16 +781,17 @@ extern "C" int urh_costas_shard_resolve(urh_ctx* ctx, const float* h_state_in, f
 // The first shard has one true run: h_out[0] = {initial state, end state}.  Returns the number of hypotheses in *count.
 extern "C" int urh_costas_shard_hypotheses(urh_ctx* ctx, float* h_out, int* count) {
     CsRun& R = g_shard_run;
-    const int nh = R.first_shard ? 1 : R.nbr;
+    const bool first_shard = R.start & CS_EXACT;
+    const int nh = first_shard ? 1 : R.nbr;
     CsState none;
     none.freq = 0.f; none.phase = 1.5f;
-    URH_CHECK(cs_stitch(ctx, R, none, R.first_shard ? 0 : nh));
+    URH_CHECK(cs_stitch(ctx, R, none, first_shard ? 0 : nh));
     CsState ends[4], starts[4];
     URH_CUDA(ctx, cudaMemcpyAsync(ends, R.st_out, sizeof(CsState) * nh, cudaMemcpyDeviceToHost, ctx->stream));
-    for (int h = 0; h < nh && !R.first_shard; h++)
+    for (int h = 0; h < nh && !first_shard; h++)
         URH_CUDA(ctx, cudaMemcpyAsync(&starts[h], R.ckpt + ((int64_t)h * R.nchunks) * (R.P.segs + 1), sizeof(CsState), cudaMemcpyDeviceToHost, ctx->stream));
     URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (R.first_shard) starts[0] = none;
+    if (first_shard) starts[0] = none;
     for (int h = 0; h < nh; h++) {
         h_out[4 * h + 0] = starts[h].freq; h_out[4 * h + 1] = starts[h].phase;
         h_out[4 * h + 2] = ends[h].freq; h_out[4 * h + 3] = ends[h].phase;
@@ -703,7 +803,7 @@ extern "C" int urh_costas_shard_hypotheses(urh_ctx* ctx, float* h_out, int* coun
 // Adopt hypothesis h (its start state equalled, bit for bit, the preceding shard's end state): assemble + fix.
 extern "C" int urh_costas_shard_adopt(urh_ctx* ctx, int h, float* h_state_out) {
     CsRun& R = g_shard_run;
-    if (h < 0 || h >= (R.first_shard ? 1 : R.nbr)) URH_FAIL(ctx, URH_ERR_INVALID, "costas_shard_adopt: no such hypothesis");
+    if (h < 0 || h >= ((R.start & CS_EXACT) ? 1 : R.nbr)) URH_FAIL(ctx, URH_ERR_INVALID, "costas_shard_adopt: no such hypothesis");
     R.adopted = h;
     return cs_finish(ctx, R, h_state_out);
 }

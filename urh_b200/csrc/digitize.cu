@@ -696,9 +696,14 @@ static int64_t finish_arena_bytes(int64_t tiles, int64_t rows_cap, bool ask) {
     return r256(tiles * (int64_t)sizeof(RunCarry)) + 2 * r256(tiles * 4) + 2 * r256(tiles * 8) + r256((32 + 8) * 8) +
            (ask ? r256(rows_cap * 16) : 0);
 }
+// loop order of a PSK footprint entry (0: not PSK)
+static int psk_order_of(int entry) { return (entry & URH_STREAM_PSK) ? ((entry & URH_STREAM_PSK4) ? 4 : 2) : 0; }
+static int psk_entry_flags(int mod_order) { return URH_STREAM_PSK | (mod_order >= 4 ? URH_STREAM_PSK4 : 0); }
+
 static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_samples, int ring, int entry) {
     StreamSizes z;
     const int kind = entry & 0xf;
+    const int psk = psk_order_of(entry);
     const bool resident = entry & URH_STREAM_RESIDENT;
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     z.cs = resident ? ntiles * URH_TILE : stream_chunk_samples(n, chunk_samples);
@@ -714,7 +719,9 @@ static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_sam
     } else {
         z.src_slot = (kind == URH_STREAM_ENTRY_GRAB_PULSE_LENS && (entry & URH_STREAM_QAD_ON_DEVICE)) ? 0
                      : URH_STREAM_PAD + z.cs * (iq ? urh_iq_bytes(dtype) : 4);
-        const bool qad_ring = kind == URH_STREAM_ENTRY_AFP_DEMOD || (kind == URH_STREAM_ENTRY_DEMOD_DIGITIZE && (entry & URH_STREAM_QAD_OUT));
+        // PSK digitizing reads each chunk's qad from a device slot, downloaded or not
+        const bool qad_ring = kind == URH_STREAM_ENTRY_AFP_DEMOD ||
+                              (kind == URH_STREAM_ENTRY_DEMOD_DIGITIZE && ((entry & URH_STREAM_QAD_OUT) || psk));
         z.qad_slot = qad_ring ? z.cs * 4 : 0;
         z.ring_bytes = ring * (r256(z.src_slot) + r256(z.qad_slot));
         if (kind == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) z.ring_bytes += r256(n * 4);   // resident qad (the caller's buffer)
@@ -723,6 +730,8 @@ static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_sam
     z.scan_items = ct > z.rows_chunk ? ct : z.rows_chunk;
     if (digitize) z.arena += r256(ct * (int64_t)sizeof(UrhTileSummary)) + r256(ct * cap * 4) + r256(16) + r256(sizeof(UrhChain)) +
                              finish_arena_bytes(ct, z.rows_chunk, true);
+    // the Costas loop's tables for one chunk, the state slots and the summed counters (costas_spec.cu)
+    if (psk && !resident) z.arena += urh_costas_arena_bytes(z.cs, psk) + r256(16) + r256(6 * 8);
     if (kind == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) {   // tile statistics, fine histogram, center chain (center.cu)
         z.arena += r256(ntiles * (int64_t)sizeof(UrhTileStats)) + r256((int64_t)URH_FINE_SLABS * URH_FINE_NB * 4) + r256((ntiles + 1) * 8) +
                    ((int64_t)2 << 20);
@@ -736,6 +745,8 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
     if (!bytes || n < 0 || tolerance < 0 || tolerance > 0xffff || (entry & 0xf) > URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) return URH_ERR_INVALID;
     if (!(entry & URH_STREAM_RESIDENT) && (ring < 2 || ring > URH_STREAM_MAX_RING)) return URH_ERR_INVALID;
     if ((entry & 0xf) != URH_STREAM_ENTRY_GRAB_PULSE_LENS && urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
+    if ((entry & URH_STREAM_PSK) && (entry & 0xf) != URH_STREAM_ENTRY_AFP_DEMOD && (entry & 0xf) != URH_STREAM_ENTRY_DEMOD_DIGITIZE)
+        return URH_ERR_INVALID;
     const StreamSizes z = stream_sizes(n, dtype, tolerance, chunk_samples, ring, entry);
     const bool digitize = (entry & 0xf) != URH_STREAM_ENTRY_AFP_DEMOD;
     // rows -1: the bound no capture exceeds; -2: what the resident finish reserves up front (finish.cu: n / 64 + 1024)
@@ -749,6 +760,8 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
                  finish_arena_bytes(ntiles, r + r / 4, true) + 16 * (r + r / 4);
         if ((entry & 0xf) == URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE)
             b += r256(ntiles * (int64_t)sizeof(UrhTileStats)) + r256((int64_t)URH_FINE_SLABS * URH_FINE_NB * 4) + r256((ntiles + 1) * 8);
+        // PSK: the Costas loop's candidates, checkpoints and chain tables over the whole capture (cs_speculate)
+        if (psk_order_of(entry)) b += urh_costas_arena_bytes(n, psk_order_of(entry));
         *bytes = b;
         return URH_OK;
     }
@@ -889,6 +902,15 @@ struct StreamDigitizer {
         return URH_OK;
     }
 };
+
+static int stream_check(urh_ctx* ctx, int64_t n, int ring, int mod_type, int dtype, bool iq);
+// the PSK entries: the IQ is streamed, the Costas loop of chunk c continues from the state chunk c - 1 left on the device
+static int psk_stream_check(urh_ctx* ctx, int64_t n, int ring, int dtype) {
+    URH_CHECK(stream_check(ctx, n, ring, URH_MOD_PSK, dtype, false));
+    if (n <= 2) URH_FAIL(ctx, URH_ERR_INVALID, "streamed PSK demodulation: n > 2");
+    if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
+    return URH_OK;
+}
 
 static int stream_check(urh_ctx* ctx, int64_t n, int ring, int mod_type, int dtype, bool iq) {
     if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "streamed call: empty capture");
@@ -1302,6 +1324,67 @@ extern "C" int urh_demod_center_digitize_stream(urh_ctx* ctx, const void* h_iq, 
     sc.ring = ring; sc.chunk_samples = chunk_samples; sc.h_iq = h_iq; sc.h_qad = h_qad_out; sc.kept = kept;
     return demod_center_digitize_impl(ctx, nullptr, dtype, n, 0, noise_mag, mod_type, tolerance, samples_per_symbol, max_size, d_qad_out,
                                       false, 0, n, center, center_state, k, nullptr, 0, &sc);
+}
+
+// PSK: the Costas loop per chunk (costas_spec.cu, DESIGN.md §4.3), no halo; its tables take the arena above the chunk mark.
+extern "C" int urh_afp_demod_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_order,
+                                        float costas_loop_bandwidth, int64_t chunk_samples, int ring, float* h_qad) {
+    if (!h_iq || !h_qad) return URH_ERR_INVALID;
+    URH_CHECK(psk_stream_check(ctx, n, ring, dtype));
+    urh_arena_reset(ctx);
+    const StreamSizes z = stream_sizes(n, dtype, 0, chunk_samples, ring, URH_STREAM_ENTRY_AFP_DEMOD | psk_entry_flags(mod_order));
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, z.ring_bytes));
+    const int64_t slot = r256(z.src_slot);
+    char* d_src = R.mem;
+    float* d_qad = (float*)(R.mem + ring * slot);
+    const UrhDemodParams dp = make_demod_params(noise_mag, URH_MOD_PSK, dtype);
+    UrhCostasStream cs;
+    URH_CHECK(urh_costas_stream_begin(ctx, &cs));
+    const UrhArenaMark mark = urh_arena_mark(ctx);
+    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, d_src, slot, h_qad, d_qad,
+                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
+                             urh_arena_release(ctx, mark);
+                             return urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, s1 - s0, dp.noise_sqrd,
+                                                            mod_order, costas_loop_bandwidth, d_qad + s * z.cs);
+                         }));
+    return urh_costas_stream_end(ctx, &cs);
+}
+
+extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, float center,
+                                             uint16_t tolerance, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
+                                             int64_t chunk_samples, int ring, float* h_qad_out, int64_t* k) {
+    if (!k || !h_iq) return URH_ERR_INVALID;
+    *k = 0;
+    ctx->pulses_k = 0;
+    URH_CHECK(psk_stream_check(ctx, n, ring, dtype));
+    urh_arena_reset(ctx);
+    UrhClassify cls;
+    URH_CHECK(fill_classify(ctx, &cls, URH_MOD_PSK, center, bits_per_symbol, center_spacing));
+    const int mod_order = 1 << bits_per_symbol;   // as urh_demod_digitize: afp_demod(..., 1 << bits_per_symbol, 0.1)
+    const UrhDemodParams dp = make_demod_params(noise_mag, URH_MOD_PSK, dtype);
+    const StreamSizes z = stream_sizes(n, dtype, tolerance, chunk_samples, ring,
+                                       URH_STREAM_ENTRY_DEMOD_DIGITIZE | (h_qad_out ? URH_STREAM_QAD_OUT : 0) | psk_entry_flags(mod_order));
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, z.ring_bytes));
+    const int64_t slot = r256(z.src_slot);
+    char* d_src = R.mem;
+    float* d_qad = (float*)(R.mem + ring * slot);
+    UrhCostasStream cs;
+    URH_CHECK(urh_costas_stream_begin(ctx, &cs));
+    StreamDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, false, samples_per_symbol));
+    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, d_src, slot, h_qad_out, d_qad,
+                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
+                             urh_arena_release(ctx, dz.mark);
+                             float* q = d_qad + s * z.cs;
+                             URH_CHECK(urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, s1 - s0, dp.noise_sqrd,
+                                                               mod_order, 0.1f, q));
+                             URH_CHECK(stream_dense_qad(ctx, q, s0, s1, cls, dz));
+                             return dz.finish(ctx, s0, s1);
+                         }));
+    *k = dz.rows;
+    return urh_costas_stream_end(ctx, &cs);
 }
 
 struct UrhShardState {

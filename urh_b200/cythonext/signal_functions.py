@@ -36,6 +36,14 @@ def _check_iq(samples):
 # copies overlap the kernels; a pageable array or np.memmap works too, but then every copy blocks the calling thread.
 STREAM_CHUNK = 1 << 24
 STREAM_RING = 2
+# PSK streams in longer chunks: the speculative Costas loop (DESIGN.md §4.3) sizes its own sub-chunks from the length it is given, and
+# a short ring chunk forces short sub-chunks whose warm-up outweighs them.  Chosen by measurement (DESIGN.md §4.11).
+PSK_STREAM_CHUNK = 1 << 26
+
+
+def psk_entry(mod_order: int) -> int:
+    """urh_stream_footprint flags of a PSK call with Costas loop order mod_order (orders above 4 run as 4)"""
+    return _lib.STREAM_PSK | (_lib.STREAM_PSK4 if int(mod_order) >= 4 else 0)
 
 
 def stream_footprint(n: int, dtype, tolerance: int, entry: int, chunk_samples: int = STREAM_CHUNK, ring: int = STREAM_RING,
@@ -84,6 +92,13 @@ def afp_demod(samples, noise_mag: float, mod_type: str, mod_order: int, costas_l
         host = np.empty(n, dtype=np.float32)
         ctx.check(ctx.lib.urh_afp_demod_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag), code,
                                                STREAM_CHUNK, STREAM_RING, _host_ptr(host)))
+        return host
+    if (not on_device and n > 2 and code == _lib.MOD_PSK
+            and use_stream(n, samples.dtype, 0, _lib.STREAM_AFP_DEMOD | psk_entry(mod_order), device_budget(ctx))):
+        host = np.empty(n, dtype=np.float32)
+        ctx.check(ctx.lib.urh_afp_demod_psk_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag),
+                                                   int(mod_order), float(costas_loop_bandwidth), PSK_STREAM_CHUNK, STREAM_RING,
+                                                   _host_ptr(host)))
         return host
     d_iq = samples if on_device else to_device(samples, ctx)
     out = DeviceArray(ctx, (n,), np.float32)
@@ -173,6 +188,15 @@ def demod_digitize(samples, noise_mag: float, mod_type: str, center: float, tole
                                                     float(center), int(tolerance), int(samples_per_symbol), int(bits_per_symbol),
                                                     float(center_spacing), STREAM_CHUNK, STREAM_RING,
                                                     _host_ptr(host) if host is not None else None, C.byref(k)))
+        return host, _fetch_pulses(ctx, k.value)
+    # PSK: the Costas loop of order 2^bits_per_symbol, as the resident call runs it
+    if (not on_device and n > 2 and code == _lib.MOD_PSK
+            and use_stream(n, samples.dtype, tolerance, entry | psk_entry(1 << int(bits_per_symbol)), device_budget(ctx))):
+        host = np.empty(n, dtype=np.float32) if return_qad else None
+        ctx.check(ctx.lib.urh_demod_digitize_psk_stream(ctx.handle, _host_ptr(samples), _lib.dtype_code(samples.dtype), n, float(noise_mag),
+                                                        float(center), int(tolerance), int(samples_per_symbol), int(bits_per_symbol),
+                                                        float(center_spacing), PSK_STREAM_CHUNK, STREAM_RING,
+                                                        _host_ptr(host) if host is not None else None, C.byref(k)))
         return host, _fetch_pulses(ctx, k.value)
     d_iq = samples if on_device else to_device(samples, ctx)
     qad = DeviceArray(ctx, (n,), np.float32) if return_qad else None

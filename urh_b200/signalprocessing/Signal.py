@@ -313,13 +313,15 @@ class Signal(object):
 
     def _host_capture_too_large(self):
         """the host capture when demodulating it resident would exceed the device budget and it can be streamed instead (ASK /
-        FSK; a capture already on the device fits), else None"""
+        FSK / PSK; a capture already on the device fits), else None"""
         iq = self.iq_array
-        if self.modulation_type not in ("ASK", "FSK") or iq._device is not None or len(iq) <= 2:
+        if self.modulation_type not in ("ASK", "FSK", "PSK") or iq._device is not None or len(iq) <= 2:
             return None
         host = iq._peek()
-        if not signal_functions.use_stream(len(host), host.dtype, 0, _lib.STREAM_AFP_DEMOD,
-                                           signal_functions.device_budget(_lib.default_context())):
+        entry = _lib.STREAM_AFP_DEMOD
+        if self.modulation_type == "PSK":   # the Costas loop's tables grow with the loop order
+            entry |= signal_functions.psk_entry(self.modulation_order)
+        if not signal_functions.use_stream(len(host), host.dtype, 0, entry, signal_functions.device_budget(_lib.default_context())):
             return None
         return host
 
