@@ -145,6 +145,15 @@ int urh_modulate_batch(urh_ctx* ctx, const uint8_t* d_bits, const int64_t* h_bit
                        uint32_t start, int out_dtype, const float* h_gauss_fir, int gauss_len, void* d_out);
 /* diagnostics: steps of the GFSK phase recurrence taken through an integer prefix sum / one by one since the last call */
 int urh_modulate_stats(urh_ctx* ctx, int64_t* h_out2);
+/* test entry point: only the GFSK (frequency, phase) table urh_modulate_batch computes for the same messages and parameters;
+ * d_table: (sum over messages of symbols*sps, 2) float32, message after message */
+int urh_modulate_gfsk_table(urh_ctx* ctx, const uint8_t* d_bits, const int64_t* h_bit_off, int nmsg, uint32_t samples_per_symbol,
+                            const float* h_params, int nparams, int bits_per_symbol, float carrier_phase, float sample_rate,
+                            uint32_t start, const float* h_gauss_fir, int gauss_len, float* d_table);
+/* test entry point: the modulator's device sinf/cosf restatement on d_x[n] (d_ok[i] = 0 for inf / nan) and its fmod(v, 2 pi)
+ * on d_v[nv] */
+int urh_selftest_modmath(urh_ctx* ctx, const float* d_x, int64_t n, float* d_sn, float* d_cs, int* d_ok, const double* d_v,
+                         int64_t nv, double* d_r);
 
 /* ---- filters (filter.cu) ----------------------------------------------------------------------------------
  * urh_fir_filter replaces signal_functions.fir_filter (signal_functions.pyx:513-525), exact accumulation order;

@@ -195,8 +195,10 @@ def get_oqpsk_bits(bits):
 
 
 def modulate_c(bits, samples_per_symbol, modulation_type, parameters, bits_per_symbol, carrier_amplitude,
-               carrier_frequency, carrier_phase, sample_rate, pause, start, dtype=np.float32, gauss_bt=0.5, filter_width=1.0):
-    """signal_functions.pyx:56-177."""
+               carrier_frequency, carrier_phase, sample_rate, pause, start, dtype=np.float32, gauss_bt=0.5, filter_width=1.0,
+               gfsk_table=None):
+    """signal_functions.pyx:56-177.  gfsk_table: a (symbols * sps, 2) float32 (frequency, phase) table to modulate GFSK from
+    instead of gauss_filtered_freqs_phases (checks the sample stage of a GPU table)."""
     bits = np.ascontiguousarray(np.asarray(bits, dtype=np.uint8))
     params = np.ascontiguousarray(np.asarray(parameters, dtype=np.float32))
     dtype = np.dtype(dtype)
@@ -214,7 +216,10 @@ def modulate_c(bits, samples_per_symbol, modulation_type, parameters, bits_per_s
     if mod == "OQPSK":
         assert bits_per_symbol == 2
         bits = np.ascontiguousarray(get_oqpsk_bits(bits))
-    if mod == "GFSK":
+    if mod == "GFSK" and gfsk_table is not None:
+        gtab = np.ascontiguousarray(gfsk_table, dtype=np.float32)
+        assert gtab.shape == (total_symbols * samples_per_symbol, 2), gtab.shape
+    elif mod == "GFSK":
         gtab = np.ascontiguousarray(gauss_filtered_freqs_phases(bits, params, total_symbols, samples_per_symbol,
                                                                 sample_rate, carrier_phase, start, gauss_bt, filter_width))
     lib().oracle_modulate(_p(bits), C.c_int64(num_bits), C.c_uint32(samples_per_symbol), MOD[mod], _p(params),

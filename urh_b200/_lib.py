@@ -170,6 +170,8 @@ SIGNATURES = {
     "urh_path_minmax": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, vp]),
     "urh_qpath_streams": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, i64, vp, vp, i32, vp, vp]),
     "urh_modulate_stats": (i32, [vp, vp]),
+    "urh_modulate_gfsk_table": (i32, [vp, vp, vp, i32, u32, vp, i32, i32, f32, f32, u32, vp, i32, vp]),
+    "urh_selftest_modmath": (i32, [vp, vp, i64, vp, vp, vp, vp, i64, vp]),
     "urh_synth_psk": (i32, [vp, vp, i64, i64, i32, i32, C.c_double, f32, f32, C.c_uint64, i64, i64, i64]),
     "urh_afp_demod_stream": (i32, [vp, vp, i32, i64, f32, i32, i64, i32, vp]),
     "urh_grab_pulse_lens_stream": (i32, [vp, vp, i32, i64, f32, u16, i32, u32, u8, f32, i64, i32, C.POINTER(i64)]),

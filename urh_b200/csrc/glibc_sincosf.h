@@ -11,8 +11,9 @@
 //   * the 14-double table __sincosf_table[2] sits at 0xb8120 (signs, 2/pi*2^24, pi/2, c0,c1,s1,c2,s2,c3,s3,c4);
 //     entry [1] negates the cosine polynomial.
 // The non-FMA (SSE2) variant differs only in the last bit of the double intermediates (observable in the
-// float result with probability ~2^-29 per call).  tests/test_sincosf_restatement.py pins this header
-// against libm bit-for-bit on the CPU.
+// float result with probability ~2^-29 per call).  tests/test_sincosf_restatement.py (|x| < 120) and
+// tests/test_modulator_pin.py (|x| >= 120) pin this header against libm bit-for-bit on the CPU;
+// tests/test_gpu_modulator_exact.py pins the device build over the whole float range.
 #pragma once
 #include <math.h>
 #include <stdint.h>

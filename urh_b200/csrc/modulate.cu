@@ -145,6 +145,11 @@ __global__ void __launch_bounds__(128) k_gfsk_phases(const int64_t* __restrict__
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     const double two_pi = 2.0 * M_PI;
+    // t = np.arange(start, start + nval, dtype=float32) / sample_rate.  numpy fills a float32 arange as t_i = fl(t0 + fl(fl(i) * d))
+    // with t0 = fl(start), d = fl(fl(start + 1) - t0) — not fl(start + i): the two part at i = 2^24 + 1 for start = 1, and from
+    // start = 2^31 + 1 on d = 0 (a constant time base).
+    const float t0 = __ll2float_rn((long long)P.start);
+    const float dt = __fsub_rn(__ll2float_rn((long long)P.start + 1), t0);
     for (int64_t m = warp; m < nmsg; m += nwarps) {
         const int64_t nsym = (bit_off[m + 1] - bit_off[m]) / P.bps;
         const int64_t nval = nsym * P.sps;
@@ -159,8 +164,7 @@ __global__ void __launch_bounds__(128) k_gfsk_phases(const int64_t* __restrict__
             double c = 0.0;
             if (valid) {
                 const float fcur = tab[2 * i], fnext = tab[2 * (i + 1)];
-                // t = np.arange(start, ..., dtype=float32) / sample_rate: float32 index, float32 division
-                const float t = __fdiv_rn(__ll2float_rn((long long)i + (long long)P.start), P.sample_rate);
+                const float t = __fdiv_rn(__fadd_rn(t0, __fmul_rn(__ll2float_rn((long long)i), dt)), P.sample_rate);
                 c = __dmul_rn(__dmul_rn(two_pi, (double)t), (double)__fsub_rn(fcur, fnext));
             }
             const int count = (int)min((int64_t)32, nval - 1 - base);
@@ -307,6 +311,25 @@ __global__ void __launch_bounds__(256) k_modulate(const uint8_t* __restrict__ bi
     }
 }
 
+// GFSK (frequency, phase) table of a batch: per-sample filtered frequencies, then the phase recurrence.  fp_table holds
+// 2 * smp_off[nmsg] floats; max_samples is the longest message in samples.
+static int gfsk_table(urh_ctx* ctx, const uint8_t* d_bits, const int64_t* d_bit_off, const int64_t* d_smp_off, int nmsg, const ModParams& P,
+                      int64_t max_samples, const float* h_gauss_fir, int gauss_len, float* fp_table) {
+    if (!h_gauss_fir || gauss_len <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "GFSK needs the gaussian filter taps");
+    std::vector<double> gsum((size_t)gauss_len + 1, 0.0);
+    for (int j = 0; j < gauss_len; j++) gsum[j + 1] = gsum[j] + (double)h_gauss_fir[j];
+    double* d_gsum;
+    URH_CHECK(urh_arena(ctx, (size_t)gauss_len + 1, &d_gsum));
+    URH_CUDA(ctx, cudaMemcpyAsync(d_gsum, gsum.data(), (gauss_len + 1) * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    const unsigned gx = (unsigned)max((int64_t)1, min(urh_div_up(max_samples, 256), (int64_t)ctx->sm_count * 8));
+    const dim3 grid(gx, (unsigned)min(nmsg, 65535));
+    URH_LAUNCH(ctx, k_gfsk_freqs, grid, 256, 0, d_bits, d_bit_off, d_smp_off, nmsg, P, d_gsum, gauss_len, fp_table);
+    URH_LAUNCH(ctx, k_gfsk_phases, (unsigned)min((int64_t)urh_div_up(nmsg, 4), (int64_t)ctx->sm_count * 16), 128, 0, d_bit_off, d_smp_off, nmsg, P,
+               fp_table);
+    return URH_OK;
+}
+
 // Batch modulate.  d_bits: concatenated bit arrays (uint8, already OQPSK-shuffled if needed);
 // h_bit_off[nmsg+1]: bit offsets; h_out_off[nmsg+1]: output SAMPLE offsets (message m occupies
 // [h_out_off[m], h_out_off[m+1]) = symbols*sps + pause samples); d_out is zero-filled here.
@@ -356,24 +379,13 @@ extern "C" int urh_modulate_batch(urh_ctx* ctx, const uint8_t* d_bits, const int
     URH_CUDA(ctx, cudaMemcpyAsync(d_out_off, h_out_off, ob, cudaMemcpyHostToDevice, ctx->stream));
     // the modulation kernel writes every output sample once, pauses included: no memset pass over the (write-only) output
     float *corr = nullptr, *fp_table = nullptr;
-    double* d_gsum = nullptr;
     if (mod_type == URH_MOD_FSK) {
         URH_CHECK(urh_arena(ctx, (size_t)sym_off[nmsg] + 1, &corr));
         URH_LAUNCH(ctx, k_fsk_corrections, (unsigned)min((int64_t)urh_div_up(nmsg, 4), (int64_t)ctx->sm_count * 16), 128, 0, d_bits, d_bit_off, d_sym_off, nmsg, P, corr);
     }
-    const unsigned gx = (unsigned)max((int64_t)1, min(urh_div_up(max_samples, 256), (int64_t)ctx->sm_count * 8));
-    const dim3 grid(gx, (unsigned)min(nmsg, 65535));
     if (mod_type == URH_MOD_GFSK) {
-        if (!h_gauss_fir || gauss_len <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "GFSK needs the gaussian filter taps");
         URH_CHECK(urh_arena(ctx, (size_t)smp_off[nmsg] * 2 + 2, &fp_table));
-        std::vector<double> gsum((size_t)gauss_len + 1, 0.0);
-        for (int j = 0; j < gauss_len; j++) gsum[j + 1] = gsum[j] + (double)h_gauss_fir[j];
-        URH_CHECK(urh_arena(ctx, (size_t)gauss_len + 1, &d_gsum));
-        URH_CUDA(ctx, cudaMemcpyAsync(d_gsum, gsum.data(), (gauss_len + 1) * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        URH_LAUNCH(ctx, k_gfsk_freqs, grid, 256, 0, d_bits, d_bit_off, d_smp_off, nmsg, P, d_gsum, gauss_len, fp_table);
-        URH_LAUNCH(ctx, k_gfsk_phases, (unsigned)min((int64_t)urh_div_up(nmsg, 4), (int64_t)ctx->sm_count * 16), 128, 0, d_bit_off, d_smp_off, nmsg, P,
-                   fp_table);
+        URH_CHECK(gfsk_table(ctx, d_bits, d_bit_off, d_smp_off, nmsg, P, max_samples, h_gauss_fir, gauss_len, fp_table));
     }
     const unsigned gp = (unsigned)max((int64_t)1, min(urh_div_up(urh_div_up(max_total, 2), 256), (int64_t)ctx->sm_count * 8));
     const dim3 gridp(gp, (unsigned)min(nmsg, 65535));
@@ -396,5 +408,63 @@ extern "C" int urh_modulate_stats(urh_ctx* ctx, int64_t* h_out2) {
     URH_CUDA(ctx, cudaMemcpyToSymbol(g_gfsk_blocks, z, sizeof(z)));
     h_out2[0] = (int64_t)v[0];
     h_out2[1] = (int64_t)v[1];
+    return URH_OK;
+}
+
+// Test entry point: only the GFSK table of a batch (k_gfsk_freqs + k_gfsk_phases, as urh_modulate_batch runs them) into
+// d_table = (sum of symbols * sps, 2) float32 (frequency, phase) rows, message after message.
+extern "C" int urh_modulate_gfsk_table(urh_ctx* ctx, const uint8_t* d_bits, const int64_t* h_bit_off, int nmsg, uint32_t samples_per_symbol,
+                                       const float* h_params, int nparams, int bits_per_symbol, float carrier_phase, float sample_rate,
+                                       uint32_t start, const float* h_gauss_fir, int gauss_len, float* d_table) {
+    if (nmsg <= 0) return URH_OK;
+    if (bits_per_symbol < 1 || bits_per_symbol > 8 || nparams > 256 || nparams < (1 << bits_per_symbol))
+        URH_FAIL(ctx, URH_ERR_INVALID, "bits_per_symbol / parameters mismatch");
+    urh_arena_reset(ctx);
+    ModParams P;
+    memset(&P, 0, sizeof(P));
+    P.sps = samples_per_symbol; P.mod_type = URH_MOD_GFSK; P.bps = bits_per_symbol; P.phi = carrier_phase; P.sample_rate = sample_rate;
+    P.start = start; P.nparams = nparams;
+    memcpy(P.params, h_params, sizeof(float) * nparams);
+    std::vector<int64_t> smp_off(nmsg + 1, 0);
+    int64_t max_samples = 0;
+    for (int m = 0; m < nmsg; m++) {
+        const int64_t nval = (h_bit_off[m + 1] - h_bit_off[m]) / bits_per_symbol * samples_per_symbol;
+        if (nval >= ((int64_t)1 << 31) - 2) URH_FAIL(ctx, URH_ERR_INVALID, "one message of >= 2^31 samples: split it");
+        smp_off[m + 1] = smp_off[m] + nval;
+        if (nval > max_samples) max_samples = nval;
+    }
+    int64_t *d_bit_off, *d_smp_off;
+    URH_CHECK(urh_arena(ctx, (size_t)nmsg + 1, &d_bit_off));
+    URH_CHECK(urh_arena(ctx, (size_t)nmsg + 1, &d_smp_off));
+    const size_t ob = (size_t)(nmsg + 1) * sizeof(int64_t);
+    URH_CUDA(ctx, cudaMemcpyAsync(d_bit_off, h_bit_off, ob, cudaMemcpyHostToDevice, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync(d_smp_off, smp_off.data(), ob, cudaMemcpyHostToDevice, ctx->stream));
+    URH_CHECK(gfsk_table(ctx, d_bits, d_bit_off, d_smp_off, nmsg, P, max_samples, h_gauss_fir, gauss_len, d_table));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the offset vectors above are host temporaries
+    return URH_OK;
+}
+
+// Test entry point: the modulator's device math on device arrays — urh_glibc_sincosf(x[i]) -> sn[i], cs[i], ok[i] and
+// urh_fmod_2pi(v[j]) -> r[j] — for comparison with libm's sinf / cosf / fmod.
+__global__ void k_selftest_modmath(const float* __restrict__ x, int64_t n, float* __restrict__ sn, float* __restrict__ cs, int* __restrict__ ok,
+                                   const double* __restrict__ v, int64_t nv, double* __restrict__ r) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        float s, c;
+        int o;
+        urh_glibc_sincosf(x[i], &s, &c, &o);
+        sn[i] = s;
+        cs[i] = c;
+        ok[i] = o;
+    }
+    for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < nv; j += stride) r[j] = urh_fmod_2pi(v[j]);
+}
+
+extern "C" int urh_selftest_modmath(urh_ctx* ctx, const float* d_x, int64_t n, float* d_sn, float* d_cs, int* d_ok, const double* d_v,
+                                    int64_t nv, double* d_r) {
+    if (n <= 0 && nv <= 0) return URH_OK;
+    const unsigned g = (unsigned)max((int64_t)1, min(urh_div_up(max(n, nv), 256), (int64_t)ctx->sm_count * 8));
+    URH_LAUNCH(ctx, k_selftest_modmath, g, 256, 0, d_x, n, d_sn, d_cs, d_ok, d_v, nv, d_r);
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return URH_OK;
 }
