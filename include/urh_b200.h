@@ -91,7 +91,8 @@ int urh_pulses_device_ptr(urh_ctx* ctx, const int64_t** d_rows, int64_t* k);
 /* replaces util.get_magnitudes (util.pyx:128-136): float64[n] */
 int urh_get_magnitudes(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double* d_out);
 /* per-chunk (sum, max) of the magnitudes, chunks counted from the END of the capture as
- * AutoInterpretation.detect_noise_level does (AutoInterpretation.py:60-91); h_sum/h_max: host arrays [nchunks] */
+ * AutoInterpretation.detect_noise_level does (AutoInterpretation.py:60-91); h_sum/h_max: host arrays [nchunks].
+ * Float32 magnitudes (is_f64 = 0): h_sum = numpy's float32 pairwise sum of each chunk, as np.mean computes it. */
 int urh_noise_chunk_stats_iq(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int64_t chunksize, int nchunks,
                              double* h_sum, double* h_max);
 int urh_noise_chunk_stats(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, int64_t chunksize, int nchunks,
@@ -354,7 +355,7 @@ int urh_fft_argmax(urh_ctx* ctx, const float* d_x, int64_t n, int64_t* h_index, 
  * other (numpy's integer wrap-around, C truncation for float -> int).  count = number of elements (2 per sample). */
 int urh_convert_iq(urh_ctx* ctx, const void* d_in, int in_dtype, void* d_out, int out_dtype, int64_t count);
 /* the sample-rate part of AutoInterpretation.detect_modulation (AutoInterpretation.py:151-208) for one message
- * (d_data = complex64[n] on the device): zero removal, normalisation, the two Haar wavelet transforms (cuFFT for the FFTs),
+ * (d_data = complex64[n] on the device): removal of the samples whose magnitude is not > 0 (zeros and NaN), normalisation, the two Haar wavelet transforms (cuFFT for the FFTs),
  * variances before/after the median filter and the spectrum features of the FSK test.  h_feat[8] = {n_nonzero, P, L, var_mag,
  * var_norm_mag, var_filtered_mag, var_filtered_norm_mag, |max|}; h_spec[23] = {arg-max bin, value, best bin >= 10 away,
  * value, the 19 values around the arg-max}.  urh_cwt_haar replaces Wavelet.cwt_haar (Wavelet.py:15-43). */

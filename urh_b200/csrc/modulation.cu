@@ -29,11 +29,14 @@
         }                                                                                                     \
     } while (0)
 
+// data[np.abs(data) > 0]: a NaN magnitude compares false, so (NaN, 0) is dropped while (inf, NaN), whose hypot is inf, stays
+__device__ __forceinline__ bool urh_mod_keep(float2 v) { return hypotf(v.x, v.y) > 0.0f; }
+
 __global__ void k_mod_flags(const float2* __restrict__ x, int64_t n, int64_t* __restrict__ flag) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) {
         const float2 v = x[i];
-        flag[i] = (v.x != 0.0f || v.y != 0.0f) ? 1 : 0;   // |v| > 0
+        flag[i] = urh_mod_keep(v) ? 1 : 0;
     }
 }
 
@@ -41,7 +44,7 @@ __global__ void k_mod_compact(const float2* __restrict__ x, int64_t n, const int
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) {
         const float2 v = x[i];
-        if (v.x != 0.0f || v.y != 0.0f) out[off[i]] = v;
+        if (urh_mod_keep(v)) out[off[i]] = v;
     }
 }
 

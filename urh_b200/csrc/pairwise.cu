@@ -46,20 +46,22 @@ __device__ __forceinline__ float pw_elem(const float* __restrict__ a, int64_t i,
     return __fmul_rn(d, d);
 }
 
-// one 8-lane group per slot; only the group of a leaf's FIRST slot does the work
+// one 8-lane group per slot; only the group of a leaf's FIRST slot does the work.  Batch b = blockIdx.y sums the n elements
+// from a + off0 + b * step into val[b << D ...]; every batch has the same tree, so batch 0 alone writes depth_of.
 template <int MODE>
 __global__ void __launch_bounds__(256) k_pw_leaves(const float* __restrict__ a, int64_t n, int D, const float* __restrict__ d_mean,
-                                                  float* __restrict__ val, uint8_t* __restrict__ depth_of) {
+                                                  float* __restrict__ val, uint8_t* __restrict__ depth_of, int64_t off0, int64_t step) {
     const int64_t g = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 3;   // slot
     const int k = threadIdx.x & 7;
     const unsigned gmask = 0xffu << ((threadIdx.x & 31) & ~7);
     if (g >= ((int64_t)1 << D)) return;
     const float mean = MODE ? *d_mean : 0.0f;
     const PwNode nd = pw_descend(n, D, g);
-    if (k == 0) depth_of[g] = (uint8_t)nd.depth;
+    if (k == 0 && blockIdx.y == 0) depth_of[g] = (uint8_t)nd.depth;
     const int64_t first = (nd.depth < D) ? ((g >> (D - nd.depth)) << (D - nd.depth)) : g;
     if (g != first) return;
-    const float* p = a;
+    const float* p = a + off0 + (int64_t)blockIdx.y * step;
+    val += (int64_t)blockIdx.y << D;
     const int64_t s = nd.start;
     const int len = (int)nd.len;
     float res;
@@ -85,15 +87,17 @@ __global__ void __launch_bounds__(256) k_pw_leaves(const float* __restrict__ a, 
 __global__ void k_pw_level(float* __restrict__ val, const uint8_t* __restrict__ depth_of, int D, int d) {
     const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= ((int64_t)1 << d)) return;
+    val += (int64_t)blockIdx.y << D;   // batch
     const int64_t left = j << (D - d);
     if (depth_of[left] <= d) return;
     const int64_t right = left + ((int64_t)1 << (D - d - 1));
     val[left] = __fadd_rn(val[left], val[right]);
 }
 
-// the top levels (d < top) in one block; then result = float32(double(0.0f + sum) / n) -> *out (and mean/var semantics)
+// the top levels (d < top) in one block per batch; then out[2b] = 0.0f + sum, out[2b + 1] = float32(double(that) / n)
 __global__ void __launch_bounds__(1024) k_pw_top(float* __restrict__ val, const uint8_t* __restrict__ depth_of, int D, int top, int64_t n,
-                                                float* __restrict__ out_sum, float* __restrict__ out_div) {
+                                                float* __restrict__ out) {
+    val += (int64_t)blockIdx.x << D;
     for (int d = top - 1; d >= 0; d--) {
         for (int64_t j = threadIdx.x; j < ((int64_t)1 << d); j += blockDim.x) {
             const int64_t left = j << (D - d);
@@ -106,8 +110,8 @@ __global__ void __launch_bounds__(1024) k_pw_top(float* __restrict__ val, const 
     }
     if (threadIdx.x == 0) {
         const float s = __fadd_rn(0.0f, val[0]);   // add.reduce starts from the identity
-        *out_sum = s;
-        *out_div = __double2float_rn(__ddiv_rn((double)s, (double)n));
+        out[2 * blockIdx.x] = s;
+        out[2 * blockIdx.x + 1] = __double2float_rn(__ddiv_rn((double)s, (double)n));
     }
 }
 
@@ -123,21 +127,31 @@ static int pw_depth(int64_t n) {
     return d;
 }
 
-// d_out[0] = add.reduce of the sequence, d_out[1] = float32(double(sum) / n).  MODE 1 reads the mean from d_mean (device).
+// d_out[2b] = add.reduce of the n elements from d_a + off0 + b * step, d_out[2b + 1] = float32(double(sum) / n), b < batch.
+// MODE 1 reads the mean from d_mean (device).
 template <int MODE>
-static int pw_reduce(urh_ctx* ctx, const float* d_a, int64_t n, const float* d_mean, float* d_out) {
+static int pw_reduce(urh_ctx* ctx, const float* d_a, int64_t n, const float* d_mean, float* d_out, int batch = 1, int64_t off0 = 0,
+                     int64_t step = 0) {
     const int D = pw_depth(n);
     const int64_t slots = (int64_t)1 << D;
     float* val;
     uint8_t* depth_of;
-    URH_CHECK(urh_arena(ctx, (size_t)slots, &val));
+    URH_CHECK(urh_arena(ctx, (size_t)slots * batch, &val));
     URH_CHECK(urh_arena(ctx, (size_t)slots, &depth_of));
-    URH_LAUNCH(ctx, (k_pw_leaves<MODE>), (unsigned)urh_div_up(slots * 8, 256), 256, 0, d_a, n, D, d_mean, val, depth_of);
+    URH_LAUNCH(ctx, (k_pw_leaves<MODE>), dim3((unsigned)urh_div_up(slots * 8, 256), (unsigned)batch), 256, 0, d_a, n, D, d_mean, val,
+               depth_of, off0, step);
     const int top = D < 12 ? D : 12;
     for (int d = D - 1; d >= top; d--)
-        URH_LAUNCH(ctx, k_pw_level, (unsigned)urh_div_up((int64_t)1 << d, 256), 256, 0, val, (const uint8_t*)depth_of, D, d);
-    URH_LAUNCH(ctx, k_pw_top, 1, 1024, 0, val, (const uint8_t*)depth_of, D, top, n, d_out, d_out + 1);
+        URH_LAUNCH(ctx, k_pw_level, dim3((unsigned)urh_div_up((int64_t)1 << d, 256), (unsigned)batch), 256, 0, val,
+                   (const uint8_t*)depth_of, D, d);
+    URH_LAUNCH(ctx, k_pw_top, (unsigned)batch, 1024, 0, val, (const uint8_t*)depth_of, D, top, n, d_out);
     return URH_OK;
+}
+
+// np.mean's float32 sums of the `batch` equal-length chunks [n - (b+1)*len, n - b*len) of d_a (detect_noise_level's end-aligned
+// 1 % chunks of a float32 magnitude array): d_out[2b] = numpy's pairwise sum of chunk b, d_out[2b + 1] = float32(sum / len).
+int urh_chunk_sums_f32(urh_ctx* ctx, const float* d_a, int64_t n, int64_t len, int batch, float* d_out) {
+    return pw_reduce<0>(ctx, d_a, len, nullptr, d_out, batch, n - len, -len);
 }
 
 // ---- compaction of the rank window ------------------------------------------------------------------------------------------

@@ -13,6 +13,8 @@
 
 #include <math.h>
 
+#include <vector>
+
 // ---- magnitudes ------------------------------------------------------------------------------------------
 // float32 IQ: (double)sqrtf(fl(re*re + im*im)); integer IQ: squares and sum in (wrapping) int32, double sqrt.
 template <int DT>
@@ -137,7 +139,11 @@ extern "C" int urh_noise_chunk_stats_iq(urh_ctx* ctx, const void* d_iq, int dtyp
     URH_DISPATCH_DT(dtype, { LoadMagIQ<DT> ld; ld.iq = d_iq; URH_CHECK(chunk_stats(ctx, ld, n, chunksize, nchunks, h_sum, h_max)); });
     return URH_OK;
 }
-// the same on an existing magnitude array (float32: is_f64 = 0, float64: is_f64 = 1)
+int urh_chunk_sums_f32(urh_ctx* ctx, const float* d_a, int64_t n, int64_t len, int batch, float* d_out);   // pairwise.cu
+
+// the same on an existing magnitude array (float32: is_f64 = 0, float64: is_f64 = 1).  For float32 magnitudes h_sum holds
+// np.mean's own float32 sum of each chunk (numpy's pairwise summation, replayed by pairwise.cu), which the caller divides in
+// float32 as np.mean does: a double sum rounds differently and flips chunks on the `mean <= 1.1 * min` edge.
 extern "C" int urh_noise_chunk_stats(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, int64_t chunksize, int nchunks,
                                      double* h_sum, double* h_max) {
     if (nchunks <= 0 || chunksize <= 0 || (int64_t)nchunks * chunksize > n) URH_FAIL(ctx, URH_ERR_INVALID, "bad chunking");
@@ -146,7 +152,15 @@ extern "C" int urh_noise_chunk_stats(urh_ctx* ctx, const void* d_mags, int is_f6
         return chunk_stats(ctx, ld, n, chunksize, nchunks, h_sum, h_max);
     }
     LoadReal<float> ld; ld.x = (const float*)d_mags;
-    return chunk_stats(ctx, ld, n, chunksize, nchunks, h_sum, h_max);
+    URH_CHECK(chunk_stats(ctx, ld, n, chunksize, nchunks, h_sum, h_max));   // the maxima (and double sums, replaced below)
+    float* d_pw;
+    URH_CHECK(urh_arena(ctx, (size_t)2 * nchunks, &d_pw));
+    URH_CHECK(urh_chunk_sums_f32(ctx, (const float*)d_mags, n, chunksize, nchunks, d_pw));
+    std::vector<float> pw((size_t)2 * nchunks);
+    URH_CUDA(ctx, cudaMemcpyAsync(pw.data(), d_pw, pw.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    for (int c = 0; c < nchunks; c++) h_sum[c] = (double)pw[2 * c];
+    return URH_OK;
 }
 
 // ---- run tables for the segmenter and the plateau RLE ----------------------------------------------------------------
