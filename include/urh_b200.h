@@ -327,6 +327,57 @@ int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samp
 int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
 int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3);
 int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
+/* ---- streaming the filters and the spectrogram: the windowed ring (stream_window.cu, filter.cu, spectrogram.cu; DESIGN.md §4.11).
+ * A chunk owns the outputs [k0, k1) and uploads the input window [a, b) those outputs read, clipped to the capture; halos come from the
+ * host buffer, so no chunk reads another chunk's slot.  Host input and host output (pinned or pageable), ring of 2..8 slots, chunk of
+ * chunk_samples input samples (<= 0: 2^24).  Results are bit-identical to the resident entry points named, except where noted.
+ * urh_convolve_c128_stream: urh_convolve_c128 (Filter.apply_bandpass_filter / fft_convolve_1d, Filter.py:69-101) over host x[n] into
+ *   h_y[out_len]; h_taps complex128[m].
+ * urh_fir_filter_stream: urh_fir_filter (signal_functions.fir_filter, signal_functions.pyx:513-525; Filter.apply_fir_filter Filter.py:35-46);
+ *   h_taps complex64[m]; chunks are at least m - 1 samples.
+ * urh_dc_correction_stream: Filter.dc_correction (Filter.py:31-33) in two passes (column sums, then the subtraction).  float32 with
+ *   exact_order != 0: urh_dc_correction's serial float32 chain continued from chunk to chunk; float32 with exact_order == 0: per-chunk
+ *   double sums added in chunk order, mean = float32(sum / n) (what the sharded correction does; not the resident reduction's order);
+ *   integer dtypes: urh_dc_correction_int (h_out double[n][2]).
+ * urh_stft_stream / urh_spectrogram_db_stream: urh_stft / urh_spectrogram_db (Spectrogram.stft Spectrogram.py:94-116,
+ *   __calculate_spectrogram :156-162) in runs of chunk_samples / hop (at least one) whole frames; h_window float64[W].
+ * urh_spectrogram_bgra_stream: urh_spectrogram_bgra (Spectrogram.create_spectrogram_image / create_image_segments, Spectrogram.py:
+ *   164-190) into host h_out; whole segments are grouped per chunk, a segment longer than a chunk is rendered in runs of frames.
+ * urh_stream_windows: the chunks {k0, k1, a, b} (4 int64 each) of an entry URH_FILTER_*; host only.  Outputs: CONVOLVE samples of
+ *   out_len (p0 = m, p1 = offset), FIR samples of n (p0 = m), DC rows of n, STFT / DB frames of out_len (p0 = W, p1 = hop), IMAGES the
+ *   frames of all segments in order (p0 = W, p1 = hop, the segments; out_len unused).
+ * urh_stream_window_schedule: the op order of the windowed ring, 7 int64 per op {kind, chunk, slot, k0, k1, a, b}, kinds and
+ *   semantics as urh_stream_schedule; h_win: the chunks of urh_stream_windows.  flags: URH_STREAM_UPLOAD / DOWNLOAD; host only.
+ * urh_stream_filter_footprint: device bytes of the streamed entry (resident = 0) or of the resident entry fed from the host (resident
+ *   != 0), without a device.  Parameters as urh_stream_windows; out_len is the output count for CONVOLVE, the frames for STFT / DB and
+ *   the frames of all segments for IMAGES; p2 is the colormap's entry count for IMAGES (at least 1) and 0 otherwise; dtype matters for
+ *   DC only.
+ * With urh_set_profiling on, these calls report through urh_stream_stats as the demodulation entries do; the chunk count is the
+ *   chunks of one pass over the capture (the DC correction's two passes cut it into the same chunks), the free-memory low point and
+ *   the arena peak cover the whole call. */
+#define URH_FILTER_CONVOLVE 0
+#define URH_FILTER_FIR 1
+#define URH_FILTER_DC 2
+#define URH_FILTER_STFT 3
+#define URH_FILTER_DB 4
+#define URH_FILTER_IMAGES 5
+int urh_convolve_c128_stream(urh_ctx* ctx, const float* h_x, int64_t n, const double* h_taps, int m, int64_t offset, int64_t out_len,
+                             int64_t chunk_samples, int ring, float* h_y);
+int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, const float* h_taps, int m, int64_t chunk_samples, int ring, float* h_y);
+int urh_dc_correction_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, int exact_order, int64_t chunk_samples, int ring,
+                             void* h_out);
+int urh_stft_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window, int64_t num_frames,
+                    int64_t chunk_samples, int ring, double* h_out);
+int urh_spectrogram_db_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
+                              int64_t num_frames, int64_t chunk_samples, int ring, float* h_out);
+int urh_spectrogram_bgra_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
+                                const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* h_colormap, int entries,
+                                float data_min, float data_max, int transpose, int64_t chunk_samples, int ring, uint8_t* h_out);
+int urh_stream_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples, const int64_t* h_seg_start,
+                       const int64_t* h_seg_len, int nseg, int64_t* h_win, int64_t cap, int64_t* count);
+int urh_stream_window_schedule(const int64_t* h_win, int64_t chunks, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
+int urh_stream_filter_footprint(int entry, int64_t n, int64_t out_len, int dtype, int64_t p0, int64_t p1, int64_t p2, int64_t chunk_samples,
+                                int ring, int resident, int64_t* bytes);
 int urh_shard_demod_center_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag,
                                     int mod_type, uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size,
                                     float* d_qad_out, int64_t global_offset, int64_t n_total, double* center,

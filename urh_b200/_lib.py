@@ -23,6 +23,7 @@ STREAM_AFP_DEMOD, STREAM_GRAB_PULSE_LENS, STREAM_DEMOD_DIGITIZE, STREAM_DEMOD_CE
 STREAM_QAD_OUT, STREAM_RESIDENT, STREAM_QAD_ON_DEVICE = 0x10, 0x20, 0x40
 STREAM_PSK, STREAM_PSK4 = 0x80, 0x100
 STREAM_UPLOAD, STREAM_DOWNLOAD, STREAM_HALO = 1, 2, 4
+FILTER_CONVOLVE, FILTER_FIR, FILTER_DC, FILTER_STFT, FILTER_DB, FILTER_IMAGES = 0, 1, 2, 3, 4, 5
 
 _DTYPE_CODE = {
     np.dtype(np.int8): DT_I8,
@@ -184,6 +185,15 @@ SIGNATURES = {
     "urh_stream_schedule": (i32, [i64, i64, i32, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_stats": (i32, [vp, vp]),
     "urh_mem_get_info": (i32, [vp, C.POINTER(szt), C.POINTER(szt)]),
+    "urh_convolve_c128_stream": (i32, [vp, vp, i64, vp, i32, i64, i64, i64, i32, vp]),
+    "urh_fir_filter_stream": (i32, [vp, vp, i64, vp, i32, i64, i32, vp]),
+    "urh_dc_correction_stream": (i32, [vp, vp, i32, i64, i32, i64, i32, vp]),
+    "urh_stft_stream": (i32, [vp, vp, i64, i32, i32, vp, i64, i64, i32, vp]),
+    "urh_spectrogram_db_stream": (i32, [vp, vp, i64, i32, i32, vp, i64, i64, i32, vp]),
+    "urh_spectrogram_bgra_stream": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, f32, f32, i32, i64, i32, vp]),
+    "urh_stream_windows": (i32, [i32, i64, i64, i64, i64, i64, vp, vp, i32, vp, i64, C.POINTER(i64)]),
+    "urh_stream_window_schedule": (i32, [vp, i64, i32, i32, vp, i64, C.POINTER(i64)]),
+    "urh_stream_filter_footprint": (i32, [i32, i64, i64, i32, i64, i64, i64, i64, i32, i32, C.POINTER(i64)]),
     "urh_synth_fsk": (i32, [vp, vp, i64, i64, i32, vp, vp, C.c_double, f32, f32, C.c_uint64, i64, i64, i64, i64, i64]),
 }
 

@@ -10,6 +10,7 @@
 #endif
 #include "fsk_fast.cuh"
 #include "dense_f32.cuh"
+#include "stream_ring.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -636,10 +637,6 @@ int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps
                      int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
                      int64_t rows_cap, int64_t* k);   // finish.cu
 
-#define URH_STREAM_MAX_RING 8
-#define URH_STREAM_PAD 256   // slot = [pad][halo][chunk]: the chunk starts 256 bytes in, the halo sample right before it
-enum { URH_OP_UPLOAD = 0, URH_OP_COMPUTE = 1, URH_OP_DOWNLOAD = 2 };
-
 static int64_t stream_chunk_samples(int64_t n, int64_t cs) {
     if (cs <= 0) cs = (int64_t)1 << 24;
     cs -= cs % URH_TILE;
@@ -691,7 +688,6 @@ struct StreamSizes {
     int64_t scan_items;  // largest table a look-back scan of the call runs over
     int64_t rows_chunk;  // bound of one chunk's rows
 };
-static int64_t r256(int64_t b) { return (b + 255) & ~(int64_t)255; }
 static int64_t finish_arena_bytes(int64_t tiles, int64_t rows_cap, bool ask) {
     return r256(tiles * (int64_t)sizeof(RunCarry)) + 2 * r256(tiles * 4) + 2 * r256(tiles * 8) + r256((32 + 8) * 8) +
            (ask ? r256(rows_cap * 16) : 0);
@@ -782,82 +778,6 @@ extern "C" int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3) {
     h_out3[0] = ctx->stream_free_low;
     h_out3[1] = ctx->stream_chunks;
     h_out3[2] = (int64_t)ctx->arena_peak;
-    return URH_OK;
-}
-
-// The ring of one streamed call: the block, its events, and the copy streams drained before the block is freed on every exit path.
-struct StreamRing {
-    urh_ctx* ctx = nullptr;
-    char* mem = nullptr;
-    cudaEvent_t ev[3][URH_STREAM_MAX_RING] = {};
-    int ring = 0;
-    int init(urh_ctx* c, int r, int64_t bytes) {
-        ctx = c;
-        ring = r;
-        ctx->stream_free_low = -1;
-        for (int k = 0; k < 3; k++)
-            for (int s = 0; s < r; s++) URH_CUDA(ctx, cudaEventCreateWithFlags(&ev[k][s], cudaEventDisableTiming));
-        if (bytes > 0) URH_CUDA(ctx, cudaMallocAsync((void**)&mem, (size_t)bytes, ctx->stream));
-        // the copy streams start after everything queued on the compute stream so far (the ring block included)
-        URH_CUDA(ctx, cudaEventRecord(ctx->ev_comp[0], ctx->stream));
-        URH_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream[0], ctx->ev_comp[0], 0));
-        URH_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_stream[1], ctx->ev_comp[0], 0));
-        return URH_OK;
-    }
-    ~StreamRing() {
-        if (!ctx) return;
-        cudaStreamSynchronize(ctx->copy_stream[0]);
-        cudaStreamSynchronize(ctx->copy_stream[1]);
-        if (mem) cudaFreeAsync(mem, ctx->stream);
-        cudaStreamSynchronize(ctx->stream);
-        for (int k = 0; k < 3; k++)
-            for (int s = 0; s < ring; s++)
-                if (ev[k][s]) cudaEventDestroy(ev[k][s]);
-    }
-};
-
-// Runs the schedule: compute(c, s0, s1, slot) enqueues chunk c's work on the compute stream (it may synchronise).  h_src: host source
-// of src_b bytes per sample uploaded into slots of src_slot bytes at d_src (NULL: the computation reads device data); h_qad: host
-// destination of the qad slots at d_qad (cs floats each; NULL: none).
-template <typename F>
-static int stream_run(urh_ctx* ctx, int64_t n, int64_t cs, StreamRing& R, const char* h_src, int src_b, bool halo, char* d_src,
-                      int64_t src_slot, float* h_qad, float* d_qad, F&& compute, bool qad_resident = false) {
-    const int flags = (h_src ? URH_STREAM_UPLOAD : 0) | (h_qad ? URH_STREAM_DOWNLOAD : 0) | (halo ? URH_STREAM_HALO : 0);
-    int64_t count = 0;
-    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, nullptr, 0, &count));
-    std::vector<int64_t> ops((size_t)(6 * count));
-    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, ops.data(), count, &count));
-    bool recorded[3][URH_STREAM_MAX_RING] = {};
-    ctx->stream_chunks = 0;
-    for (int64_t i = 0; i < count; i++) {
-        const int64_t* o = &ops[(size_t)(6 * i)];
-        const int kind = (int)o[0], s = (int)o[2];
-        const int64_t c = o[1], s0 = o[3], s1 = o[4], h = o[5];
-        if (kind == URH_OP_UPLOAD) {
-            cudaStream_t cp = ctx->copy_stream[0];
-            if (recorded[URH_OP_COMPUTE][s]) URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
-            URH_CUDA(ctx, cudaMemcpyAsync(d_src + s * src_slot + URH_STREAM_PAD - h * src_b, h_src + (s0 - h) * src_b,
-                                          (size_t)((s1 - s0 + h) * src_b), cudaMemcpyHostToDevice, cp));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_UPLOAD][s], cp));
-        } else if (kind == URH_OP_COMPUTE) {
-            if (h_src) URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_UPLOAD][s], 0));
-            if (h_qad && !qad_resident && recorded[URH_OP_DOWNLOAD][s])
-                URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_DOWNLOAD][s], 0));
-            URH_CHECK(compute(c, s0, s1, s));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_COMPUTE][s], ctx->stream));
-            urh_stream_sample_free(ctx);
-            ctx->stream_chunks++;
-        } else {
-            cudaStream_t cp = ctx->copy_stream[1];
-            URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
-            URH_CUDA(ctx, cudaMemcpyAsync(h_qad + s0, d_qad + (qad_resident ? s0 : (int64_t)s * cs), (size_t)(s1 - s0) * sizeof(float),
-                                          cudaMemcpyDeviceToHost, cp));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_DOWNLOAD][s], cp));
-        }
-        recorded[kind][s] = true;
-    }
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream[1]));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return URH_OK;
 }
 

@@ -12,6 +12,7 @@
 // direct convolution with double accumulation — the reference's own result is a complex128 FFT product, so
 // parity is tolerance-based (1e-5 of the signal scale) as stated in BASELINE.md.
 #include "common.cuh"
+#include "stream_ring.cuh"
 
 #include <cuda/barrier>
 #include <math.h>
@@ -485,4 +486,115 @@ extern "C" int urh_dc_correction_int(urh_ctx* ctx, const void* d_iq, int dtype, 
         case URH_DT_U16: return dc_int<uint16_t>(ctx, d_iq, n, d_out);
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "urh_dc_correction_int: integer capture expected");
     }
+}
+
+// ---- host captures of any size through the windowed ring (stream_ring.cuh, DESIGN.md §4.11) ------------------------------------------
+// Each chunk runs the per-window call the sharded filters run (dist.py), on the window urh_filter_windows gives it, so its outputs are
+// the resident call's words.
+extern "C" int urh_convolve_c128_stream(urh_ctx* ctx, const float* h_x, int64_t n, const double* h_taps, int m, int64_t offset,
+                                        int64_t out_len, int64_t chunk_samples, int ring, float* h_y) {
+    if (!h_x || !h_taps || !h_y || m < 1 || offset < 0 || out_len < 0) URH_FAIL(ctx, URH_ERR_INVALID, "convolve_c128_stream: bad arguments");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_CONVOLVE, n, out_len, m, offset, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_CONVOLVE, n, out_len, URH_DT_F32, m, offset, 0, chunk_samples, L));
+    const double* d_taps = (const double*)L.extra;
+    URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_taps, (size_t)m * 16, cudaMemcpyHostToDevice, ctx->stream));
+    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                              [&](int64_t, const UrhWindow& w, int s) {
+                                  return urh_convolve_c128(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, d_taps, m,
+                                                           w.k0 + offset - w.a, w.k1 - w.k0, (float*)(L.out + s * L.z.out_slot));
+                              },
+                              contiguous_download(ctx, L, (char*)h_y, 8));
+}
+
+extern "C" int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, const float* h_taps, int m, int64_t chunk_samples, int ring,
+                                     float* h_y) {
+    if (!h_x || !h_y || m < 0 || (m > 0 && !h_taps)) URH_FAIL(ctx, URH_ERR_INVALID, "fir_filter_stream: bad arguments");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_FIR, n, n, m, 0, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_FIR, n, n, URH_DT_F32, m, 0, 0, chunk_samples, L));
+    const float* d_taps = (const float*)L.extra;
+    if (m > 0) URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_taps, (size_t)m * 8, cudaMemcpyHostToDevice, ctx->stream));
+    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                              [&](int64_t, const UrhWindow& w, int s) {
+                                  // the slot starts at the first history sample: the chunk's own samples follow k0 - a samples in
+                                  const float* x = (const float*)(L.in + s * L.z.in_slot + (w.k0 - w.a) * 8);
+                                  return urh_fir_filter_shard(ctx, x, w.k1 - w.k0, w.k0 > 0, d_taps, m, (float*)(L.out + s * L.z.out_slot));
+                              },
+                              contiguous_download(ctx, L, (char*)h_y, 8));
+}
+
+// Two passes: the column sums chunk by chunk (upload only), then the subtraction of the mean (upload, compute, download).  Both cut
+// the capture into the same chunks, so urh_stream_stats' chunk count (set by each pass) is that number; one ring serves both, so its
+// free-memory low point and arena peak cover the whole call.
+//   float32, exact_order != 0: numpy's serial float32 chain continued from chunk to chunk (bit for bit urh_dc_correction);
+//   float32, exact_order == 0: each chunk's double sums added in chunk order (dist.py dc_fold_double's rule), mean = float32(sum / n);
+//   integer: exact int64 sums, mean = sum / n in double, float64 output (bit for bit urh_dc_correction_int).
+extern "C" int urh_dc_correction_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, int exact_order, int64_t chunk_samples, int ring,
+                                        void* h_out) {
+    if (!h_iq || !h_out) URH_FAIL(ctx, URH_ERR_INVALID, "dc_correction_stream: bad arguments");
+    if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "dc_correction_stream: unknown dtype");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    if (n == 0) return URH_OK;
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_DC, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_DC, n, n, dtype, 0, 0, 0, chunk_samples, L));
+    const int ib = urh_iq_bytes(dtype);
+    const bool f32 = dtype == URH_DT_F32;
+    float carry[2] = {0.0f, 0.0f};
+    double dsum[2] = {0.0, 0.0};
+    long long isum[2] = {0, 0};
+    auto no_download = [](int64_t, const UrhWindow&, int, cudaStream_t) { return URH_OK; };
+    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
+                                 [&](int64_t, const UrhWindow& w, int s) {
+                                     const void* x = L.in + s * L.z.in_slot;
+                                     if (!f32) {
+                                         int64_t part[2];
+                                         URH_CHECK(urh_dc_int_column_sums(ctx, x, dtype, w.b - w.a, part));
+                                         isum[0] += part[0];
+                                         isum[1] += part[1];
+                                         return URH_OK;
+                                     }
+                                     double part[2];
+                                     URH_CHECK(urh_dc_column_sums(ctx, (const float*)x, w.b - w.a, exact_order, exact_order ? carry : nullptr, part));
+                                     if (exact_order) {   // float32 accumulators carried in doubles: exact
+                                         carry[0] = (float)part[0];
+                                         carry[1] = (float)part[1];
+                                     } else {
+                                         dsum[0] += part[0];
+                                         dsum[1] += part[1];
+                                     }
+                                     return URH_OK;
+                                 },
+                                 no_download));
+    float mean32[2];
+    double mean64[2];
+    if (f32 && exact_order) {
+        mean32[0] = carry[0] / (float)n;   // np.mean: sum / count in float32 (k_dc_mean_serial)
+        mean32[1] = carry[1] / (float)n;
+    } else if (f32) {
+        mean32[0] = (float)(dsum[0] / (double)n);
+        mean32[1] = (float)(dsum[1] / (double)n);
+    } else {
+        mean64[0] = (double)isum[0] / (double)n;
+        mean64[1] = (double)isum[1] / (double)n;
+    }
+    const int64_t ob = f32 ? 8 : 16;
+    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, true,
+                                 [&](int64_t, const UrhWindow& w, int s) {
+                                     const void* x = L.in + s * L.z.in_slot;
+                                     void* y = L.out + s * L.z.out_slot;
+                                     if (f32) return urh_dc_subtract(ctx, (const float*)x, w.b - w.a, mean32[0], mean32[1], (float*)y);
+                                     return urh_dc_int_subtract(ctx, x, dtype, w.b - w.a, mean64[0], mean64[1], (double*)y);
+                                 },
+                                 contiguous_download(ctx, L, (char*)h_out, ob)));
+    return URH_OK;
 }

@@ -7,11 +7,14 @@
 // shared-memory FFT -> scale / fftshift / cast / dB / flip, see k_stft_fused); other sizes use cuFFT Z2Z — for the FFT only, as
 // the north_star prescribes — between two hand-written kernels, in batches that bound the working set.
 #include "common.cuh"
+#include "stream_ring.cuh"
 
 #include <cufft.h>
 #include <limits.h>
 #include <math.h>
 #include <stdlib.h>
+
+#include <algorithm>
 
 #define URH_CUFFT(ctx, call)                                                                    \
     do {                                                                                        \
@@ -689,6 +692,104 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
     }
     cudaFreeAsync(db, ctx->stream);
     return rc;
+}
+
+// ---- host captures of any size through the windowed ring (stream_ring.cuh, DESIGN.md §4.11) ------------------------------------------
+// A chunk is a run of whole frames [f0, f1) and uploads the samples they read; the window call is the one the sharded dB map runs
+// (dist.py spectrogram_db_sharded), so every frame is the resident call's.
+static int stft_stream(urh_ctx* ctx, const float* h_x, int64_t n, int W, int hop, const double* h_window, int64_t num_frames,
+                       int64_t chunk_samples, int ring, void* h_out, int mode) {
+    if (!h_x || !h_window || !h_out || W <= 0 || hop <= 0 || num_frames <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "stft_stream: bad arguments");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    const int entry = mode == 0 ? URH_FILTER_STFT : URH_FILTER_DB;
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(entry, n, num_frames, W, hop, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, entry, n, num_frames, URH_DT_F32, W, hop, 0, chunk_samples, L));
+    const double* d_window = (const double*)L.extra;
+    URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_window, (size_t)W * 8, cudaMemcpyHostToDevice, ctx->stream));
+    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                              [&](int64_t, const UrhWindow& w, int s) {
+                                  return stft_run(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, W, hop, d_window, w.k1 - w.k0,
+                                                  L.out + s * L.z.out_slot, mode);
+                              },
+                              contiguous_download(ctx, L, (char*)h_out, (int64_t)W * (mode == 0 ? 16 : 4)));
+}
+
+extern "C" int urh_stft_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window, int64_t num_frames,
+                               int64_t chunk_samples, int ring, double* h_out) {
+    return stft_stream(ctx, h_x, n, window_size, hop, h_window, num_frames, chunk_samples, ring, h_out, 0);
+}
+
+extern "C" int urh_spectrogram_db_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
+                                         int64_t num_frames, int64_t chunk_samples, int ring, float* h_out) {
+    return stft_stream(ctx, h_x, n, window_size, hop, h_window, num_frames, chunk_samples, ring, h_out, 1);
+}
+
+// Images: a chunk is a group of whole segments (their images back to back, as the resident call writes them) or a run of frames of
+// one long segment, rendered as a segment of its own; with transpose = 0 such a piece is the column band [W][f0:f1][4] of its image.
+extern "C" int urh_spectrogram_bgra_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
+                                           const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* h_colormap,
+                                           int entries, float data_min, float data_max, int transpose, int64_t chunk_samples, int ring,
+                                           uint8_t* h_out) {
+    const int W = window_size;
+    if (!h_x || !h_window || !h_out || !h_colormap || W <= 0 || hop <= 0 || nseg <= 0)
+        URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra_stream: bad window/hop/segments");
+    if (entries <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra_stream: empty colormap");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    std::vector<UrhWindow> win;
+    if (urh_filter_windows(URH_FILTER_IMAGES, n, 0, W, hop, chunk_samples, h_seg_start, h_seg_len, nseg, win) != URH_OK)
+        URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra_stream: a segment lies outside the capture");
+    std::vector<int64_t> cum((size_t)nseg + 1, 0);   // frames before segment s
+    for (int s = 0; s < nseg; s++) cum[s + 1] = cum[s] + (h_seg_len[s] < W ? 1 : (h_seg_len[s] - W) / hop + 1);
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_IMAGES, n, cum[nseg], URH_DT_F32, W, hop, entries, chunk_samples, L));
+    const double* d_window = (const double*)L.extra;
+    const uint8_t* d_cmap = (const uint8_t*)(L.extra + r256((int64_t)W * 8));
+    URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_window, (size_t)W * 8, cudaMemcpyHostToDevice, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync((void*)d_cmap, h_colormap, (size_t)entries * 4, cudaMemcpyHostToDevice, ctx->stream));
+    // the segment holding frame k0, and whether the chunk lies within it.  Such a chunk (a run of its frames, or all of them) is
+    // rendered as a segment of its own over the uploaded window, which holds exactly what its frames read and may end before the
+    // segment does; its frame count from that window is the chunk's.  Other chunks are runs of whole segments.
+    auto locate = [&](const UrhWindow& w, bool* piece) {
+        const int s = (int)(std::upper_bound(cum.begin(), cum.end(), w.k0) - cum.begin()) - 1;
+        *piece = w.k1 <= cum[s + 1];
+        return s;
+    };
+    return stream_run_windows(
+        ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+        [&](int64_t, const UrhWindow& w, int slot) {
+            bool piece;
+            const int s = locate(w, &piece);
+            std::vector<int64_t> st, len;
+            if (piece) {
+                st.push_back(0);
+                len.push_back(w.b - w.a);
+            } else {
+                for (int q = s; q < nseg && cum[q] < w.k1; q++) {
+                    st.push_back(h_seg_start[q] - w.a);
+                    len.push_back(h_seg_len[q]);
+                }
+            }
+            return urh_spectrogram_bgra(ctx, (const float*)(L.in + slot * L.z.in_slot), w.b - w.a, W, hop, d_window, st.data(), len.data(),
+                                        (int)st.size(), d_cmap, entries, data_min, data_max, transpose, (uint8_t*)(L.out + slot * L.z.out_slot));
+        },
+        [&](int64_t, const UrhWindow& w, int slot, cudaStream_t cp) {
+            bool piece;
+            const int s = locate(w, &piece);
+            const char* src = L.out + slot * L.z.out_slot;
+            const int64_t nf = w.k1 - w.k0;
+            if (piece && !transpose) {   // rows of nf pixels into rows of the segment's F pixels (one copy when nf = F)
+                const int64_t F = cum[s + 1] - cum[s];
+                URH_CUDA(ctx, cudaMemcpy2DAsync(h_out + (cum[s] * W + (w.k0 - cum[s])) * 4, (size_t)F * 4, src, (size_t)nf * 4, (size_t)nf * 4,
+                                                (size_t)W, cudaMemcpyDeviceToHost, cp));
+            } else {
+                URH_CUDA(ctx, cudaMemcpyAsync(h_out + w.k0 * W * 4, src, (size_t)(nf * W * 4), cudaMemcpyDeviceToHost, cp));
+            }
+            return URH_OK;
+        });
 }
 
 // out[i] = x[start + i * step] (complex64 samples; Python slice semantics, step may be negative)

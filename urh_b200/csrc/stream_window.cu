@@ -1,0 +1,255 @@
+// The windowed ring's plan (DESIGN.md §4.11, "The windowed ring"): which outputs each chunk of a streamed filter or spectrogram call
+// owns, which input window it uploads, the order of its copies and computations, and the device bytes of the streamed and the
+// resident form of each entry.  Host code only: everything here runs without a device.
+#include "stream_ring.cuh"
+
+static int64_t filter_chunk(int64_t cs) { return cs > 0 ? cs : (int64_t)1 << 24; }
+static int64_t frames_per_chunk(int64_t cs, int64_t hop) { return cs / hop > 0 ? cs / hop : 1; }
+// frames of a segment of len samples, as Spectrogram.stft and urh_spectrogram_bgra count them (short segments: one frame)
+static int64_t frames_of(int64_t len, int64_t W, int64_t hop) { return len < W ? 1 : (len - W) / hop + 1; }
+static int64_t clamp64(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+int urh_filter_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples, const int64_t* h_seg_start,
+                       const int64_t* h_seg_len, int nseg, std::vector<UrhWindow>& out) {
+    out.clear();
+    if (n < 0 || out_len < 0) return URH_ERR_INVALID;
+    int64_t cs = filter_chunk(chunk_samples);
+    switch (entry) {
+        case URH_FILTER_CONVOLVE: {   // output k reads x[k + offset - (m - 1) .. k + offset]
+            const int64_t m = p0, off = p1;
+            if (m < 1 || off < 0) return URH_ERR_INVALID;
+            for (int64_t k0 = 0; k0 < out_len; k0 += cs) {
+                const int64_t k1 = k0 + cs < out_len ? k0 + cs : out_len;
+                const int64_t b = clamp64(k1 + off, 0, n);
+                const int64_t a = clamp64(k0 + off - (m - 1), 0, b);
+                out.push_back({k0, k1, a, b});
+            }
+            return URH_OK;
+        }
+        case URH_FILTER_FIR: {   // output k reads x[k - (m - 1) .. k]; a chunk is at least the history long
+            if (p0 < 0) return URH_ERR_INVALID;
+            const int64_t h = p0 > 1 ? p0 - 1 : 0;
+            if (cs < h) cs = h;
+            for (int64_t k0 = 0; k0 < n; k0 += cs) {
+                const int64_t k1 = k0 + cs < n ? k0 + cs : n;
+                out.push_back({k0, k1, k0 > 0 ? k0 - h : 0, k1});
+            }
+            return URH_OK;
+        }
+        case URH_FILTER_DC:
+            for (int64_t k0 = 0; k0 < n; k0 += cs) out.push_back({k0, k0 + cs < n ? k0 + cs : n, k0, k0 + cs < n ? k0 + cs : n});
+            return URH_OK;
+        case URH_FILTER_STFT:
+        case URH_FILTER_DB: {   // frame f reads x[f hop .. f hop + W - 1]
+            const int64_t W = p0, hop = p1;
+            if (W <= 0 || hop <= 0) return URH_ERR_INVALID;
+            const int64_t fpc = frames_per_chunk(cs, hop);
+            for (int64_t f0 = 0; f0 < out_len; f0 += fpc) {
+                const int64_t f1 = f0 + fpc < out_len ? f0 + fpc : out_len;
+                const int64_t b = clamp64((f1 - 1) * hop + W, 0, n);
+                out.push_back({f0, f1, clamp64(f0 * hop, 0, b), b});
+            }
+            return URH_OK;
+        }
+        case URH_FILTER_IMAGES: {
+            // Outputs are the frames of all segments in segment order (the images back to back).  Whole segments are grouped while
+            // the group's samples fit a chunk and its frames fit frames_per_chunk; a segment that fits neither alone is cut by frames
+            // into pieces of frames_per_chunk frames (what urh_spectrogram_db does with a window of frames).  A chunk within one
+            // segment (a piece, or a group of one) uploads exactly the samples its frames read, which may end before the segment does.
+            const int64_t W = p0, hop = p1;
+            if (W <= 0 || hop <= 0 || nseg < 0 || (nseg > 0 && (!h_seg_start || !h_seg_len))) return URH_ERR_INVALID;
+            const int64_t fpc = frames_per_chunk(cs, hop);
+            auto reach = [&](int64_t f1, int64_t len) { return (f1 - 1) * hop + W < len ? (f1 - 1) * hop + W : len; };   // read by frames < f1
+            int64_t k = 0;              // frames before segment s
+            int64_t g0 = -1, ga = 0, gb = 0;   // the open group: its first frame and its sample window
+            int gn = 0;                        // its segments
+            auto close = [&]() {
+                if (g0 >= 0) {
+                    if (gn == 1) gb = ga + reach(k - g0, gb - ga);
+                    out.push_back({g0, k, ga, gb});
+                }
+                g0 = -1;
+                gn = 0;
+            };
+            for (int s = 0; s < nseg; s++) {
+                const int64_t st = h_seg_start[s], len = h_seg_len[s];
+                if (st < 0 || len < 0 || st + len > n) return URH_ERR_INVALID;
+                const int64_t F = frames_of(len, W, hop);
+                if (len > cs || F > fpc) {
+                    close();
+                    for (int64_t f0 = 0; f0 < F; f0 += fpc) {
+                        const int64_t f1 = f0 + fpc < F ? f0 + fpc : F;
+                        out.push_back({k + f0, k + f1, st + f0 * hop, st + reach(f1, len)});
+                    }
+                    k += F;
+                    continue;
+                }
+                if (g0 >= 0) {
+                    const int64_t a = ga < st ? ga : st, b = gb > st + len ? gb : st + len;
+                    if (b - a > cs || k + F - g0 > fpc) close();
+                }
+                if (g0 < 0) {
+                    g0 = k; ga = st; gb = st + len;
+                } else {
+                    ga = ga < st ? ga : st;
+                    gb = gb > st + len ? gb : st + len;
+                }
+                gn++;
+                k += F;
+            }
+            close();
+            return URH_OK;
+        }
+        default: return URH_ERR_INVALID;
+    }
+}
+
+extern "C" int urh_stream_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples,
+                                  const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, int64_t* h_win, int64_t cap, int64_t* count) {
+    if (!count) return URH_ERR_INVALID;
+    std::vector<UrhWindow> w;
+    URH_CHECK(urh_filter_windows(entry, n, out_len, p0, p1, chunk_samples, h_seg_start, h_seg_len, nseg, w));
+    *count = (int64_t)w.size();
+    if (!h_win) return URH_OK;
+    if ((int64_t)w.size() > cap) return URH_ERR_INVALID;
+    memcpy(h_win, w.data(), w.size() * sizeof(UrhWindow));
+    return URH_OK;
+}
+
+// The op order of urh_stream_schedule (uploads R - 1 chunks ahead, each compute followed by its download), 7 int64 per op.
+extern "C" int urh_stream_window_schedule(const int64_t* h_win, int64_t chunks, int ring, int flags, int64_t* h_ops, int64_t cap,
+                                          int64_t* count) {
+    if (!count || chunks < 0 || (chunks > 0 && !h_win) || ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
+    const bool up = flags & URH_STREAM_UPLOAD, down = flags & URH_STREAM_DOWNLOAD;
+    int64_t k = 0;
+    auto emit = [&](int64_t kind, int64_t c) {
+        if (h_ops && k < cap) {
+            int64_t* o = h_ops + 7 * k;
+            o[0] = kind; o[1] = c; o[2] = c % ring;
+            memcpy(o + 3, h_win + 4 * c, 4 * sizeof(int64_t));
+        }
+        k++;
+    };
+    if (up)
+        for (int64_t c = 0; c < ring - 1 && c < chunks; c++) emit(URH_OP_UPLOAD, c);
+    for (int64_t c = 0; c < chunks; c++) {
+        if (up && c + ring - 1 < chunks) emit(URH_OP_UPLOAD, c + ring - 1);
+        emit(URH_OP_COMPUTE, c);
+        if (down) emit(URH_OP_DOWNLOAD, c);
+    }
+    *count = k;
+    return (h_ops && k > cap) ? URH_ERR_INVALID : URH_OK;
+}
+
+// ---- device bytes --------------------------------------------------------------------------------------------------------------------
+// scratch of a window call of nf frames (spectrogram.cu stft_run): the fused kernel's twiddles, or the cuFFT path's batch of complex128
+// frames (at most 512 MiB) and a work area of the same size for cuFFT
+static int64_t frames_work(int64_t W, int64_t nf) {
+    const int64_t max_batch = ((int64_t)512 << 20) / (W * 16) > 0 ? ((int64_t)512 << 20) / (W * 16) : 1;
+    const int64_t batch = nf < max_batch ? (nf > 0 ? nf : 1) : max_batch;
+    return r256(W * 16) + 2 * r256(batch * W * 16);
+}
+// the composed image path's dB rows (urh_spectrogram_bgra: at most 256 MiB) and the fused path's segment table
+static int64_t image_work(int64_t W, int64_t nf) {
+    const int64_t rows = ((int64_t)256 << 20) / (W * 4) > 0 ? ((int64_t)256 << 20) / (W * 4) : 1;
+    return r256((nf < rows ? nf : rows) * W * 4) + r256(nf * 40);
+}
+
+static int out_bytes_dc(int dtype) { return dtype == URH_DT_F32 ? 8 : 16; }
+
+FilterStreamSizes urh_filter_stream_sizes(int entry, int64_t n, int64_t out_len, int dtype, int64_t p0, int64_t p1, int64_t p2,
+                                          int64_t chunk_samples) {
+    (void)out_len;
+    FilterStreamSizes z{0, 0, 0, 0};
+    int64_t cs = filter_chunk(chunk_samples);
+    switch (entry) {
+        case URH_FILTER_CONVOLVE:
+            z.in_slot = r256((cs + p0 - 1) * 8);
+            z.out_slot = r256(cs * 8);
+            z.extra = r256(p0 * 16);
+            break;
+        case URH_FILTER_FIR: {
+            const int64_t h = p0 > 1 ? p0 - 1 : 0;
+            if (cs < h) cs = h;
+            z.in_slot = r256((cs + h) * 8);
+            z.out_slot = r256(cs * 8);
+            z.extra = r256((p0 > 1 ? p0 : 1) * 8);
+            break;
+        }
+        case URH_FILTER_DC:
+            z.in_slot = r256(cs * urh_iq_bytes(dtype));
+            z.out_slot = r256(cs * out_bytes_dc(dtype));
+            z.work = 3 * r256(4096 * 16);   // column partials of up to 4096 blocks, the sums, the mean
+            break;
+        case URH_FILTER_STFT:
+        case URH_FILTER_DB: {
+            const int64_t fpc = frames_per_chunk(cs, p1);
+            const int64_t in = (fpc - 1) * p1 + p0;
+            z.in_slot = r256((in < n ? in : n) * 8);
+            z.out_slot = r256(fpc * p0 * (entry == URH_FILTER_STFT ? 16 : 4));
+            z.extra = r256(p0 * 8);
+            z.work = frames_work(p0, fpc);
+            break;
+        }
+        case URH_FILTER_IMAGES: {
+            const int64_t fpc = frames_per_chunk(cs, p1);
+            const int64_t in = (fpc - 1) * p1 + p0 > cs ? (fpc - 1) * p1 + p0 : cs;
+            z.in_slot = r256((in < n ? in : n) * 8);
+            z.out_slot = r256(fpc * p0 * 4);
+            z.extra = r256(p0 * 8) + r256(p2 * 4);   // the window and the colormap (p2 BGRA entries)
+            z.work = frames_work(p0, fpc) + image_work(p0, fpc);
+            break;
+        }
+        default: break;
+    }
+    return z;
+}
+
+static bool filter_args_ok(int entry, int64_t n, int64_t out_len, int dtype, int64_t p0, int64_t p1, int64_t p2) {
+    if (n < 0 || out_len < 0) return false;
+    switch (entry) {
+        case URH_FILTER_CONVOLVE: return p0 >= 1 && p1 >= 0;
+        case URH_FILTER_FIR: return p0 >= 0;
+        case URH_FILTER_DC: return urh_iq_bytes(dtype) != 0;
+        case URH_FILTER_STFT:
+        case URH_FILTER_DB: return p0 > 0 && p1 > 0;
+        case URH_FILTER_IMAGES: return p0 > 0 && p1 > 0 && p2 > 0;
+        default: return false;
+    }
+}
+
+// resident: what the resident entry needs for a host capture (the capture, the whole output, the scratch of one call over all of it)
+extern "C" int urh_stream_filter_footprint(int entry, int64_t n, int64_t out_len, int dtype, int64_t p0, int64_t p1, int64_t p2,
+                                           int64_t chunk_samples, int ring, int resident, int64_t* bytes) {
+    if (!bytes || !filter_args_ok(entry, n, out_len, dtype, p0, p1, p2)) return URH_ERR_INVALID;
+    if (!resident && (ring < 2 || ring > URH_STREAM_MAX_RING)) return URH_ERR_INVALID;
+    const int64_t arena_block = (int64_t)64 << 20;   // the arena grows in blocks of at least 64 MiB
+    if (resident) {
+        int64_t b = arena_block;
+        switch (entry) {
+            case URH_FILTER_CONVOLVE: b += r256(n * 8) + r256(out_len * 8) + r256(p0 * 16); break;
+            case URH_FILTER_FIR: b += 2 * r256(n * 8) + r256((p0 > 1 ? p0 : 1) * 8); break;
+            case URH_FILTER_DC: b += r256(n * urh_iq_bytes(dtype)) + r256(n * out_bytes_dc(dtype)) + 3 * r256(4096 * 16); break;
+            case URH_FILTER_STFT:
+            case URH_FILTER_DB:
+                b += r256(n * 8) + r256(out_len * p0 * (entry == URH_FILTER_STFT ? 16 : 4)) + r256(p0 * 8) + frames_work(p0, out_len);
+                break;
+            case URH_FILTER_IMAGES:
+                b += r256(n * 8) + r256(out_len * p0 * 4) + r256(p0 * 8) + r256(p2 * 4) + frames_work(p0, out_len) +
+                     image_work(p0, out_len);
+                break;
+        }
+        *bytes = b;
+        return URH_OK;
+    }
+    const FilterStreamSizes z = urh_filter_stream_sizes(entry, n, out_len, dtype, p0, p1, p2, chunk_samples);
+    // arena requests: at most twice what is asked plus one block (urh_stream_footprint's rule)
+    *bytes = ring * (z.in_slot + z.out_slot) + z.extra + 2 * z.work + arena_block;
+    return URH_OK;
+}
+
+int urh_filter_stream_check(urh_ctx* ctx, int64_t n, int ring) {
+    if (n < 0) URH_FAIL(ctx, URH_ERR_INVALID, "streamed filter: negative length");
+    if (ring < 2 || ring > URH_STREAM_MAX_RING) URH_FAIL(ctx, URH_ERR_INVALID, "streamed filter: ring of %d slots (2 .. 8)", ring);
+    return URH_OK;
+}

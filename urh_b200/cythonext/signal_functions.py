@@ -74,6 +74,30 @@ def use_stream(n: int, dtype, tolerance: int, entry: int, budget: int) -> bool:
     return stream_footprint(n, dtype, tolerance, entry | _lib.STREAM_RESIDENT, rows=-2) > budget
 
 
+# The band-pass, FIR and DC filters and the spectrogram stream through the windowed ring (urh_*_stream of filter.cu and spectrogram.cu,
+# DESIGN.md §4.11) on the same rule: a host input whose resident call does not fit the device budget.
+FILTER_STREAM_CHUNK = 1 << 24
+
+
+def filter_footprint(entry: int, n: int, out_len: int, dtype, p0: int, p1: int, chunk_samples: int = FILTER_STREAM_CHUNK,
+                     ring: int = STREAM_RING, resident: bool = False, cmap_entries: int = 0) -> int:
+    """device bytes of a streamed filter / spectrogram call (entry = _lib.FILTER_*; p0, p1 = taps and offset, or W and hop;
+    cmap_entries: the colormap's entries, images only), or of its resident call fed from the host with resident=True; no device
+    involved (urh_stream_filter_footprint)"""
+    out = C.c_int64(0)
+    rc = _lib.load_library().urh_stream_filter_footprint(int(entry), int(n), int(out_len), _lib.dtype_code(dtype), int(p0), int(p1),
+                                                         int(cmap_entries), int(chunk_samples), int(ring), int(bool(resident)),
+                                                         C.byref(out))
+    if rc != _lib.URH_OK:
+        raise ValueError("urh_stream_filter_footprint: invalid arguments")
+    return out.value
+
+
+def filter_use_stream(entry: int, n: int, out_len: int, dtype, p0: int, p1: int, budget: int, cmap_entries: int = 0) -> bool:
+    """stream when the resident call's footprint exceeds the budget (use_stream's rule)"""
+    return filter_footprint(entry, n, out_len, dtype, p0, p1, resident=True, cmap_entries=cmap_entries) > budget
+
+
 def _host_ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -449,6 +473,11 @@ def fir_filter(input_samples, filter_taps):
         input_samples = np.ascontiguousarray(input_samples)
     taps = np.ascontiguousarray(np.asarray(filter_taps, dtype=np.complex64))
     n = len(input_samples)
+    if not on_device and n and filter_use_stream(_lib.FILTER_FIR, n, n, np.float32, len(taps), 0, device_budget(ctx)):
+        host = np.empty(n, dtype=np.complex64)
+        ctx.check(ctx.lib.urh_fir_filter_stream(ctx.handle, _host_ptr(input_samples), n, _host_ptr(taps) if len(taps) else None, len(taps),
+                                                FILTER_STREAM_CHUNK, STREAM_RING, _host_ptr(host)))
+        return host
     out = DeviceArray(ctx, (n,), np.complex64)
     if n:
         d = input_samples if on_device else to_device(input_samples.view(np.float32), ctx)

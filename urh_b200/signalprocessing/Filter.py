@@ -43,6 +43,9 @@ class Filter(object):
                 raise ValueError("dc_correction expects an (n, 2) capture of int8/uint8/int16/uint16/float32")
             if len(x) == 0:
                 return x.astype(np.float64)
+            streamed = Filter._dc_correction_stream(x, 1, ctx)
+            if streamed is not None:
+                return streamed
             d = to_device(x, ctx)
             out = DeviceArray(ctx, x.shape, np.float64)
             ctx.check(ctx.lib.urh_dc_correction_int(ctx.handle, C.c_void_p(d.ptr), _lib.dtype_code(x.dtype), len(x), C.c_void_p(out.ptr)))
@@ -52,10 +55,27 @@ class Filter(object):
         n = len(x)
         if n == 0:
             return x.copy()
+        streamed = Filter._dc_correction_stream(x, int(n <= Filter.EXACT_DC_MAX), ctx)
+        if streamed is not None:
+            return streamed
         d = to_device(x, ctx)
         out = DeviceArray(ctx, x.shape, np.float32)
         ctx.check(ctx.lib.urh_dc_correction(ctx.handle, C.c_void_p(d.ptr), n, C.c_void_p(out.ptr), int(n <= Filter.EXACT_DC_MAX)))
         return out.get()
+
+    @staticmethod
+    def _dc_correction_stream(x: np.ndarray, exact_order: int, ctx):
+        """dc_correction of a host capture through the windowed ring when the resident call does not fit the device budget (None:
+        it fits).  Bit for bit the resident result, except float32 above EXACT_DC_MAX, whose double column sums are added chunk by
+        chunk: the mean is float32(float64 mean) there as well."""
+        n = len(x)
+        if not signal_functions.filter_use_stream(_lib.FILTER_DC, n, n, x.dtype, 0, 0, signal_functions.device_budget(ctx)):
+            return None
+        out = np.empty(x.shape, dtype=np.float32 if x.dtype == np.float32 else np.float64)
+        ctx.check(ctx.lib.urh_dc_correction_stream(ctx.handle, x.ctypes.data_as(C.c_void_p), _lib.dtype_code(x.dtype), n, int(exact_order),
+                                                   signal_functions.FILTER_STREAM_CHUNK, signal_functions.STREAM_RING,
+                                                   out.ctypes.data_as(C.c_void_p)))
+        return out
 
     def apply_fir_filter(self, input_signal: np.ndarray) -> np.ndarray:
         if input_signal.dtype != np.complex64:
@@ -85,10 +105,19 @@ class Filter(object):
 
     @staticmethod
     def _convolve_full_slice(data: np.ndarray, h: np.ndarray, offset: int, out_len: int) -> np.ndarray:
-        """full_convolution(data, h)[offset : offset + out_len] on the GPU (complex128 taps, double accumulation)"""
+        """full_convolution(data, h)[offset : offset + out_len] on the GPU (complex128 taps, double accumulation); a host capture whose
+        resident call does not fit the device budget streams through the windowed ring"""
         ctx = _lib.default_context()
         x = np.ascontiguousarray(data, dtype=np.complex64)
         taps = np.ascontiguousarray(h, dtype=np.complex128)
+        if (len(x) and len(taps) and out_len > 0
+                and signal_functions.filter_use_stream(_lib.FILTER_CONVOLVE, len(x), out_len, np.float32, len(taps), offset,
+                                                       signal_functions.device_budget(ctx))):
+            out = np.empty(out_len, dtype=np.complex64)
+            ctx.check(ctx.lib.urh_convolve_c128_stream(ctx.handle, x.ctypes.data_as(C.c_void_p), len(x), taps.ctypes.data_as(C.c_void_p),
+                                                       len(taps), int(offset), int(out_len), signal_functions.FILTER_STREAM_CHUNK,
+                                                       signal_functions.STREAM_RING, out.ctypes.data_as(C.c_void_p)))
+            return out
         d_x = to_device(x.view(np.float32), ctx)
         d_t = to_device(taps.view(np.float64), ctx)
         out = DeviceArray(ctx, (out_len,), np.complex64)

@@ -8,6 +8,7 @@ import math
 import numpy as np
 
 from .. import _lib
+from ..cythonext import signal_functions as sf
 from ..device import DeviceArray, PinnedArray, to_device
 from .IQArray import IQArray
 
@@ -76,8 +77,22 @@ class Spectrogram(object):
 
     def _run(self, samples, mode, keep=False):
         ctx = _lib.default_context()
-        d_x, n = self._device_samples(samples, ctx)
         W, hop = int(self.window_size), int(self.hop_size)
+        if not keep and not isinstance(samples, DeviceArray):
+            # a host capture whose resident call does not fit the device budget: frames streamed through the windowed ring
+            x = np.ascontiguousarray(samples, dtype=np.complex64)
+            n = len(x)
+            frames = self._num_frames(n)
+            entry = _lib.FILTER_STFT if mode == 0 else _lib.FILTER_DB
+            if n and sf.filter_use_stream(entry, n, frames, np.float32, W, hop, sf.device_budget(ctx)):
+                out = np.empty((frames, W), dtype=np.complex128 if mode == 0 else np.float32)
+                call = ctx.lib.urh_stft_stream if mode == 0 else ctx.lib.urh_spectrogram_db_stream
+                w = np.ascontiguousarray(self.window_function(W), dtype=np.float64)
+                ctx.check(call(ctx.handle, x.ctypes.data_as(C.c_void_p), n, W, hop, w.ctypes.data_as(C.c_void_p), frames,
+                               sf.FILTER_STREAM_CHUNK, sf.STREAM_RING, out.ctypes.data_as(C.c_void_p)))
+                return out
+            samples = x
+        d_x, n = self._device_samples(samples, ctx)
         frames = self._num_frames(n)
         d_w = self._window(ctx)
         if mode == 0:
@@ -158,6 +173,29 @@ class Spectrogram(object):
                                                int(bool(transpose)), C.c_void_p(out.ptr)))
         return out, shapes
 
+    def _stream_images(self, x, segments, transpose, cmap, ctx):
+        """the images of _images from a host capture (numpy arrays) through the windowed ring, when the resident call does not fit the
+        device budget (None: it fits)"""
+        W, hop = int(self.window_size), int(self.hop_size)
+        frames = [self._num_frames(int(ln)) for _, ln in segments]
+        if not len(x) or not sf.filter_use_stream(_lib.FILTER_IMAGES, len(x), sum(frames), np.float32, W, hop, sf.device_budget(ctx),
+                                                  cmap_entries=len(cmap)):
+            return None
+        starts = np.array([s for s, _ in segments], dtype=np.int64)
+        lens = np.array([ln for _, ln in segments], dtype=np.int64)
+        out = np.empty(sum(frames) * W * 4, dtype=np.uint8)
+        w = np.ascontiguousarray(self.window_function(W), dtype=np.float64)
+        ctx.check(ctx.lib.urh_spectrogram_bgra_stream(ctx.handle, x.ctypes.data_as(C.c_void_p), len(x), W, hop, w.ctypes.data_as(C.c_void_p),
+                                                      starts.ctypes.data_as(C.c_void_p), lens.ctypes.data_as(C.c_void_p), len(segments),
+                                                      cmap.ctypes.data_as(C.c_void_p), len(cmap), float(self.data_min), float(self.data_max),
+                                                      int(bool(transpose)), sf.FILTER_STREAM_CHUNK, sf.STREAM_RING,
+                                                      out.ctypes.data_as(C.c_void_p)))
+        images, off = [], 0
+        for f in frames:
+            images.append(out[off: off + f * W * 4].reshape((f, W, 4) if transpose else (W, f, 4)))
+            off += f * W * 4
+        return images
+
     @staticmethod
     def _split(out, shapes, on_device):
         """the images of one buffer: DeviceArray views, or numpy views of one download"""
@@ -190,7 +228,11 @@ class Spectrogram(object):
                 ctx.check(ctx.lib.urh_gather_samples(ctx.handle, C.c_void_p(samples.ptr), n, start, st, count, C.c_void_p(d_x.ptr)))
                 n, seg = count, (0, count)
         else:
-            d_x, n = self._device_samples(samples[sample_start:sample_end:step], ctx)
+            x = np.ascontiguousarray(samples[sample_start:sample_end:step], dtype=np.complex64)
+            streamed = self._stream_images(x, [(0, len(x))], transpose, cmap, ctx)
+            if streamed is not None:
+                return streamed[0]
+            d_x, n = self._device_samples(x, ctx)
             seg = (0, n)
         out, shapes = self._images(d_x, n, [seg], transpose, cmap, ctx)
         return next(self._split(out, shapes, on_device))
@@ -202,8 +244,14 @@ class Spectrogram(object):
         if not bounds:
             return
         ctx = _lib.default_context()
+        segments = [(s, e - s) for s, e, _ in bounds]
+        if not isinstance(self.samples, DeviceArray):
+            streamed = self._stream_images(np.ascontiguousarray(self.samples, dtype=np.complex64), segments, False, cmap, ctx)
+            if streamed is not None:
+                yield from streamed
+                return
         d_x, n = self._device_samples(self.samples, ctx)   # uploaded once
-        out, shapes = self._images(d_x, n, [(s, e - s) for s, e, _ in bounds], False, cmap, ctx)
+        out, shapes = self._images(d_x, n, segments, False, cmap, ctx)
         yield from self._split(out, shapes, isinstance(self.samples, DeviceArray))
 
     # ---- FTA export (Spectrogram.py:118-154) ------------------------------------------------------------------------------------
