@@ -52,36 +52,15 @@ template <typename T> struct UrhVec2;
 template <> struct UrhVec2<float> { typedef float2 type; };
 template <> struct UrhVec2<double> { typedef double2 type; };
 
+// One tile (warp-uniform): classify, track runs, write the summary and the staged candidates.
 template <typename SRC, typename T>
-__global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32)
-k_dense_f32(const T* __restrict__ x, int64_t n, int vec_in, const __grid_constant__ UrhClassify cls, int tol,
-            UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
-            int16_t* __restrict__ init_cls, int cls_of_zero, const float* __restrict__ d_thr0 = nullptr,
-            const UrhTileStats* __restrict__ tile_stats = nullptr, const UrhSpec spec = UrhSpec{}) {
-    // d_thr0: the (binary) threshold lives in device memory (center detected on the device); then cls_of_zero is derived here
-    const float thr0 = d_thr0 ? *d_thr0 : cls.thr[0];
-    if (d_thr0) cls_of_zero = (0.0f <= thr0) ? 0 : 1;
-    const int lane = threadIdx.x & 31;
-    const int64_t tile = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
+__device__ __forceinline__ void dense_f32_tile(const T* __restrict__ x, int64_t n, int vec_in, const UrhClassify& cls, float thr0, int tol,
+                                               UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
+                                               int16_t* __restrict__ init_cls, int cls_of_zero, const UrhTileStats* __restrict__ tile_stats,
+                                               int64_t tile, int lane) {
     const int64_t tile_start = tile * URH_TILE;
-    if (tile_start >= n) return;
     const int tile_len = (int)((n - tile_start) < URH_TILE ? (n - tile_start) : URH_TILE);
     const int iters = (tile_len + 63) >> 6;
-    // the demodulator's tile table says the whole tile is NOISE: one run of class -1, nothing to read (captures are mostly silence)
-    if (tile_stats && tile_stats[tile].all_noise) {
-        if (lane == 0) {
-            UrhTileSummary s;
-            s.first_cls = -1; s.last_cls = -1; s.head_len = tile_len; s.tail_len = tile_len; s.ncand = 0;
-            tiles[tile] = s;
-            if (tile_start == 0 && init_cls) *init_cls = (int16_t)-1;
-        }
-        return;
-    }
-    // the demodulation pass digitized the tile at the guess t_g: keep its result when the margin proves the classes (UrhSpec)
-    if (tile >= spec.lo && tile < spec.hi) {
-        if (spec.margin[tile] > fabsf(__fsub_rn(thr0, *spec.tg))) return;
-        if (lane == 0) atomicAdd(spec.redone, 1u);
-    }
     UrhRunTracker rt;
     rt.init(tol, staging + tile * (int64_t)stage_cap);
     if (vec_in && tile_len == URH_TILE) {
@@ -172,3 +151,41 @@ k_dense_f32(const T* __restrict__ x, int64_t n, int vec_in, const __grid_constan
     rt.finish(tile_len, tiles + tile, lane);
 }
 
+// Warp-stride loop over tiles: warp w digitizes tiles w, w + W, w + 2W, ... (W warps in the grid).  A grid of one warp per tile runs
+// the loop once per warp; the detect step's pass after speculation runs a grid sized to the GPU, because it redoes a handful of tiles
+// and one block per eight tiles would cost more in block launches than the work.  Lane i triages the warp's (i+1)-th next tile, so
+// the checks that skip a tile cost one load per 32 tiles: an all-NOISE tile first, then the speculation proof, then the count.
+template <typename SRC, typename T>
+__global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32)
+k_dense_f32(const T* __restrict__ x, int64_t n, int vec_in, const __grid_constant__ UrhClassify cls, int tol,
+            UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
+            int16_t* __restrict__ init_cls, int cls_of_zero, const float* __restrict__ d_thr0 = nullptr,
+            const UrhTileStats* __restrict__ tile_stats = nullptr, const UrhSpec spec = UrhSpec{}) {
+    // d_thr0: the (binary) threshold lives in device memory (center detected on the device); then cls_of_zero is derived here
+    const float thr0 = d_thr0 ? *d_thr0 : cls.thr[0];
+    if (d_thr0) cls_of_zero = (0.0f <= thr0) ? 0 : 1;
+    const int lane = threadIdx.x & 31;
+    const int64_t ntiles = urh_div_up(n, URH_TILE);
+    const int64_t stride = (int64_t)gridDim.x * URH_WARPS_PER_BLOCK;
+    for (int64_t t0 = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5); t0 < ntiles; t0 += 32 * stride) {
+        const int64_t mine = t0 + lane * stride;
+        bool work = mine < ntiles;
+        if (work && tile_stats && tile_stats[mine].all_noise) {
+            // the demodulator's tile table says the whole tile is NOISE: one run of class -1, nothing to read (captures are mostly silence)
+            const int64_t rem = n - mine * URH_TILE;
+            const int tile_len = rem < URH_TILE ? (int)rem : URH_TILE;
+            UrhTileSummary s;
+            s.first_cls = -1; s.last_cls = -1; s.head_len = tile_len; s.tail_len = tile_len; s.ncand = 0;
+            tiles[mine] = s;
+            if (mine == 0 && init_cls) *init_cls = (int16_t)-1;
+            work = false;
+        } else if (work && mine >= spec.lo && mine < spec.hi) {
+            // the demodulation pass digitized the tile at the guess t_g: keep its result when the margin proves the classes (UrhSpec)
+            if (spec.margin[mine] > fabsf(__fsub_rn(thr0, *spec.tg))) work = false;
+            else atomicAdd(spec.redone, 1u);
+        }
+        for (unsigned m = __ballot_sync(URH_FULL_MASK, work); m; m &= m - 1)
+            dense_f32_tile<SRC, T>(x, n, vec_in, cls, thr0, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, tile_stats,
+                                   t0 + (int64_t)(__ffs(m) - 1) * stride, lane);
+    }
+}

@@ -1078,7 +1078,15 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     } else {
         URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
         const int vec_in = (((uintptr_t)d_qad_out % 8) == 0) ? 1 : 0;
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK), URH_WARPS_PER_BLOCK * 32, 0,
+        // after speculation most tiles only need their margin checked: one resident wave of warps loops over them (k_dense_f32)
+        int64_t grid = urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
+        if (speculate) {
+            int per_sm = 0;
+            URH_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dense_f32<SrcQad2, float>, URH_WARPS_PER_BLOCK * 32, 0));
+            const int64_t resident = (int64_t)ctx->sm_count * (per_sm > 0 ? per_sm : 1);
+            if (grid > resident) grid = resident;
+        }
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)grid, URH_WARPS_PER_BLOCK * 32, 0,
                    (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts, spec);
         URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));

@@ -6,13 +6,17 @@
 //
 //   A  run carry           exclusive scan of {class, length, whole?} of each tile's closing run  -> carry[t]
 //   B  candidates          per tile: head candidate from carry[t] (+ the carry of the preceding shards), number of
-//                          candidates, class of the last one; scan -> class of the candidate preceding the tile
-//   C  firings             per tile: walk its candidates (a candidate fires iff its class differs from the one
-//                          before it), count firings, position of the last; scan -> row offset, previous firing
+//                          candidates, class of the last one; scan -> class of the candidate preceding the tile.  The
+//                          same walk over the staged words leaves the tile's firings apart from its first candidate's
+//                          (a candidate fires iff its class differs from the one before it) -> fire[t]
+//   C  firings             per tile: fire[t] plus the first candidate's firing against the preceding class (O(1));
+//                          scan -> row offset, previous firing
 //   D  rows                per tile: walk again, write (state, length) rows at the tile's row offset; the last
 //                          tile appends the tail row (pyx:485-493) and the row count
-// (C and D run one THREAD per tile: a tile holds ~20 candidates, and 32 independent walks per warp keep far more loads in
-// flight than one warp per tile would.)
+// B walks one THREAD per tile (it reads the staging row for the last class anyway, and counting needs no more than that).
+// D runs one WARP per 32 consecutive tiles: the lanes take 32 candidates of a tile at once, the firings come from a ballot,
+// and the rows of one chunk land at consecutive addresses.  The first 32 staged words of eight tiles are loaded before the
+// first of them is walked.
 //
 // One read-back (row count) ends the call.  Rows go straight into the context's pulse buffer, sized optimistically;
 // an overflow only repeats stage D.  ASK (short pauses relabelled, pyx:471-473, so equal neighbours can meet) runs a
@@ -75,6 +79,14 @@ struct ScanRunCarry {
 };
 
 // ---- B ---------------------------------------------------------------------------------------------------------------
+// The tile's candidates apart from the class that precedes them: its first candidate, and the firings after it (each candidate
+// against the one before it inside the tile).  Stage C decides the first one's firing once the preceding class is known.
+struct __align__(16) TileFire {
+    int32_t first_cls;   // class of the first candidate (CLS_NONE: the tile has none)
+    int32_t first_rel;   // its tile-relative position
+    int32_t fired;       // firings among the later candidates
+    int32_t last_rel;    // tile-relative position of the last of those (-1: none)
+};
 struct ScanCandidates {
     const UrhTileSummary* tiles;
     const uint32_t* staging;
@@ -84,6 +96,7 @@ struct ScanCandidates {
     int tol;
     int32_t* head_rel;
     int32_t* prev_cls;
+    TileFire* fire;
     __device__ __forceinline__ CandAgg load(int64_t t) const {
         const UrhTileSummary s = tiles[t];
         RunCarry c = carry[t];
@@ -93,11 +106,40 @@ struct ScanCandidates {
         int32_t rel = -1;
         if (start_len <= tol && (int64_t)tol < start_len + s.head_len) rel = (int32_t)(tol - start_len);
         head_rel[t] = rel;
+        TileFire f;
+        f.first_cls = CLS_NONE; f.first_rel = -1; f.fired = 0; f.last_rel = -1;
+        int prev = CLS_NONE;
+        if (rel >= 0) {
+            prev = s.first_cls;
+            f.first_cls = prev;
+            f.first_rel = rel;
+        }
+        // the staged words (~20 per tile on the bench capture), four loads in flight
+        const uint32_t* st = staging + t * (int64_t)stage_cap;
+        for (int j = 0; j < s.ncand; j += 4) {
+            uint32_t w[4];
+#pragma unroll
+            for (int u = 0; u < 4; u++) w[u] = (j + u < s.ncand) ? st[j + u] : 0u;
+#pragma unroll
+            for (int u = 0; u < 4; u++) {
+                if (j + u < s.ncand) {
+                    const int cl = (int)(w[u] & 0xffffu) - 1;
+                    const int p = (int)(w[u] >> 16);
+                    if (prev == CLS_NONE) {
+                        f.first_cls = cl;
+                        f.first_rel = p;
+                    } else if (cl != prev) {
+                        f.fired++;
+                        f.last_rel = p;
+                    }
+                    prev = cl;
+                }
+            }
+        }
+        fire[t] = f;
         CandAgg r;
         r.cnt = (int64_t)s.ncand + (rel >= 0 ? 1 : 0);
-        r.last_cls = CLS_NONE;
-        if (s.ncand > 0) r.last_cls = (int32_t)(staging[t * (int64_t)stage_cap + s.ncand - 1] & 0xffffu) - 1;
-        else if (rel >= 0) r.last_cls = s.first_cls;
+        r.last_cls = prev;
         r.pad = 0;
         return r;
     }
@@ -106,36 +148,24 @@ struct ScanCandidates {
 
 // ---- C ---------------------------------------------------------------------------------------------------------------
 struct ScanFirings {
-    const UrhTileSummary* tiles;
-    const uint32_t* staging;
-    int stage_cap;
-    const int32_t* head_rel;
+    const TileFire* fire;
     const int32_t* prev_cls;
     const int16_t* d_prev0;   // device: class of the candidate preceding the shard (the digitizer's initial state)
     int64_t global_offset;
     int64_t* row_off;
     int64_t* prev_fired;
     __device__ __forceinline__ FireAgg load(int64_t t) const {
-        const UrhTileSummary s = tiles[t];
+        const TileFire f = fire[t];
         int prev = prev_cls[t];
         if (prev == CLS_NONE) prev = *d_prev0;
-        const int64_t base = t * URH_TILE + global_offset;
         FireAgg r;
-        r.fired = 0;
-        r.last_pos = -1;
-        const int32_t rel = head_rel[t];
-        if (rel >= 0) {
-            const int c = s.first_cls;
-            if (c != prev) { r.fired++; r.last_pos = base + rel; }
-            prev = c;
+        r.fired = f.fired;
+        int32_t last = f.last_rel;
+        if (f.first_cls != CLS_NONE && f.first_cls != prev) {
+            r.fired++;
+            if (last < 0) last = f.first_rel;
         }
-        const uint32_t* st = staging + t * (int64_t)stage_cap;
-        for (int j = 0; j < s.ncand; j++) {
-            const uint32_t v = st[j];
-            const int c = (int)(v & 0xffffu) - 1;
-            if (c != prev) { r.fired++; r.last_pos = base + (v >> 16); }
-            prev = c;
-        }
+        r.last_pos = (last >= 0) ? t * URH_TILE + global_offset + last : -1;
         return r;
     }
     __device__ __forceinline__ void post(int64_t t, const FireAgg& excl, const FireAgg&) const {
@@ -144,9 +174,57 @@ struct ScanFirings {
     }
 };
 
+// ---- the walk of stage D: one warp per run of FIN_TILES consecutive tiles ------------------------------------------------------
+// A candidate fires iff its class differs from the one before it.  The lanes take a tile's staged words 32 at a time (one coalesced
+// load from the tile's staging row), the predecessor's class with a shuffle (lane 0: the carried one), the firings with a ballot.
+constexpr int FIN_TILES = 32;   // tiles per warp: lane i loads the per-tile scalars of the warp's i-th tile
+constexpr int FIN_BATCH = 8;    // tiles whose first 32 staged words are loaded before the first of them is walked
+
+struct FinRows {   // stage D's output
+    int64_t* out;
+    int64_t cap_rows;
+    int tol;
+    int is_ask;
+    int64_t sps;
+};
+
+// What a tile's walk carries from one candidate to the next (warp-uniform).
+struct FinWalk {
+    int prev;         // class of the preceding candidate
+    int64_t pp;       // position of the preceding firing (-1: none)
+    int64_t idx;      // row of the next firing
+};
+
+// One firing, written by one lane: (state, length) at row idx (pyx:471-482); rows beyond cap_rows are dropped but counted.
+__device__ __forceinline__ void fin_row(const FinRows& R, int64_t idx, int64_t p, int64_t pp, int prev) {
+    // pulse lengths (pyx:476-482): the first pulse of the capture is counted from its start
+    const int64_t rec = (pp >= 0) ? (p - pp) : (p + 1 - R.tol);
+    int64_t st = prev;
+    if (R.is_ask && st == -1 && rec < R.sps) st = 0;   // ASK: a pause shorter than one symbol is a zero (pyx:471-473)
+    if (idx < R.cap_rows) *((longlong2*)R.out + idx) = make_longlong2(st, rec);   // one 16-byte store per row
+}
+
+// Up to 32 staged candidates of one tile: this lane's word w (lanes >= cnt: none).  Firing lanes write consecutive rows.
+__device__ __forceinline__ void fin_chunk(FinWalk& W, uint32_t w, int cnt, int lane, int64_t base, const FinRows& R) {
+    const int c = (int)(w & 0xffffu) - 1;
+    const int rel = (int)(w >> 16);
+    int pc = __shfl_up_sync(URH_FULL_MASK, c, 1);
+    if (lane == 0) pc = W.prev;
+    const bool fire = lane < cnt && c != pc;
+    const unsigned fm = __ballot_sync(URH_FULL_MASK, fire);
+    // the firing before this lane's: the highest firing lane below it (positions grow with the lane), else the carried one
+    const unsigned lower = fm & ((1u << lane) - 1u);
+    const int before = __shfl_sync(URH_FULL_MASK, rel, lower ? 31 - __clz(lower) : 0);
+    if (fire) fin_row(R, W.idx + __popc(lower), base + rel, lower ? base + before : W.pp, pc);
+    if (fm) W.pp = base + __shfl_sync(URH_FULL_MASK, rel, 31 - __clz(fm));
+    W.idx += __popc(fm);
+    if (cnt > 0) W.prev = __shfl_sync(URH_FULL_MASK, c, cnt - 1);
+}
+
 // ---- D ---------------------------------------------------------------------------------------------------------------
 // out = (state, length) pairs; rows beyond cap_rows are dropped (the caller grows the buffer and repeats).
-// d_out[0] = rows written incl. tail, d_out[1] = firings.
+// d_out[0] = rows written incl. tail, d_out[1] = firings.  The warp's tiles [t0, t0 + FIN_TILES) in order: head candidate, then the
+// staged ones.
 __global__ void __launch_bounds__(256) k_finish_rows(const UrhTileSummary* __restrict__ tiles, const uint32_t* __restrict__ staging,
                                                     int stage_cap, const int32_t* __restrict__ head_rel, const int32_t* __restrict__ prev_cls,
                                                     const int16_t* __restrict__ d_prev0, const int64_t* __restrict__ row_off,
@@ -154,43 +232,71 @@ __global__ void __launch_bounds__(256) k_finish_rows(const UrhTileSummary* __res
                                                     int64_t ntiles, int64_t global_offset, int64_t n_total, int tol, int is_ask, int64_t sps,
                                                     int emit_tail, int64_t row_base, int64_t* __restrict__ out, int64_t cap_rows,
                                                     int64_t* __restrict__ d_out) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ntiles) return;
-    const UrhTileSummary s = tiles[t];
-    int prev = prev_cls[t];
-    if (prev == CLS_NONE) prev = *d_prev0;
-    int64_t pp = prev_fired[t];
-    if (pp < 0) pp = *d_xprev_fired;
-    int64_t idx = row_off[t];
-    const int64_t base = t * URH_TILE + global_offset;
-    auto fire = [&](int64_t p, int c) {
-        if (c != prev) {
-            // pulse lengths (pyx:476-482): the first pulse of the capture is counted from its start
-            const int64_t rec = (pp >= 0) ? (p - pp) : (p + 1 - tol);
-            int64_t st = prev;
-            if (is_ask && st == -1 && rec < sps) st = 0;   // ASK: a pause shorter than one symbol is a zero (pyx:471-473)
-            if (idx < cap_rows) *((longlong2*)out + idx) = make_longlong2(st, rec);   // one 16-byte store per row
-            idx++;
-            pp = p;
-        }
-        prev = c;
-    };
-    const int32_t rel = head_rel[t];
-    if (rel >= 0) fire(base + rel, s.first_cls);
-    const uint32_t* st = staging + t * (int64_t)stage_cap;
-    for (int j = 0; j < s.ncand; j++) {
-        const uint32_t v = st[j];
-        fire(base + (v >> 16), (int)(v & 0xffffu) - 1);
+    const int64_t t0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32 * FIN_TILES;
+    if (t0 >= ntiles) return;
+    const int lane = threadIdx.x & 31;
+    FinRows R;
+    R.out = out; R.cap_rows = cap_rows; R.tol = tol; R.is_ask = is_ask; R.sps = sps;
+    // lane i: the scalars of tile t0 + i
+    const int64_t tl = t0 + lane;
+    int l_first = 0, l_ncand = 0, l_rel = -1, l_prev = 0;
+    int64_t l_idx = 0, l_pp = -1;
+    if (tl < ntiles) {
+        const UrhTileSummary s = tiles[tl];
+        l_first = s.first_cls;
+        l_ncand = s.ncand;
+        l_rel = head_rel[tl];
+        l_prev = prev_cls[tl];
+        if (l_prev == CLS_NONE) l_prev = *d_prev0;
+        l_idx = row_off[tl];
+        l_pp = prev_fired[tl];
+        if (l_pp < 0) l_pp = *d_xprev_fired;
     }
-    if (t == ntiles - 1) {
-        const int64_t fired = idx;
-        // tail row (pyx:485-493): appended only while fewer than n rows exist (row_base: rows of the chunks before this one)
-        if (emit_tail && (is_ask || row_base + fired < n_total)) {
-            if (idx < cap_rows) *((longlong2*)out + idx) = make_longlong2(prev, (pp >= 0) ? (n_total - 1 - pp) : (n_total - tol));
-            idx++;
+    for (int j0 = 0; j0 < FIN_TILES && t0 + j0 < ntiles; j0 += FIN_BATCH) {
+        uint32_t w0[FIN_BATCH];
+#pragma unroll
+        for (int u = 0; u < FIN_BATCH; u++) {
+            const int nc = __shfl_sync(URH_FULL_MASK, l_ncand, j0 + u);
+            w0[u] = (lane < nc) ? __ldg(staging + (t0 + j0 + u) * (int64_t)stage_cap + lane) : 0u;
         }
-        d_out[0] = idx;
-        d_out[1] = fired;
+#pragma unroll
+        for (int u = 0; u < FIN_BATCH; u++) {
+            const int j = j0 + u;
+            const int64_t t = t0 + j;
+            if (t >= ntiles) break;
+            const int64_t base = t * URH_TILE + global_offset;
+            const int ncand = __shfl_sync(URH_FULL_MASK, l_ncand, j);
+            const int rel = __shfl_sync(URH_FULL_MASK, l_rel, j);
+            FinWalk W;
+            W.prev = __shfl_sync(URH_FULL_MASK, l_prev, j);
+            W.pp = __shfl_sync(URH_FULL_MASK, l_pp, j);
+            W.idx = __shfl_sync(URH_FULL_MASK, l_idx, j);
+            if (rel >= 0) {   // the head candidate (a run entering the tile reaches the tolerance inside it)
+                const int c = __shfl_sync(URH_FULL_MASK, l_first, j);
+                if (c != W.prev) {
+                    if (lane == 0) fin_row(R, W.idx, base + rel, W.pp, W.prev);
+                    W.idx++;
+                    W.pp = base + rel;
+                }
+                W.prev = c;
+            }
+            const uint32_t* st = staging + t * (int64_t)stage_cap;
+            for (int k = 0; k < ncand; k += 32) {   // a tile holds up to stage_cap (1026 at tolerance 0) candidates
+                const uint32_t w = (k == 0) ? w0[u] : ((k + lane < ncand) ? __ldg(st + k + lane) : 0u);
+                fin_chunk(W, w, min(32, ncand - k), lane, base, R);
+            }
+            if (t == ntiles - 1 && lane == 0) {
+                int64_t idx = W.idx;
+                const int64_t fired = idx;
+                // tail row (pyx:485-493): appended only while fewer than n rows exist (row_base: rows of the chunks before this one)
+                if (emit_tail && (is_ask || row_base + fired < n_total)) {
+                    if (idx < cap_rows) *((longlong2*)out + idx) = make_longlong2(W.prev, (W.pp >= 0) ? (n_total - 1 - W.pp) : (n_total - tol));
+                    idx++;
+                }
+                d_out[0] = idx;
+                d_out[1] = fired;
+            }
+        }
     }
 }
 
@@ -312,6 +418,8 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     URH_CHECK(urh_arena(ctx, (size_t)ntiles, &prev_cls));
     URH_CHECK(urh_arena(ctx, (size_t)ntiles, &row_off));
     URH_CHECK(urh_arena(ctx, (size_t)ntiles, &prev_fired));
+    TileFire* fire;
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &fire));
     // small block (int64 units): [0..1] stage D's outputs, [2] -1 (no previous firing), [4..5] RunCarry total, [6..7] CandAgg total,
     // [8..9] FireAgg total, [10..11] folded run carry, [12] folded previous class (int16), [13] folded previous firing,
     // [16..19] stage-1 message, [32..) gathered messages: world x 4 (stage 1), world x 2 (stage 2), world x 2 (stage 3)
@@ -344,10 +452,10 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     ScanCandidates fb;
     fb.tiles = tiles; fb.staging = staging; fb.stage_cap = stage_cap; fb.carry = carry;
     fb.xcarry = sharded ? d_xcarry : (chain ? &chain->run : nullptr);
-    fb.tol = tol; fb.head_rel = head_rel; fb.prev_cls = prev_cls;
+    fb.tol = tol; fb.head_rel = head_rel; fb.prev_cls = prev_cls; fb.fire = fire;
     CandAgg ca_ident;
     ca_ident.cnt = 0; ca_ident.last_cls = CLS_NONE; ca_ident.pad = 0;
-    URH_CHECK((urhts::scan<CandAgg, CandOp, ScanCandidates>(ctx, ntiles, ca_ident, CandOp(), fb, d_tot_cand)));
+    URH_CHECK((urhts::scan<CandAgg, CandOp, ScanCandidates, 4>(ctx, ntiles, ca_ident, CandOp(), fb, d_tot_cand)));   // heavy load(): thin blocks
     const int16_t* prev0 = chain ? &chain->prev_cls : d_init;
     if (sharded) {
         URH_TL_MARK(ctx, "x5 candidates: enter");
@@ -357,11 +465,11 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
         prev0 = d_prev0;
     }
     ScanFirings fc;
-    fc.tiles = tiles; fc.staging = staging; fc.stage_cap = stage_cap; fc.head_rel = head_rel; fc.prev_cls = prev_cls; fc.d_prev0 = prev0;
-    fc.global_offset = sh.global_offset; fc.row_off = row_off; fc.prev_fired = prev_fired;
+    fc.fire = fire; fc.prev_cls = prev_cls; fc.d_prev0 = prev0; fc.global_offset = sh.global_offset; fc.row_off = row_off;
+    fc.prev_fired = prev_fired;
     FireAgg fi_ident;
     fi_ident.fired = 0; fi_ident.last_pos = -1;
-    URH_CHECK((urhts::scan<FireAgg, FireOp, ScanFirings, 4>(ctx, ntiles, fi_ident, FireOp(), fc, d_tot_fire)));   // heavy load(): thin blocks
+    URH_CHECK((urhts::scan<FireAgg, FireOp, ScanFirings>(ctx, ntiles, fi_ident, FireOp(), fc, d_tot_fire)));
     const int64_t* xprev = chain ? &chain->prev_fired : d_small + 2;
     if (sharded) {
         URH_TL_MARK(ctx, "x6 firings: enter");
@@ -384,7 +492,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     if (is_ask) URH_CHECK(urh_arena(ctx, (size_t)raw_cap * 2, &raw));
     int64_t got[2] = {0, 0};
     for (int attempt = 0; attempt < 2; attempt++) {
-        URH_LAUNCH(ctx, k_finish_rows, (unsigned)urh_div_up(ntiles, 256), 256, 0, tiles, staging, stage_cap, (const int32_t*)head_rel,
+        URH_LAUNCH(ctx, k_finish_rows, (unsigned)urh_div_up(ntiles, 8 * FIN_TILES), 256, 0, tiles, staging, stage_cap, (const int32_t*)head_rel,
                    (const int32_t*)prev_cls, prev0, (const int64_t*)row_off, (const int64_t*)prev_fired, xprev, ntiles, sh.global_offset,
                    sh.n_total, tol, is_ask ? 1 : 0, (int64_t)sps, sh.emit_tail, row_base, raw, raw_cap, d_small);
         if (sharded && attempt == 0) URH_TL_MARK(ctx, "rows written");
