@@ -108,7 +108,7 @@ int urh_center_histogram(urh_ctx* ctx, const float* d_x, int64_t n, int64_t r0, 
  * of the samples detect_center keeps; *h_kept = their number.  The caller forms the rank window [r0, r1) (5 %..95 %,
  * capped by max_size; a shard subtracts its rank offset), urh_center_window_stats returns h_out5 = {count, min, max, sum,
  * sumsq} inside it (a shard all-reduces these), and urh_center_histogram_tiles is then the only extra pass over qad.
- * halo != 0: the previous shard's last sample is stored right before d_iq (as for urh_shard_dense). */
+ * halo != 0: the previous shard's last sample is stored right before d_iq (as for urh_shard_digitize). */
 int urh_afp_demod_tiles(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float noise_mag, int mod_type, float* d_qad_out,
                         int halo, int64_t* h_kept);
 int urh_center_window_stats(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out5);
@@ -227,23 +227,15 @@ int urh_path_minmax(urh_ctx* ctx, const void* d_src, int dtype, int64_t stride, 
 int urh_qpath_streams(urh_ctx* ctx, const void* d_src, int dtype, int64_t stride, int64_t n, int64_t start, int64_t end, int64_t spp,
                       int64_t x0, const void* d_values, const int64_t* h_bounds, int count, uint8_t* d_out, int64_t* h_offsets);
 
-/* ---- sharded captures: one contiguous sample range per GPU (digitize.cu, nccl.cu; SURVEY 8e) ----------
- * urh_shard_dense      every rank: demodulate + classify its shard (d_iq[-1] = halo sample when has_halo);
- *                      h_summary = {last_cls, last_len, whole, init_cls}
- * urh_shard_candidates every rank, after exchanging the summaries: candidate table with GLOBAL positions
- * urh_pulses_from_table the gathering rank: concatenated tables -> (state, length) rows of the whole capture */
-int urh_shard_dense(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag, int mod_type,
-                    float center, uint16_t tolerance, uint8_t bits_per_symbol, float center_spacing, float* d_qad_out,
-                    int64_t* h_summary);
-/* the same step for a shard that is already demodulated (digitizing once a capture-wide center is known) */
-int urh_shard_dense_qad(urh_ctx* ctx, const float* d_qad, int64_t n, int mod_type, float center, uint16_t tolerance,
-                        uint8_t bits_per_symbol, float center_spacing, int64_t* h_summary);
+/* ---- sharded captures: one contiguous sample range per GPU (digitize.cu, finish.cu, nccl.cu; SURVEY 8e) ----------
+ * The digitizer: urh_shard_digitize (known center) and urh_shard_demod_center_digitize(_host) (below) run on every rank
+ *   (d_iq[-1] = halo sample when has_halo); each finishes its own shard's rows, exchanging three small NCCL all-gathers on the
+ *   stream.
+ * The message segmenter: urh_segment_shard_pass (above) on every rank; after the ranks have exchanged its summaries,
+ *   urh_shard_candidates gives the shard's candidate table with GLOBAL positions (carry_*: the run that ends right before the
+ *   shard) and urh_fetch_candidates copies it to the host. */
 int urh_shard_candidates(urh_ctx* ctx, int carry_valid, int carry_cls, int64_t carry_len, int64_t global_offset,
                          int64_t* count, const int64_t** d_pos, const int16_t** d_cls, int* last_cand_cls);
-/* distributed finish (no gather): every rank keeps its own rows; see urh_b200/dist.py for the two scalars exchanged */
-int urh_shard_fire(urh_ctx* ctx, int prev_cls, int64_t* fired, int64_t* last_fired_pos);
-int urh_shard_rows(urh_ctx* ctx, int64_t n_total, uint16_t tolerance, int mod_type, uint32_t samples_per_symbol,
-                   int64_t prev_fired_pos, int emit_tail, int64_t* k);
 /* One-call variants: every stage is enqueued on the context stream, the host synchronises once at the end.
  * urh_demod_center_digitize: afp_demod (ASK/FSK) + AutoInterpretation.detect_center (AutoInterpretation.py:226-277, capture-wide)
  *   + grab_pulse_lens (signal_functions.pyx:392-495, binary symbols) = BASELINE configs[1].  *center_state: 0 no center (None),
@@ -386,8 +378,6 @@ int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, const float* d
                        float noise_mag, int mod_type, float center, uint16_t tolerance, uint32_t samples_per_symbol,
                        uint8_t bits_per_symbol, float center_spacing, float* d_qad_out, int64_t global_offset,
                        int64_t n_total, int64_t* k);
-int urh_pulses_from_table(urh_ctx* ctx, const int64_t* d_pos, const int16_t* d_cls, int64_t count, int64_t n_total,
-                          uint16_t tolerance, int mod_type, uint32_t samples_per_symbol, int init_cls, int64_t* k);
 /* PSK (Costas loop) over shards: speculate concurrently on every rank, then hand the loop state from rank to rank */
 int urh_costas_halo_samples(void);
 int urh_costas_shard_speculate(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int first_shard, float noise_mag,

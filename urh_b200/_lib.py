@@ -110,11 +110,7 @@ SIGNATURES = {
     "urh_dc_int_subtract": (i32, [vp, vp, i32, i64, C.c_double, C.c_double, vp]),
     "urh_stft": (i32, [vp, vp, i64, i32, i32, vp, i64, vp]),
     "urh_spectrogram_db": (i32, [vp, vp, i64, i32, i32, vp, i64, vp]),
-    "urh_shard_dense": (i32, [vp, vp, i32, i64, i32, f32, i32, f32, u16, u8, f32, vp, vp]),
-    "urh_shard_dense_qad": (i32, [vp, vp, i64, i32, f32, u16, u8, f32, vp]),
     "urh_shard_candidates": (i32, [vp, i32, i32, i64, i64, C.POINTER(i64), C.POINTER(vp), C.POINTER(vp), C.POINTER(i32)]),
-    "urh_shard_fire": (i32, [vp, i32, C.POINTER(i64), C.POINTER(i64)]),
-    "urh_shard_rows": (i32, [vp, i64, u16, i32, u32, i64, i32, C.POINTER(i64)]),
     "urh_nccl_allgather_host": (i32, [vp, vp, vp, szt]),
     "urh_nccl_allreduce_host_i64": (i32, [vp, vp, i64, i32]),
     "urh_p2p_create": (i32, [vp, vp]),
@@ -135,7 +131,6 @@ SIGNATURES = {
     "urh_segment_shard_pass": (i32, [vp, vp, i32, i64, f32, vp]),
     "urh_segments_from_runs": (i32, [vp, vp, i64, i32, i32, i64, i64, vp, i64, C.POINTER(i64)]),
     "urh_fetch_candidates": (i32, [vp, vp, vp, i64]),
-    "urh_pulses_from_table": (i32, [vp, vp, vp, i64, i64, u16, i32, u32, i32, C.POINTER(i64)]),
     "urh_costas_halo_samples": (i32, []),
     "urh_costas_shard_speculate": (i32, [vp, vp, i32, i64, i32, f32, i32, f32, vp]),
     "urh_costas_shard_resolve": (i32, [vp, vp, vp]),

@@ -54,7 +54,7 @@ struct urh_ctx {
     // twiddles of the last window size urh_spectrogram_bgra ran with (spectrogram.cu; 4096 entries allocated)
     void* img_tw;
     int img_tw_n;
-    // sharded digitizer state between urh_shard_dense and urh_shard_candidates (arena memory)
+    // sharded segmenter state between urh_segment_shard_pass and urh_shard_candidates / urh_fetch_candidates (arena memory)
     void* shard_tiles;
     void* shard_staging;
     int shard_cap, shard_tol;

@@ -454,17 +454,31 @@ int urh_finish_local(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps
 int urh_finish_shard(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
                      int stage_cap, const int16_t* d_init, int64_t global_offset, int64_t n_total, int64_t* k);   // finish.cu
 
-static int digitize_finish(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, UrhTileSummary* tiles,
-                           uint32_t* staging, int stage_cap, int16_t* d_init, int64_t* k) {
-    if (getenv("URH_B200_OLD_FINISH")) {   // the candidate-table formulation (kept for the segmenter; A/B switch for measurements)
-        UrhCandidates cand;
-        URH_CHECK(urh_collect_candidates(ctx, n, tol, tiles, staging, stage_cap, &cand));
-        return urh_pulses_from_candidates(ctx, n, tol, is_ask, sps, cand, d_init, k);
-    }
-    return urh_finish_local(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, k);
+static int stage_cap_for(int tol) { return URH_TILE / (tol + 1) + 2; }
+
+// The digitizer's tables for ntiles tiles in the arena: tile summaries, cap staged candidates per tile, the initial state.
+static int digitizer_tables(urh_ctx* ctx, int64_t ntiles, int cap, UrhTileSummary** tiles, uint32_t** staging, int16_t** d_init) {
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles, tiles));
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, staging));
+    return urh_arena(ctx, 8, d_init);
 }
 
-static int stage_cap_for(int tol) { return URH_TILE / (tol + 1) + 2; }
+// The digitizer's dense pass over qad x[0, n), one warp per tile; binary symbols take the paired loads.  init: where the first tile
+// stores the digitizer's initial state (NULL: nowhere).  d_thr0: the threshold in device memory (then c0 is derived on the device);
+// ts: the demodulator's tile statistics, whose all-NOISE tiles are not read.
+static int launch_dense_qad(urh_ctx* ctx, const float* x, int64_t n, const UrhClassify& cls, int tol, UrhTileSummary* tiles,
+                            uint32_t* staging, int cap, int16_t* init, int c0, const float* d_thr0 = nullptr,
+                            const UrhTileStats* ts = nullptr) {
+    const unsigned grid = (unsigned)urh_div_up(urh_div_up(n, URH_TILE), URH_WARPS_PER_BLOCK);
+    const int vec_in = (((uintptr_t)x % 8) == 0) ? 1 : 0;
+    if (cls.order == 2)
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, tol, tiles, staging, cap, init,
+                   c0, d_thr0, ts);
+    else
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, tol, tiles, staging, cap, init,
+                   c0, d_thr0, ts);
+    return URH_OK;
+}
 
 extern "C" int urh_grab_pulse_lens(urh_ctx* ctx, const float* d_qad, int64_t n, float center, uint16_t tolerance,
                                    int mod_type, uint32_t samples_per_symbol, uint8_t bits_per_symbol,
@@ -483,20 +497,11 @@ extern "C" int urh_grab_pulse_lens(urh_ctx* ctx, const float* d_qad, int64_t n, 
     UrhTileSummary* tiles;
     uint32_t* staging;
     int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
-    const unsigned grid = (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
-    const int vec_in = (((uintptr_t)d_qad % 8) == 0) ? 1 : 0;
+    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
     URH_PROF_BEGIN(ctx);
-    if (cls.order == 2)
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad, n, vec_in, cls, tol, tiles,
-                   staging, cap, d_init, host_classify(0.0f, cls));
-    else
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad, n, vec_in, cls, tol, tiles,
-                   staging, cap, d_init, host_classify(0.0f, cls));
+    URH_CHECK(launch_dense_qad(ctx, d_qad, n, cls, tol, tiles, staging, cap, d_init, host_classify(0.0f, cls)));
     URH_PROF_END(ctx);
-    return digitize_finish(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
+    return urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
 }
 
 extern "C" int urh_demod_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float noise_mag,
@@ -532,101 +537,13 @@ extern "C" int urh_demod_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int
     UrhTileSummary* tiles;
     uint32_t* staging;
     int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
+    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
     const int c0 = host_classify(0.0f, cls);
     if (mod_type == URH_MOD_ASK)
         URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0)));
     else
         URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0)));
-    return digitize_finish(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
-}
-
-// =====================================================================================================
-// Sharded captures (SURVEY §8e): one contiguous sample range per GPU, 1-sample halo for the FSK conjugate
-// product, run-carry descriptors exchanged between ranks, candidate tables gathered to one rank.
-// =====================================================================================================
-// Step 1 on every rank.  d_iq points at the shard's first own sample; when has_halo != 0 the sample that precedes
-// the shard in the capture is stored immediately before it (d_iq[-1]).  Keeps the tile table in the arena for step 2.
-// h_summary = {last_cls, last_len, whole, init_cls}: the shard's closing run and (rank 0) the digitizer's initial state.
-extern "C" int urh_shard_dense(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag, int mod_type,
-                               float center, uint16_t tolerance, uint8_t bits_per_symbol, float center_spacing,
-                               float* d_qad_out, int64_t* h_summary) {
-    if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "empty shard");
-    if (mod_type != URH_MOD_ASK && mod_type != URH_MOD_FSK) URH_FAIL(ctx, URH_ERR_INVALID, "sharded path: ASK / FSK only (PSK is a serial recurrence)");
-    if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
-    urh_arena_reset(ctx);
-    UrhClassify cls;
-    URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
-    const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
-    const int tol = tolerance;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
-    URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
-    const int c0 = host_classify(0.0f, cls);
-    if (mod_type == URH_MOD_ASK)
-        URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0, has_halo)));
-    else
-        URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0, has_halo)));
-    ctx->shard_tiles = tiles;
-    ctx->shard_staging = staging;
-    ctx->shard_cap = cap;
-    ctx->shard_n = n;
-    ctx->shard_tol = tol;
-    URH_CHECK(urh_shard_run_total(ctx, n, tiles, h_summary));
-    int16_t init16 = 0;
-    URH_CUDA(ctx, cudaMemcpyAsync(&init16, d_init, sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    h_summary[3] = init16;
-    return URH_OK;
-}
-
-// Step 1 for a shard that is already demodulated (the center became known only after the demodulation pass): the
-// digitizer's dense pass over qad.  Classification is per sample, so no halo is involved; same h_summary as urh_shard_dense.
-extern "C" int urh_shard_dense_qad(urh_ctx* ctx, const float* d_qad, int64_t n, int mod_type, float center, uint16_t tolerance,
-                                   uint8_t bits_per_symbol, float center_spacing, int64_t* h_summary) {
-    if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "empty shard");
-    urh_arena_reset(ctx);
-    UrhClassify cls;
-    URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
-    const int tol = tolerance;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
-    URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
-    const int vec_in = (((uintptr_t)d_qad % 8) == 0) ? 1 : 0;
-    URH_PROF_BEGIN(ctx);
-    const unsigned grid = (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
-    if (cls.order == 2)
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad, n, vec_in, cls, tol, tiles, staging, cap,
-                   d_init, host_classify(0.0f, cls));
-    else
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad, n, vec_in, cls, tol, tiles, staging, cap,
-                   d_init, host_classify(0.0f, cls));
-    URH_PROF_END(ctx);
-    ctx->shard_tiles = tiles;
-    ctx->shard_staging = staging;
-    ctx->shard_cap = cap;
-    ctx->shard_n = n;
-    ctx->shard_tol = tol;
-    URH_CHECK(urh_shard_run_total(ctx, n, tiles, h_summary));
-    int16_t init16 = 0;
-    URH_CUDA(ctx, cudaMemcpyAsync(&init16, d_init, sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    h_summary[3] = init16;
-    return URH_OK;
+    return urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
 }
 
 // ---- streaming through a ring of device slots (DESIGN.md §4.11) -----------------------------------------------------------------
@@ -796,10 +713,7 @@ struct StreamDigitizer {
         n = n_total; tol = tolerance; is_ask = ask; sps = samples_per_symbol; rows = 0;
         cap = stage_cap_for(tol);
         rows_all = rows_bound(n, tol);
-        const int64_t ct = cs / URH_TILE;
-        URH_CHECK(urh_arena(ctx, (size_t)ct, &tiles));
-        URH_CHECK(urh_arena(ctx, (size_t)ct * cap, &staging));
-        URH_CHECK(urh_arena(ctx, 8, &d_init));
+        URH_CHECK(digitizer_tables(ctx, cs / URH_TILE, cap, &tiles, &staging, &d_init));
         URH_CHECK(urh_arena(ctx, 1, &chain));
         URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
         mark = urh_arena_mark(ctx);
@@ -862,19 +776,8 @@ static int stream_dense_iq(urh_ctx* ctx, int dtype, int mod_type, const char* d_
 // Digitizer dense pass over qad [s0, s1) at x (local view: chunk-relative tiles; only chunk 0 sets the initial state).
 static int stream_dense_qad(urh_ctx* ctx, const float* x, int64_t s0, int64_t s1, const UrhClassify& cls, StreamDigitizer& dz,
                             const float* d_thr0 = nullptr, const UrhTileStats* ts = nullptr) {
-    const int64_t nc = s1 - s0;
-    const unsigned grid = (unsigned)urh_div_up(urh_div_up(nc, URH_TILE), URH_WARPS_PER_BLOCK);
-    const int vec_in = (((uintptr_t)x % 8) == 0) ? 1 : 0;
-    int16_t* init = s0 == 0 ? dz.d_init : nullptr;
-    const int c0 = d_thr0 ? 0 : host_classify(0.0f, cls);
-    const UrhTileStats* tsc = ts ? ts + s0 / URH_TILE : nullptr;
-    if (cls.order == 2)
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, nc, vec_in, cls, dz.tol, dz.tiles, dz.staging,
-                   dz.cap, init, c0, d_thr0, tsc);
-    else
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, nc, vec_in, cls, dz.tol, dz.tiles, dz.staging,
-                   dz.cap, init, c0, d_thr0, tsc);
-    return URH_OK;
+    return launch_dense_qad(ctx, x, s1 - s0, cls, dz.tol, dz.tiles, dz.staging, dz.cap, s0 == 0 ? dz.d_init : nullptr,
+                            d_thr0 ? 0 : host_classify(0.0f, cls), d_thr0, ts ? ts + s0 / URH_TILE : nullptr);
 }
 
 // ---- one-call paths: every stage enqueued on the context stream, ONE synchronisation at the end -----------------------------
@@ -885,8 +788,9 @@ int urh_center_plan_result(urh_ctx* ctx, const CenterPlan* plan, const float** d
 int urh_center_plan_certify_stats(urh_ctx* ctx, const CenterPlan* plan, int64_t* h_dst3);
 
 // Sharded demod + digitize for a KNOWN center (SURVEY 8e): dense pass over this rank's shard, then the tile-level finish with
-// its three 16-byte exchanges on the stream (finish.cu).  d_qad_in != NULL: the shard is already demodulated, digitize from it.
-// Every rank ends with the rows of its own shard (urh_fetch_pulses).
+// its three 16-byte exchanges on the stream (finish.cu).  d_iq points at the shard's first own sample; when has_halo != 0 the sample
+// that precedes the shard in the capture is stored right before it (d_iq[-1]).  d_qad_in != NULL: the shard is already demodulated,
+// digitize from it.  Every rank ends with the rows of its own shard (urh_fetch_pulses).
 extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, const float* d_qad_in, int64_t n, int has_halo,
                                   float noise_mag, int mod_type, float center, uint16_t tolerance, uint32_t samples_per_symbol,
                                   uint8_t bits_per_symbol, float center_spacing, float* d_qad_out, int64_t global_offset,
@@ -907,21 +811,12 @@ extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, con
     UrhTileSummary* tiles;
     uint32_t* staging;
     int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
+    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
     URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
     const int c0 = host_classify(0.0f, cls);
     if (d_qad_in) {
-        const int vec_in = (((uintptr_t)d_qad_in % 8) == 0) ? 1 : 0;
-        const unsigned grid = (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
         URH_PROF_BEGIN(ctx);
-        if (cls.order == 2)
-            URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad_in, n, vec_in, cls, tol, tiles, staging, cap,
-                       d_init, c0, (const float*)nullptr);
-        else
-            URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_qad_in, n, vec_in, cls, tol, tiles, staging, cap,
-                       d_init, c0, (const float*)nullptr);
+        URH_CHECK(launch_dense_qad(ctx, d_qad_in, n, cls, tol, tiles, staging, cap, d_init, c0));
         URH_PROF_END(ctx);
     } else {
         const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
@@ -934,7 +829,7 @@ extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, con
 }
 
 // demod (ASK / FSK) + capture-wide detect_center + digitize (binary symbols) in one call (BASELINE configs[1]).
-// sharded != 0: this rank's shard of a capture spread over the context's NCCL communicator (has_halo as urh_shard_dense).
+// sharded != 0: this rank's shard of a capture spread over the context's NCCL communicator (has_halo as urh_shard_digitize).
 // *center_state: 0 = detect_center finds no center (None; *k = 0), 1 = *center is valid, 2 = the device could not decide
 // (a tie between histogram peaks whose order numpy's argsort defines, or more than 6000 bins): d_qad_out is valid, the
 // caller finishes through the stepwise entry points (urh_center_window_stats / urh_center_histogram_tiles / urh_grab_pulse_lens).
@@ -1007,11 +902,7 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
     UrhTileSummary* tiles = nullptr;
     uint32_t* staging = nullptr;
     int16_t* d_init = nullptr;
-    if (!sc) {
-        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-        URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-        URH_CHECK(urh_arena(ctx, 8, &d_init));
-    }
+    if (!sc) URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
     // speculative digitizing (UrhSpec, DESIGN.md §4.4.1): the pass digitizes its fast tiles at a guessed threshold, the qad digitizer
     // re-reads only the tiles whose margin does not prove the classes at the detected center.  The resident single-GPU float32 FSK
     // step only; $URH_B200_NO_SPECULATE=1 turns it off, $URH_B200_SPECULATE_GUESS=<float> replaces the guess (read per call).
@@ -1315,22 +1206,24 @@ extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int
     return urh_costas_stream_end(ctx, &cs);
 }
 
+// ---- sharded message segmentation (SURVEY 8e) -----------------------------------------------------------------------------------
+// urh_segment_shard_pass (stats.cu) leaves its shard's tile table in the context; once the ranks have exchanged their closing runs,
+// urh_shard_candidates turns it into the shard's candidate table with global positions and urh_fetch_candidates copies that to the
+// host.
 struct UrhShardState {
     UrhCandidates cand;
-    UrhFireState fs;
-    int16_t* d_prev;
 };
 static UrhShardState* shard_state(urh_ctx* ctx) {
     if (!ctx->shard_state) ctx->shard_state = calloc(1, sizeof(UrhShardState));
     return (UrhShardState*)ctx->shard_state;
 }
 
-// Step 2 on every rank, after the summaries were exchanged: carry_* describe the run that ends right before this
-// shard (fold of the preceding shards' summaries; carry_valid = 0 on the first shard).  Positions are global.
+// After the summaries were exchanged: carry_* describe the run that ends right before this shard (fold of the preceding shards'
+// summaries; carry_valid = 0 on the first shard).  Positions are global.
 // *last_cand_cls = class of the shard's last candidate (meaningful when *count > 0).
 extern "C" int urh_shard_candidates(urh_ctx* ctx, int carry_valid, int carry_cls, int64_t carry_len, int64_t global_offset,
                                     int64_t* count, const int64_t** d_pos, const int16_t** d_cls, int* last_cand_cls) {
-    if (!ctx->shard_tiles) URH_FAIL(ctx, URH_ERR_INVALID, "urh_shard_dense must precede urh_shard_candidates");
+    if (!ctx->shard_tiles) URH_FAIL(ctx, URH_ERR_INVALID, "urh_segment_shard_pass must precede urh_shard_candidates");
     UrhShardCarry in;
     in.valid = carry_valid; in.cls = carry_cls; in.len = carry_len;
     UrhShardState* S = shard_state(ctx);
@@ -1361,45 +1254,6 @@ extern "C" int urh_fetch_candidates(urh_ctx* ctx, int64_t* h_pos, int16_t* h_cls
     URH_CUDA(ctx, cudaMemcpyAsync(h_cls, S->cand.cls, (size_t)count * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
     URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return URH_OK;
-}
-
-// Step 3 (distributed finish): prev_cls = class of the last candidate of the preceding shards (the digitizer's
-// initial state on the first shard).  Returns the number of firings and the position of the last one (-1: none).
-extern "C" int urh_shard_fire(urh_ctx* ctx, int prev_cls, int64_t* fired, int64_t* last_fired_pos) {
-    UrhShardState* S = shard_state(ctx);
-    URH_CHECK(urh_arena(ctx, 8, &S->d_prev));
-    const int16_t v = (int16_t)prev_cls;
-    URH_CUDA(ctx, cudaMemcpyAsync(S->d_prev, &v, sizeof(v), cudaMemcpyHostToDevice, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    URH_CHECK(urh_fire_stage(ctx, S->cand, S->d_prev, &S->fs, last_fired_pos));
-    *fired = S->fs.F;
-    return URH_OK;
-}
-
-// Step 4: this shard's rows (merged locally; equal states across a shard edge are merged by the consumer).
-// prev_fired_pos = position of the last firing in the preceding shards (-1: none); emit_tail on the last shard only.
-extern "C" int urh_shard_rows(urh_ctx* ctx, int64_t n_total, uint16_t tolerance, int mod_type, uint32_t samples_per_symbol,
-                              int64_t prev_fired_pos, int emit_tail, int64_t* k) {
-    UrhShardState* S = shard_state(ctx);
-    return urh_rows_stage(ctx, S->fs, n_total, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol, prev_fired_pos, emit_tail != 0, k);
-}
-
-// Step 3 on the gathering rank: the concatenated candidate tables of all shards -> pulse table of the whole capture.
-extern "C" int urh_pulses_from_table(urh_ctx* ctx, const int64_t* d_pos, const int16_t* d_cls, int64_t count, int64_t n_total,
-                                     uint16_t tolerance, int mod_type, uint32_t samples_per_symbol, int init_cls, int64_t* k) {
-    urh_arena_reset(ctx);
-    int16_t* d_init;
-    URH_CHECK(urh_arena(ctx, 8, &d_init));
-    const int16_t v = (int16_t)init_cls;
-    URH_CUDA(ctx, cudaMemcpyAsync(d_init, &v, sizeof(v), cudaMemcpyHostToDevice, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    UrhCandidates cand;
-    cand.count = count;
-    cand.pos = (int64_t*)d_pos;
-    cand.cls = (int16_t*)d_cls;
-    cand.last_cls = 0;
-    cand.last_len = 0;
-    return urh_pulses_from_candidates(ctx, n_total, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol, cand, d_init, k);
 }
 
 extern "C" int urh_fetch_pulses(urh_ctx* ctx, int64_t* h_rows, int64_t k) {

@@ -1,6 +1,6 @@
 // NCCL plumbing for captures sharded across the GPUs of one box (SURVEY §8e).
-// The exchanges on this path are tiny (chunk statistics, run-carry descriptors, histograms) plus one gather of the
-// sparse candidate tables; NVLink bandwidth is irrelevant, latency is what counts.  libnccl is dlopen()ed so that
+// The exchanges on this path are tiny (chunk statistics, run-carry descriptors, histograms); NVLink bandwidth is
+// irrelevant, latency is what counts.  libnccl is dlopen()ed so that
 // liburh_b200.so has no link-time dependency on it (single-GPU users never load it) and cannot clash with another
 // NCCL copy in the process.
 #include "common.cuh"

@@ -1,4 +1,5 @@
-// Sparse stages of the digitizer (see sparse.cuh, DESIGN.md §digitizer).
+// Run stitching and candidate collection over a tile table: the segmenter's and the plateau RLE's candidate tables and a shard's
+// closing run (see sparse.cuh, DESIGN.md §4.2).
 #include "sparse.cuh"
 #include "scan.cuh"
 
@@ -136,134 +137,4 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
     const unsigned gg = (unsigned)urh_div_up(ntiles * 32, 256);
     URH_LAUNCH(ctx, k_gather, gg, 256, 0, tiles, staging, stage_cap, head_rel, total, ntiles, global_offset, out->pos, out->cls);
     return URH_OK;
-}
-
-// ---- grab_pulse_lens on the candidate table ---------------------------------------------------------
-__global__ void k_fire_flags(const int16_t* __restrict__ cls, const int16_t* __restrict__ init, int64_t C,
-                             int64_t* __restrict__ fire) {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= C) return;
-    const int prev = j ? cls[j - 1] : *init;
-    fire[j] = (cls[j] != prev) ? 1 : 0;
-}
-
-__global__ void k_fired_rows(const int64_t* __restrict__ pos, const int16_t* __restrict__ cls,
-                             const int16_t* __restrict__ init, const int64_t* __restrict__ fidx, int64_t C,
-                             int64_t* __restrict__ fpos, int64_t* __restrict__ st) {
-    const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= C) return;
-    const int prev = j ? cls[j - 1] : *init;
-    if (cls[j] != prev) {
-        const int64_t f = fidx[j];
-        fpos[f] = pos[j];
-        st[f] = prev;  // the state that ends here (cur_state at pyx:475-479)
-    }
-}
-
-// pulse lengths (pyx:476-482), ASK short-pause relabel (pyx:471-473), tail row (pyx:485-493).
-// Sharded captures: prev_fired (position of the last firing in the preceding shards, -1 if none) replaces the
-// "first pulse" rule, and only the last shard emits the tail row.
-__global__ void k_row_lengths(const int64_t* __restrict__ fpos, int64_t* __restrict__ st, int64_t* __restrict__ ln,
-                              int64_t F, int64_t n, int tol, int is_ask, int64_t sps, const int16_t* __restrict__ cls,
-                              int64_t C, const int16_t* __restrict__ init, int64_t prev_fired, int emit_tail) {
-    const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (f > F) return;
-    if (f == F) {
-        if (!emit_tail) return;
-        st[f] = C ? cls[C - 1] : *init;
-        ln[f] = F ? (n - 1 - fpos[F - 1]) : (prev_fired >= 0 ? (n - 1 - prev_fired) : (n - tol));
-        return;
-    }
-    const int64_t rec = f ? (fpos[f] - fpos[f - 1]) : (prev_fired >= 0 ? (fpos[0] - prev_fired) : (fpos[0] + 1 - tol));
-    if (is_ask && st[f] == -1 && rec < sps) st[f] = 0;
-    ln[f] = rec;
-}
-
-__global__ void k_row_heads(const int64_t* __restrict__ st, int64_t rows, int64_t* __restrict__ head) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= rows) return;
-    head[r] = (r == 0 || st[r] != st[r - 1]) ? 1 : 0;
-}
-
-__global__ void k_row_merge(const int64_t* __restrict__ st, const int64_t* __restrict__ ln,
-                            const int64_t* __restrict__ seg_incl, int64_t rows, int64_t* __restrict__ out) {
-    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= rows) return;
-    const int64_t o = seg_incl[r] - 1;
-    if (r == 0 || st[r] != st[r - 1]) out[2 * o] = st[r];
-    atomicAdd((unsigned long long*)&out[2 * o + 1], (unsigned long long)ln[r]);
-}
-
-int urh_fire_stage(urh_ctx* ctx, const UrhCandidates& cand, const int16_t* d_prev_cls, UrhFireState* fs, int64_t* last_fired_pos) {
-    const int64_t C = cand.count;
-    fs->C = C;
-    fs->F = 0;
-    fs->pos = cand.pos;
-    fs->cls = cand.cls;
-    fs->d_prev_cls = d_prev_cls;
-    fs->fire = nullptr;
-    int64_t* d_tot = nullptr;
-    URH_CHECK(urh_arena(ctx, 4, &d_tot));
-    if (C > 0) {
-        URH_CHECK(urh_arena(ctx, (size_t)C, &fs->fire));
-        URH_LAUNCH(ctx, k_fire_flags, (unsigned)urh_div_up(C, 256), 256, 0, cand.cls, d_prev_cls, C, fs->fire);
-        URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, fs->fire, C, urhscan::AddI64(), (int64_t)0, true, d_tot)));
-        URH_CHECK(urh_read_i64(ctx, d_tot, 1, &fs->F));
-    }
-    const int64_t F = fs->F;
-    URH_CHECK(urh_arena(ctx, (size_t)F + 1, &fs->fpos));
-    URH_CHECK(urh_arena(ctx, (size_t)F + 1, &fs->st));
-    URH_CHECK(urh_arena(ctx, (size_t)F + 1, &fs->ln));
-    URH_CHECK(urh_arena(ctx, (size_t)F + 1, &fs->head));
-    if (F > 0) URH_LAUNCH(ctx, k_fired_rows, (unsigned)urh_div_up(C, 256), 256, 0, cand.pos, cand.cls, d_prev_cls, fs->fire, C, fs->fpos, fs->st);
-    if (last_fired_pos) {
-        *last_fired_pos = -1;
-        if (F > 0) URH_CHECK(urh_read_i64(ctx, fs->fpos + F - 1, 1, last_fired_pos));
-    }
-    return URH_OK;
-}
-
-int urh_rows_stage(urh_ctx* ctx, const UrhFireState& fs, int64_t n, int tol, bool is_ask, uint32_t sps, int64_t prev_fired,
-                   bool emit_tail, int64_t* k) {
-    const int64_t F = fs.F, C = fs.C;
-    int64_t *fpos = fs.fpos, *st = fs.st, *ln = fs.ln, *head = fs.head;
-    const int64_t cand_rows = emit_tail ? F + 1 : F;
-    if (cand_rows == 0) {
-        ctx->pulses_k = 0;
-        *k = 0;
-        return URH_OK;
-    }
-    URH_LAUNCH(ctx, k_row_lengths, (unsigned)urh_div_up(F + 1, 256), 256, 0, fpos, st, ln, F, n, tol, is_ask ? 1 : 0,
-               (int64_t)sps, fs.cls, C, fs.d_prev_cls, prev_fired, emit_tail ? 1 : 0);
-    URH_LAUNCH(ctx, k_row_heads, (unsigned)urh_div_up(cand_rows, 256), 256, 0, st, cand_rows, head);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, head, cand_rows, urhscan::AddI64(), (int64_t)0, false, nullptr)));
-    // merged row count before/with the tail row
-    int64_t hv[2] = {0, 0};
-    if (emit_tail) {
-        if (F > 0) {
-            URH_CHECK(urh_read_i64(ctx, head + F - 1, 2, hv));
-        } else {
-            URH_CHECK(urh_read_i64(ctx, head, 1, &hv[1]));
-        }
-    } else {
-        URH_CHECK(urh_read_i64(ctx, head + F - 1, 1, &hv[0]));
-    }
-    const int64_t merged_before_tail = F > 0 ? hv[0] : 0;
-    // pyx:487: the tail row is only appended while cur_index < len(result) == n
-    const bool keep_tail = emit_tail && merged_before_tail < n;
-    const int64_t rows = keep_tail ? F + 1 : F;
-    const int64_t K = keep_tail ? hv[1] : merged_before_tail;
-    URH_CHECK(urh_ensure_pulses(ctx, (size_t)K));
-    URH_CUDA(ctx, cudaMemsetAsync(ctx->pulses, 0, (size_t)K * 2 * sizeof(int64_t), ctx->stream));
-    if (rows > 0) URH_LAUNCH(ctx, k_row_merge, (unsigned)urh_div_up(rows, 256), 256, 0, st, ln, head, rows, ctx->pulses);
-    ctx->pulses_k = K;
-    *k = K;
-    return URH_OK;
-}
-
-int urh_pulses_from_candidates(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhCandidates& cand,
-                               const int16_t* d_init_cls, int64_t* k) {
-    UrhFireState fs;
-    URH_CHECK(urh_fire_stage(ctx, cand, d_init_cls, &fs, nullptr));
-    return urh_rows_stage(ctx, fs, n, tol, is_ask, sps, -1, true, k);
 }

@@ -1,5 +1,6 @@
-// Sparse stages shared by the digitizer, the message segmenter and the plateau RLE:
-// tile summaries + per-tile staged candidates  ->  one ordered, compact candidate table.
+// Run stitching across tiles (RunCarry), used by the digitizer's tile-level finish (finish.cu), and the gathered candidate table of
+// the message segmenter and the plateau RLE (stats.cu): tile summaries + per-tile staged candidates  ->  one ordered, compact table.
+// UrhChain: what a chunk's finish receives from the chunks before it (finish.cu).
 #pragma once
 #include "dense.cuh"
 
@@ -65,22 +66,3 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
 // The shard's own run summary for the exchange: h_out = {last_cls, last_len, whole (1 if the shard is one run)}.
 int urh_shard_run_total(urh_ctx* ctx, int64_t n, const UrhTileSummary* tiles, int64_t* h_out);
 
-// grab_pulse_lens tail (signal_functions.pyx:455-495) on the candidate table: fire filter, pulse lengths,
-// ASK short-pause relabel, merge of equal neighbours, tail row.  Result -> ctx->pulses / ctx->pulses_k.
-int urh_pulses_from_candidates(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhCandidates& cand,
-                               const int16_t* d_init_cls, int64_t* k);
-
-// The two halves of urh_pulses_from_candidates, separable so that shards can exchange the two scalars each half
-// needs from its predecessors: the class of the last candidate before the shard (fire decision of its first
-// candidate) and the position of the last firing before the shard (length of its first pulse).
-struct UrhFireState {
-    int64_t C, F;
-    int64_t* fire;
-    const int64_t* pos;
-    const int16_t* cls;
-    const int16_t* d_prev_cls;
-    int64_t *fpos, *st, *ln, *head;
-};
-int urh_fire_stage(urh_ctx* ctx, const UrhCandidates& cand, const int16_t* d_prev_cls, UrhFireState* fs, int64_t* last_fired_pos);
-int urh_rows_stage(urh_ctx* ctx, const UrhFireState& fs, int64_t n, int tol, bool is_ask, uint32_t sps, int64_t prev_fired,
-                   bool emit_tail, int64_t* k);

@@ -2,16 +2,16 @@
 
 One process per GPU (launched by torchrun).  ``torch.distributed`` (gloo) is the launcher plumbing: rendezvous and
 the exchange of tiny host-side descriptors; the data path between GPUs is NCCL over NVLink, driven from
-liburh_b200 (nccl.cu): the 1-sample halo, the all-reduce of the global noise statistics and the gather of the
-sparse candidate tables.  Per rank the sample-rate work is exactly the single-GPU dense pass.
+liburh_b200 (nccl.cu): the 1-sample halo, the all-reduce of the global noise statistics and the digitizer's three
+small all-gathers.  Per rank the sample-rate work is exactly the single-GPU dense pass.
 
-Protocol of the sharded digitizer (exactness argument in DESIGN.md §6):
-  1. every rank: dense pass over its shard (+1 halo sample for the FSK conjugate product) -> tile table and the
-     summary (class, length, whole?) of the run that closes the shard;
-  2. all-gather the summaries; rank r folds those of ranks < r with the run-carry operator -> the run that ends
-     right before its shard;
-  3. every rank: candidate table with global positions (the carry only affects the first run of the shard);
-  4. gather the candidate tables on rank 0 (NCCL send/recv), which finishes exactly like the single-GPU path.
+Protocol of the sharded digitizer, one library call per rank (exactness argument in DESIGN.md §6):
+  1. every rank: dense pass over its shard (+1 halo sample for the FSK conjugate product) -> tile table;
+  2. the tile-level finish (finish.cu) on every rank, with three NCCL all-gathers of 32, 16 and 16 bytes per rank on the
+     context stream, each folded over the ranks before it: the run that ends right before the shard, the class of the
+     candidate preceding it and the position of the last firing before it;
+  3. every rank ends with the (state, length) rows of its own shard; ``merge_shard_rows`` joins them, merging equal states
+     that meet at a shard edge.
 """
 import ctypes as C
 import math
@@ -219,45 +219,6 @@ def nccl_allgather_wide(ctx, world, values):
     return recv
 
 
-def demod_digitize_sharded(ctx, hx, sb: ShardBuffer, global_offset, n_total, noise_mag, mod_type, center, tolerance,
-                           samples_per_symbol, bits_per_symbol=1, center_spacing=0.1, d_qad=None, root=0):
-    """FSK/ASK demod + digitize of a capture sharded over the ranks.  Returns the (k,2) pulse table on `root`
-    (None elsewhere).  `d_qad` (optional DeviceArray[n_local]) receives this rank's demodulated samples."""
-    lib = ctx.lib
-    code = _lib.demod_mod_code(mod_type)
-    summary = (C.c_int64 * 4)()
-    ctx.check(lib.urh_shard_dense(ctx.handle, C.c_void_p(sb.shard.ptr), _lib.dtype_code(sb.dtype), sb.n, int(hx.rank > 0),
-                                  float(noise_mag), code, float(center), int(tolerance), int(bits_per_symbol), float(center_spacing),
-                                  C.c_void_p(d_qad.ptr if d_qad is not None else 0), summary))
-    mine = (int(summary[0]), int(summary[1]), int(summary[2]), int(summary[3]))
-    every = hx.allgather(mine)
-    carry = fold_carry([(c, l, w) for c, l, w, _ in every])[hx.rank]
-    count = C.c_int64(0)
-    d_pos, d_cls = C.c_void_p(), C.c_void_p()
-    ctx.check(lib.urh_shard_candidates(ctx.handle, int(carry is not None), carry[0] if carry else 0, carry[1] if carry else 0,
-                                       int(global_offset), C.byref(count), C.byref(d_pos), C.byref(d_cls), None))
-    counts = hx.allgather(int(count.value))
-    total = int(sum(counts))
-    pos_all = cls_all = None
-    if hx.rank == root:
-        pos_all = DeviceArray(ctx, (max(total, 1),), np.int64)
-        cls_all = DeviceArray(ctx, (max(total, 1),), np.int16)
-    b8 = (C.c_int64 * hx.world)(*[c * 8 for c in counts])
-    b2 = (C.c_int64 * hx.world)(*[c * 2 for c in counts])
-    ctx.check(lib.urh_nccl_gatherv(ctx.handle, d_pos, C.c_void_p(pos_all.ptr if pos_all else 0), b8, root))
-    ctx.check(lib.urh_nccl_gatherv(ctx.handle, d_cls, C.c_void_p(cls_all.ptr if cls_all else 0), b2, root))
-    if hx.rank != root:
-        ctx.sync()
-        return None
-    k = C.c_int64(0)
-    ctx.check(lib.urh_pulses_from_table(ctx.handle, C.c_void_p(pos_all.ptr), C.c_void_p(cls_all.ptr), total, int(n_total),
-                                        int(tolerance), code, int(samples_per_symbol), every[0][3], C.byref(k)))
-    rows = np.empty((k.value, 2), dtype=np.int64)
-    if k.value:
-        ctx.check(lib.urh_fetch_pulses(ctx.handle, rows.ctypes.data_as(C.c_void_p), k.value))
-    return rows
-
-
 def nccl_allgather_i64(ctx, world, values):
     """all-gather a few int64 per rank over NCCL (device-staged, ~tens of microseconds) -> array [world, len(values)]"""
     send = np.ascontiguousarray(values, dtype=np.int64)
@@ -267,14 +228,6 @@ def nccl_allgather_i64(ctx, world, values):
     return recv
 
 
-def previous_nonempty(values, counts, rank, default):
-    """value of the nearest rank < `rank` whose count is non-zero, else `default`"""
-    for r in range(rank - 1, -1, -1):
-        if counts[r] > 0:
-            return values[r]
-    return default
-
-
 def demod_digitize_distributed(ctx, rank, world, sb: ShardBuffer, global_offset, n_total, noise_mag, mod_type, center, tolerance,
                                samples_per_symbol, bits_per_symbol=1, center_spacing=0.1, d_qad=None, fetch=True, qad_source=None):
     """Sharded FSK/ASK demod + digitize with a DISTRIBUTED finish: no gather, every rank ends with the rows of its own
@@ -282,9 +235,6 @@ def demod_digitize_distributed(ctx, rank, world, sb: ShardBuffer, global_offset,
     tile-level finish whose three 16-byte exchanges (run carry / class of the last candidate / position of the last firing)
     are NCCL all-gathers enqueued on the context stream — the host waits once, for the row count.
     ``qad_source``: the shard is already demodulated (float32 DeviceArray) -> digitize from it instead of the IQ samples."""
-    if os.environ.get("URH_B200_DIST_STEPWISE"):
-        return demod_digitize_distributed_stepwise(ctx, rank, world, sb, global_offset, n_total, noise_mag, mod_type, center, tolerance,
-                                                   samples_per_symbol, bits_per_symbol, center_spacing, d_qad, fetch, qad_source)
     lib = ctx.lib
     code = _lib.demod_mod_code(mod_type)
     k = C.c_int64(0)
@@ -292,48 +242,6 @@ def demod_digitize_distributed(ctx, rank, world, sb: ShardBuffer, global_offset,
                                      C.c_void_p(qad_source.ptr if qad_source is not None else 0), sb.n, int(rank > 0), float(noise_mag), code,
                                      float(center), int(tolerance), int(samples_per_symbol), int(bits_per_symbol), float(center_spacing),
                                      C.c_void_p(d_qad.ptr if d_qad is not None else 0), int(global_offset), int(n_total), C.byref(k)))
-    if not fetch:
-        return int(k.value)
-    rows = np.empty((k.value, 2), dtype=np.int64)
-    if k.value:
-        ctx.check(lib.urh_fetch_pulses(ctx.handle, rows.ctypes.data_as(C.c_void_p), k.value))
-    return rows
-
-
-def demod_digitize_distributed_stepwise(ctx, rank, world, sb: ShardBuffer, global_offset, n_total, noise_mag, mod_type, center, tolerance,
-                               samples_per_symbol, bits_per_symbol=1, center_spacing=0.1, d_qad=None, fetch=True, qad_source=None):
-    """Call-by-call variant (host folds between the stages; kept as the reference for the one-call path).
-    Sharded FSK/ASK demod + digitize with a DISTRIBUTED finish: no gather, every rank ends with the rows of its own
-    shard (``merge_shard_rows`` joins them).  Three NCCL all-gathers of a few int64 per rank are the whole exchange:
-      (last_cls, last_len, whole, init_cls)  ->  run carry into the shard;
-      (candidate count, class of the last candidate)  ->  fire decision of the shard's first candidate;
-      (firing count, position of the last firing)  ->  length of the shard's first pulse.
-    ``qad_source``: the shard is already demodulated (float32 DeviceArray) -> digitize from it instead of the IQ samples."""
-    lib = ctx.lib
-    code = _lib.demod_mod_code(mod_type)
-    summary = (C.c_int64 * 4)()
-    if qad_source is not None:
-        ctx.check(lib.urh_shard_dense_qad(ctx.handle, C.c_void_p(qad_source.ptr), sb.n, code, float(center), int(tolerance),
-                                          int(bits_per_symbol), float(center_spacing), summary))
-    else:
-        ctx.check(lib.urh_shard_dense(ctx.handle, C.c_void_p(sb.shard.ptr), _lib.dtype_code(sb.dtype), sb.n, int(rank > 0),
-                                      float(noise_mag), code, float(center), int(tolerance), int(bits_per_symbol),
-                                      float(center_spacing), C.c_void_p(d_qad.ptr if d_qad is not None else 0), summary))
-    every = nccl_allgather_i64(ctx, world, list(summary))
-    carry = fold_carry([(int(c), int(l), int(w)) for c, l, w, _ in every])[rank]
-    init_cls = int(every[0][3])
-    count, last_cls = C.c_int64(0), C.c_int(0)
-    ctx.check(lib.urh_shard_candidates(ctx.handle, int(carry is not None), carry[0] if carry else 0, carry[1] if carry else 0,
-                                       int(global_offset), C.byref(count), None, None, C.byref(last_cls)))
-    cc = nccl_allgather_i64(ctx, world, [count.value, last_cls.value])
-    prev_cls = int(previous_nonempty(cc[:, 1], cc[:, 0], rank, init_cls))
-    fired, last_pos = C.c_int64(0), C.c_int64(-1)
-    ctx.check(lib.urh_shard_fire(ctx.handle, prev_cls, C.byref(fired), C.byref(last_pos)))
-    ff = nccl_allgather_i64(ctx, world, [fired.value, last_pos.value])
-    prev_fired = int(previous_nonempty(ff[:, 1], ff[:, 0], rank, -1))
-    k = C.c_int64(0)
-    ctx.check(lib.urh_shard_rows(ctx.handle, int(n_total), int(tolerance), code, int(samples_per_symbol), prev_fired,
-                                 int(rank == world - 1), C.byref(k)))
     if not fetch:
         return int(k.value)
     rows = np.empty((k.value, 2), dtype=np.int64)
@@ -414,7 +322,7 @@ def demod_center_digitize_distributed(ctx, rank, world, sb: ShardBuffer, global_
     landed are demodulated (the halo sample must already be in ``sb.halo``); ``rows_out``: pinned int64 buffer for the rows."""
     lib = ctx.lib
     code = _lib.demod_mod_code(mod_type)
-    if bits_per_symbol == 1 and not os.environ.get("URH_B200_DIST_STEPWISE"):
+    if bits_per_symbol == 1:
         center, state, k = C.c_double(0.0), C.c_int(0), C.c_int64(0)
         if host_iq is not None:
             ctx.check(lib.urh_shard_demod_center_digitize_host(ctx.handle, host_iq.ctypes.data_as(C.c_void_p), _lib.dtype_code(sb.dtype), sb.n,
