@@ -113,7 +113,7 @@ int urh_afp_demod_tiles(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, fl
                         int halo, int64_t* h_kept);
 int urh_center_window_stats(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out5);
 /* {np.mean, np.var} of the same window as numpy computes them for a float32 array — float32 pairwise sums replayed bit for bit
- * (AutoInterpretation.py:240: the histogram's bin width); urh_center_stats uses it unless URH_B200_CENTER_DOUBLE is set. */
+ * (AutoInterpretation.py:240: the histogram's bin width); urh_center_stats uses it. */
 int urh_center_window_var(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out2);
 int urh_center_histogram_tiles(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double hmin, double hstep,
                                int64_t nbins, int64_t* h_hist);
@@ -423,20 +423,6 @@ int urh_nccl_sendrecv(urh_ctx* ctx, const void* d_send, size_t send_bytes, int s
                       int recv_peer);
 int urh_nccl_allgather_host(urh_ctx* ctx, const void* h_send, void* h_recv, size_t bytes_per_rank);
 int urh_nccl_allreduce_host_i64(urh_ctx* ctx, int64_t* h_buf, int64_t count, int op);
-/* the same few-bytes all-gather over NVLink peer memory, one small kernel per rank (p2p.cu): every rank creates a mailbox and
- * hands its 64-byte IPC handle to the launcher plumbing; urh_p2p_open maps the peers' mailboxes (world <= 8, one node). */
-int urh_p2p_create(urh_ctx* ctx, char* out_handle64);
-int urh_p2p_open(urh_ctx* ctx, const char* handles, int rank, int world);
-int urh_p2p_close(urh_ctx* ctx);
-int urh_p2p_allgather_host(urh_ctx* ctx, const void* h_send, void* h_recv, size_t bytes_per_rank);
-/* The same exchange between DEVICE buffers, enqueued on the context stream with no host synchronisation (what the sharded chains
- * urh_shard_* use between their kernels when the mailboxes are open; NCCL otherwise): all-gather of 8..240 bytes per rank (a multiple
- * of 8); sum over ranks of min(*d_count, max_words) uint64 words (max_words <= 6000, d_out must not alias d_in, d_count a device
- * pointer or NULL).  A peer that does not show up within ~5 s raises a flag instead of hanging the GPU: urh_p2p_check, called after
- * the next synchronisation, returns URH_ERR_CUDA and closes the mailboxes. */
-int urh_p2p_allgather_dev(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank);
-int urh_p2p_allreduce_u64_dev(urh_ctx* ctx, const void* d_in, void* d_out, const int64_t* d_count, int max_words);
-int urh_p2p_check(urh_ctx* ctx);
 
 /* ---- measurement utilities (not part of the reference's API surface) -------------------------------- */
 /* CUDA-event timing of the dominant (dense, sample-rate) kernel of the last demod/digitize call */

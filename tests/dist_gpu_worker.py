@@ -17,7 +17,7 @@ def main():
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from conftest import synth_fsk
     from urh_b200 import _lib, dist as udist
-    from urh_b200.device import DeviceArray, to_device
+    from urh_b200.device import DeviceArray
     from urh_b200.cythonext import signal_functions as sf
     from urh_b200.ainterpretation import AutoInterpretation as AI
 
@@ -25,74 +25,6 @@ def main():
     hx = udist.HostExchange()
     udist.init_nccl(ctx, hx)
     failures = []
-    # NVLink peer mailboxes == NCCL for the few-bytes all-gathers (and they were actually opened)
-    import ctypes as C
-    rng_x = np.random.default_rng(1000 + rank)
-    if rank == 0:
-        print("DIST_GPU p2p mailboxes:", "open" if getattr(ctx, "p2p", False) else "not open (NCCL only)", flush=True)
-    if getattr(ctx, "p2p", False):
-        # device-resident exchanges (what the sharded chains use between their kernels) against NCCL
-        for it in range(200):
-            words = 1 + it % 30
-            send = rng_x.integers(-2**62, 2**62, words).astype(np.int64)
-            d_send = to_device(send, ctx)
-            d_a = DeviceArray(ctx, (world, words), np.int64)
-            d_b = DeviceArray(ctx, (world, words), np.int64)
-            ctx.check(ctx.lib.urh_p2p_allgather_dev(ctx.handle, C.c_void_p(d_send.ptr), C.c_void_p(d_a.ptr), send.nbytes))
-            ctx.check(ctx.lib.urh_nccl_allgather(ctx.handle, C.c_void_p(d_send.ptr), C.c_void_p(d_b.ptr), send.nbytes))
-            a, b = d_a.get(), d_b.get()
-            ctx.check(ctx.lib.urh_p2p_check(ctx.handle))
-            if not np.array_equal(a, b) or not np.array_equal(a[rank], send):
-                failures.append(("p2p device allgather", it))
-        for it, cnt in enumerate([1, 7, 256, 1000, 6000, 6000, 33]):
-            vals = rng_x.integers(0, 2**40, 6000).astype(np.int64)
-            d_in = to_device(vals, ctx)
-            d_out = DeviceArray(ctx, (6000,), np.int64)
-            d_out.zero()
-            d_cnt = to_device(np.array([cnt], np.int64), ctx)
-            ctx.check(ctx.lib.urh_p2p_allreduce_u64_dev(ctx.handle, C.c_void_p(d_in.ptr), C.c_void_p(d_out.ptr), C.c_void_p(d_cnt.ptr), 6000))
-            d_ref = to_device(vals, ctx)
-            ctx.check(ctx.lib.urh_nccl_allreduce_i64(ctx.handle, C.c_void_p(d_ref.ptr), 6000, 0))
-            got, ref = d_out.get(), d_ref.get()
-            ctx.check(ctx.lib.urh_p2p_check(ctx.handle))
-            if not np.array_equal(got[:cnt], ref[:cnt]) or np.any(got[cnt:] != 0):
-                failures.append(("p2p device allreduce", it, cnt))
-        # latency of the exchanges (context timer: CUDA events on the context stream)
-        d_send = to_device(np.arange(4, dtype=np.int64), ctx)
-        d_g = DeviceArray(ctx, (world, 4), np.int64)
-        d_in = to_device(np.arange(6000, dtype=np.int64), ctx)
-        d_out = DeviceArray(ctx, (6000,), np.int64)
-        d_cnt = to_device(np.array([8], np.int64), ctx)
-        d_cnt_all = to_device(np.array([6000], np.int64), ctx)
-        lat = {}
-        for name, call in [
-            ("p2p_allgather_dev", lambda: ctx.lib.urh_p2p_allgather_dev(ctx.handle, C.c_void_p(d_send.ptr), C.c_void_p(d_g.ptr), 32)),
-            ("nccl_allgather", lambda: ctx.lib.urh_nccl_allgather(ctx.handle, C.c_void_p(d_send.ptr), C.c_void_p(d_g.ptr), 32)),
-            ("p2p_allreduce_dev[8]", lambda: ctx.lib.urh_p2p_allreduce_u64_dev(ctx.handle, C.c_void_p(d_in.ptr), C.c_void_p(d_out.ptr), C.c_void_p(d_cnt.ptr), 6000)),
-            ("p2p_allreduce_dev[6000]", lambda: ctx.lib.urh_p2p_allreduce_u64_dev(ctx.handle, C.c_void_p(d_in.ptr), C.c_void_p(d_out.ptr), C.c_void_p(d_cnt_all.ptr), 6000)),
-            ("nccl_allreduce[6000]", lambda: ctx.lib.urh_nccl_allreduce_i64(ctx.handle, C.c_void_p(d_in.ptr), 6000, 0)),
-        ]:
-            for _ in range(20):
-                ctx.check(call())
-            ctx.sync()
-            hx.barrier()
-            ctx.timer_start()
-            for _ in range(200):
-                ctx.check(call())
-            lat[name] = ctx.timer_stop() * 1000.0 / 200
-        ctx.check(ctx.lib.urh_p2p_check(ctx.handle))
-        if rank == 0:
-            print("DIST_GPU exchange latency (us per call, 200 back to back):", {k: round(v, 2) for k, v in lat.items()}, flush=True)
-        for it in range(300):
-            k = 1 + it % 6
-            send = rng_x.integers(-2**62, 2**62, k).astype(np.int64)
-            a = np.empty((world, k), np.int64)
-            b = np.empty((world, k), np.int64)
-            ctx.check(ctx.lib.urh_p2p_allgather_host(ctx.handle, send.ctypes.data_as(C.c_void_p), a.ctypes.data_as(C.c_void_p), send.nbytes))
-            ctx.check(ctx.lib.urh_nccl_allgather_host(ctx.handle, send.ctypes.data_as(C.c_void_p), b.ctypes.data_as(C.c_void_p), send.nbytes))
-            if not np.array_equal(a, b) or not np.array_equal(a[rank], send):
-                failures.append(("p2p allgather", it))
-                break
     for case, (n, sps, tol, mod, dtype) in enumerate([
         (3_000_000, 100, 5, "FSK", np.float32), (1_000_003, 37, 0, "FSK", np.float32), (700_001, 50, 9, "ASK", np.float32),
         (2_500_000, 100, 5000, "FSK", np.float32), (900_000, 64, 3, "FSK", np.int16),

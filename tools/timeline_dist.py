@@ -95,7 +95,7 @@ def main():
         print(json.dumps({
             "what": "stream timeline of the sharded step (demod + detect_center + digitize), %d x 2^%d samples on %d GPUs, median of %d steps"
                     % (world, args.log2n, world, args.steps),
-            "exchange": "NVLink peer mailboxes" if getattr(ctx, "p2p", False) else "NCCL",
+            "exchange": "NCCL",
             "segments": rows,
             "step_us_median_over_ranks": float(np.median(t[:, -1]) * 1e3),
             "sum_compute_us": {"median_rank": compute_med, "slowest_rank_per_segment": compute_max},

@@ -113,13 +113,6 @@ SIGNATURES = {
     "urh_shard_candidates": (i32, [vp, i32, i32, i64, i64, C.POINTER(i64), C.POINTER(vp), C.POINTER(vp), C.POINTER(i32)]),
     "urh_nccl_allgather_host": (i32, [vp, vp, vp, szt]),
     "urh_nccl_allreduce_host_i64": (i32, [vp, vp, i64, i32]),
-    "urh_p2p_create": (i32, [vp, vp]),
-    "urh_p2p_open": (i32, [vp, vp, i32, i32]),
-    "urh_p2p_close": (i32, [vp]),
-    "urh_p2p_allgather_host": (i32, [vp, vp, vp, szt]),
-    "urh_p2p_allgather_dev": (i32, [vp, vp, vp, szt]),
-    "urh_p2p_allreduce_u64_dev": (i32, [vp, vp, vp, vp, i32]),
-    "urh_p2p_check": (i32, [vp]),
     "urh_demod_center_digitize": (i32, [vp, vp, i32, i64, f32, i32, u16, u32, i64, vp, C.POINTER(C.c_double), C.POINTER(i32), C.POINTER(i64)]),
     "urh_demod_center_digitize_host": (i32, [vp, vp, i32, i64, f32, i32, u16, u32, i64, i64, vp, vp, C.POINTER(C.c_double), C.POINTER(i32),
                                              C.POINTER(i64)]),

@@ -271,19 +271,11 @@ extern "C" int urh_center_stats(urh_ctx* ctx, const float* d_x, int64_t n, int64
     URH_CHECK(urh_center_window_stats(ctx, d_x, n, r0, r1, w));
     if (w[0] <= 0.0) return URH_OK;
     h_out[3] = w[1]; h_out[4] = w[2];
-    if (!getenv("URH_B200_CENTER_DOUBLE")) {
-        // np.var(rect) replayed bit for bit (pairwise.cu): numpy's float32 pairwise sums, float32 deviations
-        float mv[2];
-        URH_CHECK(urh_window_var_bitwise(ctx, d_x, n, (const int64_t*)ctx->center_prefix, 0, urh_div_up(n, URH_TILE) - 1, r0, r1, mv));
-        h_out[5] = (double)mv[0];
-        h_out[6] = (double)mv[1];
-        return URH_OK;
-    }
-    // population variance from the double sums (np.var semantics; numpy's float32 pairwise result differs ~1e-7)
-    const double mean = w[3] / w[0];
-    double ss = w[4] - w[0] * mean * mean;
-    if (ss < 0.0) ss = 0.0;
-    h_out[5] = mean; h_out[6] = ss / w[0];
+    // np.var(rect) replayed bit for bit (pairwise.cu): numpy's float32 pairwise sums, float32 deviations
+    float mv[2];
+    URH_CHECK(urh_window_var_bitwise(ctx, d_x, n, (const int64_t*)ctx->center_prefix, 0, urh_div_up(n, URH_TILE) - 1, r0, r1, mv));
+    h_out[5] = (double)mv[0];
+    h_out[6] = (double)mv[1];
     return URH_OK;
 }
 
@@ -1032,11 +1024,6 @@ __global__ void __launch_bounds__(256) k_center_pick(const unsigned long long* _
     (void)top_val;
 }
 
-int urh_coll_allgather(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank);   // nccl.cu: mailboxes or NCCL
-bool urh_p2p_usable(urh_ctx* ctx, size_t bytes_per_rank);
-extern "C" int urh_p2p_allreduce_u64_dev(urh_ctx* ctx, const void* d_in, void* d_out, const int64_t* d_count, int max_words);
-extern "C" int urh_nccl_allreduce_i64(urh_ctx* ctx, int64_t* d_buf, int64_t count, int op);
-
 // The chain.  ts = the demodulator's tile table of d_qad (arena); *d_plan_out stays valid until the next arena reset.
 // Enqueues everything on the context stream; no synchronisation.  world > 1: the context's NCCL communicator.
 // fine != NULL (world == 1 only): the demodulator's fine histogram of d_qad; k_center_certify may then decide the center without
@@ -1071,7 +1058,7 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     const int64_t* counts = prefix + ntiles;
     if (world > 1) {
         URH_TL_MARK(ctx, "x1 kept counts: enter");
-        URH_CHECK(urh_coll_allgather(ctx, prefix + ntiles, d_counts, sizeof(int64_t)));
+        URH_CHECK(urh_nccl_allgather(ctx, prefix + ntiles, d_counts, sizeof(int64_t)));
         URH_TL_MARK(ctx, "x1 kept counts: done");
         counts = d_counts;
     }
@@ -1080,7 +1067,7 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     const CenStats* parts = &plan->local;
     if (world > 1) {
         URH_TL_MARK(ctx, "x2 window partials: enter");
-        URH_CHECK(urh_coll_allgather(ctx, &plan->local, d_parts, sizeof(CenStats)));
+        URH_CHECK(urh_nccl_allgather(ctx, &plan->local, d_parts, sizeof(CenStats)));
         URH_TL_MARK(ctx, "x2 window partials: done");
         parts = d_parts;
     }
@@ -1093,20 +1080,12 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     if (fine) URH_LAUNCH(ctx, k_center_certify, 1, CERT_THREADS, 0, *fine, plan, (const float*)fe, (const unsigned long long*)xhist, cert_lo, cert_hi);
     URH_LAUNCH(ctx, (k_hist_interior_dev<true>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
     URH_LAUNCH(ctx, (k_hist_interior_dev<false>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
-    const unsigned long long* hist_all = hist;
-    if (world > 1) URH_TL_MARK(ctx, "x3 histogram sum: enter");
     if (world > 1) {
-        if (urh_p2p_usable(ctx, 8)) {   // NVLink mailboxes: only the plan's nbins words travel
-            unsigned long long* hist_sum;
-            URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &hist_sum));
-            URH_CHECK(urh_p2p_allreduce_u64_dev(ctx, hist, hist_sum, (const int64_t*)&plan->nbins, CEN_MAX_BINS));
-            hist_all = hist_sum;
-        } else {
-            URH_CHECK(urh_nccl_allreduce_i64(ctx, (int64_t*)hist, CEN_MAX_BINS, 0));
-        }
+        URH_TL_MARK(ctx, "x3 histogram sum: enter");
+        URH_CHECK(urh_nccl_allreduce_i64(ctx, (int64_t*)hist, CEN_MAX_BINS, 0));
+        URH_TL_MARK(ctx, "x3 histogram sum: done");
     }
-    if (world > 1) URH_TL_MARK(ctx, "x3 histogram sum: done");
-    URH_LAUNCH(ctx, k_center_pick, 1, 256, 0, hist_all, plan);
+    URH_LAUNCH(ctx, k_center_pick, 1, 256, 0, (const unsigned long long*)hist, plan);
     ctx->center_prefix = prefix;
     ctx->center_ts = ts;
     ctx->center_n = n;

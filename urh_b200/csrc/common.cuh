@@ -82,12 +82,6 @@ struct urh_ctx {
     void* nccl_stage;
     void* nccl_hstage;  // pinned twin of nccl_stage
     int nccl_rank, nccl_world;
-    // NVLink peer mailboxes (p2p.cu)
-    void* p2p_local;
-    void* p2p_peer[8];
-    void* p2p_hout;
-    int p2p_rank, p2p_world;
-    unsigned long long p2p_seq;
     // tilescan.cuh workspace (look-back scans over tile tables)
     void* ts_mem;
     int64_t ts_cap_blocks;

@@ -40,12 +40,6 @@ extern "C" int urh_ctx_create(int device, urh_ctx** out) {
     ctx->nccl_comm = nullptr;
     ctx->nccl_stage = nullptr;
     ctx->nccl_hstage = nullptr;
-    ctx->p2p_local = nullptr;
-    ctx->p2p_hout = nullptr;
-    ctx->p2p_world = 0;
-    ctx->p2p_rank = 0;
-    ctx->p2p_seq = 0;
-    for (int i = 0; i < 8; i++) ctx->p2p_peer[i] = nullptr;
     ctx->nccl_rank = 0;
     ctx->nccl_world = 1;
     ctx->stream_free_low = -1;

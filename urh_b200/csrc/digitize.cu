@@ -5,9 +5,6 @@
 #include "dense.cuh"
 #include "scan.cuh"
 #include "sparse.cuh"
-#ifndef URH_FAST_MIN_BLOCKS
-#define URH_FAST_MIN_BLOCKS 4
-#endif
 #include "fsk_fast.cuh"
 #include "dense_f32.cuh"
 #include "stream_ring.cuh"
@@ -118,35 +115,8 @@ k_dense_iq(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
 }
 
 // Fast kernel: full, aligned, order-2 FSK tiles [tile_begin, tile_begin + tile_count), tile_begin >= 1
-// (fsk_fast.cuh: float2-paired math, same bits as the generic kernel).
-template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
-__global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, URH_FAST_MIN_BLOCKS)
-k_fsk_fast(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
-           float cls_noise, int tol, UrhTileSummary* __restrict__ tiles, uint32_t* __restrict__ staging, int stage_cap,
-           int64_t tile_begin, int64_t tile_count, UrhTileStats* __restrict__ tile_stats, const UrhFine fine) {
-    extern __shared__ unsigned int s_fine[];   // [URH_FINE_NB] when STATS and fine.gh
-    const bool fine_on = STATS && fine.gh;
-    const int lane = threadIdx.x & 31;
-    const int64_t tile_rel = (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    const int64_t block_tile0 = tile_begin + (int64_t)blockIdx.x * URH_WARPS_PER_BLOCK;
-    if (fine_on) urh_fine_zero(s_fine);
-    if (tile_rel < tile_count) {
-        const int64_t tile = tile_begin + tile_rel;
-        UrhRunTracker rt;
-        if (DIGITIZE) rt.init(tol, staging + tile * (int64_t)stage_cap);
-        UrhOne one;
-        one.p = dp.one;
-        one.m = dp.mone;
-        urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
-                                                      STATS ? tile_stats + tile : nullptr, 0u, DIGITIZE ? tiles + tile : nullptr, fine,
-                                                      fine_on ? s_fine : nullptr, fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr);
-    }
-    if (fine_on) urh_fine_flush(fine, s_fine, block_tile0);
-}
-
-// The same kernel with the input staged through the shared-memory FIFO.
+// (fsk_fast.cuh: float2-paired math, same bits as the generic kernel; the input is staged through a shared-memory FIFO).
 // DIGITIZE and STATS: the speculative pass of the detect-center step; the threshold is the guess *d_thr0, margin[tile] its proof.
-#define URH_FSK_FIFO 3
 template <int DT, bool DIGITIZE, bool WRITE, bool STATS>
 __global__ void __launch_bounds__(URH_WARPS_PER_BLOCK * 32, (DT == URH_DT_F32) ? 5 : 4)   // (the integer variants spill at 48 registers)
 k_fsk_fifo(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __restrict__ qad_out, float thr0,
@@ -169,11 +139,10 @@ k_fsk_fifo(const void* __restrict__ iq, int64_t n, UrhDemodParams dp, float* __r
         one.p = dp.one;
         one.m = dp.mone;
         const uint32_t fifo = (uint32_t)__cvta_generic_to_shared(&s_fifo[threadIdx.x >> 5][0][0]);
-        urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS, URH_FSK_FIFO>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
-                                                                    STATS ? tile_stats + tile : nullptr, fifo,
-                                                                    DIGITIZE ? tiles + tile : nullptr, fine, fine_on ? s_fine : nullptr,
-                                                                    fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr,
-                                                                    (DIGITIZE && STATS) ? margin + tile : nullptr);
+        urh_fsk_full_tile<DT, DIGITIZE, WRITE, STATS>(iq, n, tile * URH_TILE, dp, qad_out, thr0, cls_noise, rt, lane, one,
+                                                      STATS ? tile_stats + tile : nullptr, fifo, DIGITIZE ? tiles + tile : nullptr, fine,
+                                                      fine_on ? s_fine : nullptr, fine_on ? urh_fine_row(fine, tile, block_tile0) : nullptr,
+                                                      (DIGITIZE && STATS) ? margin + tile : nullptr);
     }
     if (fine_on) urh_fine_flush(fine, s_fine, block_tile0);
 }
@@ -327,12 +296,9 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
         const int64_t fb = tile_lo > 1 ? tile_lo : 1, fe = tile_hi < nfull ? tile_hi : nfull;
         if (fe > fb) {
             const unsigned grid = (unsigned)urh_div_up(fe - fb, URH_WARPS_PER_BLOCK);
-            // the variant that stages its input through the shared-memory FIFO (URH_B200_FSK_NO_FIFO selects the register-fed loop)
-            static const bool fifo = getenv("URH_B200_FSK_NO_FIFO") == nullptr;
-            const bool ff = fifo;
             bool speculated = false;
             if constexpr (DT == URH_DT_F32 && MOD == URH_MOD_FSK && !DIG) {
-                if (spec && ff && tile_stats && d_qad) {
+                if (spec && tile_stats && d_qad) {
                     URH_LAUNCH(ctx, (k_fsk_fifo<DT, true, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, 0.0f, dp.noise_value,
                                tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine, (const float*)spec->tg, spec->margin);
                     spec->lo = fb;
@@ -342,20 +308,14 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
             }
             if (speculated) {
             } else if (tile_stats && d_qad && !DIG) {
-                if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
-                                   tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
-                else URH_LAUNCH(ctx, (k_fsk_fast<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
-                                tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
+                           tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
             } else if (d_qad) {
-                if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                   tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
-                else URH_LAUNCH(ctx, (k_fsk_fast<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
+                           tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
             } else {
-                if (ff) URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                   tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
-                else URH_LAUNCH(ctx, (k_fsk_fast<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                                tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
+                           tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
             }
         }
         URH_CHECK(generic(0, 1));

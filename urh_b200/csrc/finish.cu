@@ -390,9 +390,6 @@ __global__ void k_chain_last_row(UrhChain* __restrict__ chain, const int64_t* __
     if (rows > 0) chain->last_state = table[2 * (rows - 1)];
 }
 
-int urh_coll_allgather(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank);   // nccl.cu: mailboxes or NCCL
-extern "C" int urh_p2p_check(urh_ctx* ctx);
-
 // ---- driver --------------------------------------------------------------------------------------------------------------
 struct FinishShard {
     int rank, world;            // world == 1: unsharded
@@ -445,7 +442,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     if (sharded) {
         URH_LAUNCH(ctx, k_pack_stage1, 1, 1, 0, d_init, (const RunCarry*)d_tot_run, d_msg1);
         URH_TL_MARK(ctx, "x4 run carry: enter");
-        URH_CHECK(urh_coll_allgather(ctx, d_msg1, d_all1, 4 * sizeof(int64_t)));
+        URH_CHECK(urh_nccl_allgather(ctx, d_msg1, d_all1, 4 * sizeof(int64_t)));
         URH_TL_MARK(ctx, "x4 run carry: done");
         URH_LAUNCH(ctx, k_fold_carry, 1, 1, 0, (const int64_t*)d_all1, sh.rank, d_xcarry);
     }
@@ -459,7 +456,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     const int16_t* prev0 = chain ? &chain->prev_cls : d_init;
     if (sharded) {
         URH_TL_MARK(ctx, "x5 candidates: enter");
-        URH_CHECK(urh_coll_allgather(ctx, d_tot_cand, d_all2, sizeof(CandAgg)));
+        URH_CHECK(urh_nccl_allgather(ctx, d_tot_cand, d_all2, sizeof(CandAgg)));
         URH_TL_MARK(ctx, "x5 candidates: done");
         URH_LAUNCH(ctx, k_fold_prev_cls, 1, 1, 0, (const int64_t*)d_all2, sh.rank, (const int64_t*)d_all1, d_prev0);
         prev0 = d_prev0;
@@ -473,7 +470,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     const int64_t* xprev = chain ? &chain->prev_fired : d_small + 2;
     if (sharded) {
         URH_TL_MARK(ctx, "x6 firings: enter");
-        URH_CHECK(urh_coll_allgather(ctx, d_tot_fire, d_all3, sizeof(FireAgg)));
+        URH_CHECK(urh_nccl_allgather(ctx, d_tot_fire, d_all3, sizeof(FireAgg)));
         URH_TL_MARK(ctx, "x6 firings: done");
         URH_LAUNCH(ctx, k_fold_prev_fired, 1, 1, 0, (const int64_t*)d_all3, sh.rank, d_xprev);
         xprev = d_xprev;
@@ -497,7 +494,6 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
                    sh.n_total, tol, is_ask ? 1 : 0, (int64_t)sps, sh.emit_tail, row_base, raw, raw_cap, d_small);
         if (sharded && attempt == 0) URH_TL_MARK(ctx, "rows written");
         URH_CHECK(urh_read_i64(ctx, d_small, 2, got));
-        if (sharded) URH_CHECK(urh_p2p_check(ctx));   // a mailbox exchange of this step (or of the center chain before it) timed out?
         if (got[0] <= raw_cap) break;
         // rows_cap bounds a chained chunk's rows (one per candidate plus the tail), so only the unchained table can overflow
         if (attempt == 1 || chain) URH_FAIL(ctx, URH_ERR_CUDA, "finish_tiles: row buffer overflow after regrowth");

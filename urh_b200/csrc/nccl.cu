@@ -130,16 +130,9 @@ extern "C" int urh_nccl_allgather(urh_ctx* ctx, const void* d_send, void* d_recv
     URH_NCCL(ctx, g_nccl.AllGather(d_send, d_recv, bytes_per_rank, URH_NCCL_UINT8, (urh_ncclComm_t)ctx->nccl_comm, ctx->stream));
     return URH_OK;
 }
+
 // variable-length gather to `root`: h_bytes[world] are the per-rank byte counts (known to every rank);
 // root receives rank r's block at d_recv + sum(h_bytes[0..r))
-// The few-bytes all-gathers of the sharded chains: NVLink mailboxes (p2p.cu) when every rank opened them, NCCL otherwise.
-bool urh_p2p_usable(urh_ctx* ctx, size_t bytes_per_rank);
-extern "C" int urh_p2p_allgather_dev(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank);
-int urh_coll_allgather(urh_ctx* ctx, const void* d_send, void* d_recv, size_t bytes_per_rank) {
-    if (urh_p2p_usable(ctx, bytes_per_rank)) return urh_p2p_allgather_dev(ctx, d_send, d_recv, bytes_per_rank);
-    return urh_nccl_allgather(ctx, d_send, d_recv, bytes_per_rank);
-}
-
 extern "C" int urh_nccl_gatherv(urh_ctx* ctx, const void* d_send, void* d_recv, const int64_t* h_bytes, int root) {
     URH_CHECK(need_comm(ctx));
     urh_ncclComm_t comm = (urh_ncclComm_t)ctx->nccl_comm;

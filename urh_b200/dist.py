@@ -15,7 +15,6 @@ Protocol of the sharded digitizer, one library call per rank (exactness argument
 """
 import ctypes as C
 import math
-import os
 
 import numpy as np
 
@@ -91,28 +90,6 @@ def init_nccl(ctx: _lib.Context, hx: HostExchange):
             raise RuntimeError("urh_nccl_unique_id failed (libnccl.so.2 not loadable?)")
     ident = hx.broadcast(bytes(buf.raw) if hx.rank == 0 else None, src=0)
     ctx.check(ctx.lib.urh_nccl_init(ctx.handle, C.c_char_p(ident), hx.rank, hx.world))
-    init_p2p(ctx, hx)
-
-
-def init_p2p(ctx: _lib.Context, hx: HostExchange):
-    """NVLink peer mailboxes for the few-bytes exchanges (p2p.cu): host-side all-gathers and the device-resident, stream-ordered
-    all-gather / histogram sum the sharded chains use between their kernels.  Used only if EVERY rank could map every peer (one
-    node, <= 8 GPUs, CUDA IPC available); otherwise those exchanges stay on NCCL.
-    Opt-in with URH_B200_P2P=1: the exchanges carry a few bytes to a few KB, so a sharded step's cost is dominated by rank skew and
-    the small device stages between the exchanges rather than by the collective's latency, and NCCL stays the default
-    (DESIGN.md section 6)."""
-    ctx.p2p = False
-    ok = hx.world <= 8 and hx.world > 1 and os.environ.get("URH_B200_P2P", "0") == "1"
-    handle = C.create_string_buffer(64)
-    if ok:
-        ok = ctx.lib.urh_p2p_create(ctx.handle, handle) == 0
-    handles = hx.allgather(bytes(handle.raw) if ok else None)
-    ok = ok and all(h is not None for h in handles)
-    if ok:
-        ok = ctx.lib.urh_p2p_open(ctx.handle, C.c_char_p(b"".join(handles)), hx.rank, hx.world) == 0
-    ctx.p2p = all(hx.allgather(bool(ok)))
-    if ok and not ctx.p2p:
-        ctx.lib.urh_p2p_close(ctx.handle)
 
 
 class ShardBuffer(object):
@@ -219,15 +196,6 @@ def nccl_allgather_wide(ctx, world, values):
     return recv
 
 
-def nccl_allgather_i64(ctx, world, values):
-    """all-gather a few int64 per rank over NCCL (device-staged, ~tens of microseconds) -> array [world, len(values)]"""
-    send = np.ascontiguousarray(values, dtype=np.int64)
-    recv = np.empty((world, len(send)), dtype=np.int64)
-    entry = ctx.lib.urh_p2p_allgather_host if (getattr(ctx, "p2p", False) and send.nbytes <= 48) else ctx.lib.urh_nccl_allgather_host
-    ctx.check(entry(ctx.handle, send.ctypes.data_as(C.c_void_p), recv.ctypes.data_as(C.c_void_p), send.nbytes))
-    return recv
-
-
 def demod_digitize_distributed(ctx, rank, world, sb: ShardBuffer, global_offset, n_total, noise_mag, mod_type, center, tolerance,
                                samples_per_symbol, bits_per_symbol=1, center_spacing=0.1, d_qad=None, fetch=True, qad_source=None):
     """Sharded FSK/ASK demod + digitize with a DISTRIBUTED finish: no gather, every rank ends with the rows of its own
@@ -307,7 +275,7 @@ def detect_center_distributed(ctx, rank, world, sb: ShardBuffer, noise_mag, mod_
         ctx.check(lib.urh_nccl_allreduce_host_i64(ctx.handle, y.ctypes.data_as(C.c_void_p), len(y), 0))
         return y
 
-    return center_protocol(rank, world, kept.value, window_stats, histogram, lambda v: nccl_allgather_i64(ctx, world, v), allreduce,
+    return center_protocol(rank, world, kept.value, window_stats, histogram, lambda v: nccl_allgather_wide(ctx, world, v), allreduce,
                            max_size)
 
 
