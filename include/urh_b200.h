@@ -315,6 +315,27 @@ int urh_afp_demod_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t 
 int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, float center, uint16_t tolerance,
                                   uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing, int64_t chunk_samples,
                                   int ring, float* h_qad_out, int64_t* k);
+/* Auto-interpretation from a host capture of any size (stats.cu, convert.cu; DESIGN.md §4.11, "Noise level, segmentation and
+ * conversion").  Results are bit-identical to the resident entry points named.
+ * urh_noise_chunk_stats_iq_stream: urh_noise_chunk_stats_iq through the windowed ring; each window uploads whole slices of the noise
+ *   chunks (urh_stream_windows with URH_FILTER_NOISE, p0 = chunksize, p1 = nchunks), the head before n - nchunks * chunksize is not read.
+ * urh_segment_messages_iq_stream: urh_segment_messages over urh_get_magnitudes (float64) of the capture, chunk by chunk (chunks of whole
+ *   tiles as urh_stream_schedule cuts them); *k = number of messages, fetched with urh_fetch_segments ((start, end) int64 pairs).
+ * urh_convert_iq_stream: urh_convert_iq of n samples (2 n elements) from host h_src into host h_dst through the windowed ring
+ *   (URH_FILTER_CONVERT, p0 = dst_dtype).
+ * Footprints: URH_FILTER_NOISE / URH_FILTER_CONVERT in urh_stream_filter_footprint, URH_STREAM_ENTRY_SEGMENT_MESSAGES in
+ *   urh_stream_footprint (tolerance and rows unused).  URH_STREAM_ENTRY_ESTIMATE (with URH_STREAM_RESIDENT only) is the resident
+ *   AutoInterpretation.estimate: the capture, its float64 magnitudes and the resident order-2 PSK demodulation, the largest of the
+ *   three (AutoInterpretation.py:373-471). */
+#define URH_STREAM_ENTRY_SEGMENT_MESSAGES 4
+#define URH_STREAM_ENTRY_ESTIMATE 5
+int urh_noise_chunk_stats_iq_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, int64_t chunksize, int nchunks,
+                                    int64_t chunk_samples, int ring, double* h_sum, double* h_max);
+int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_threshold, int64_t chunk_samples,
+                                   int ring, int64_t* k);
+int urh_fetch_segments(urh_ctx* ctx, int64_t* h_segments, int64_t k);
+int urh_convert_iq_stream(urh_ctx* ctx, const void* h_src, int src_dtype, void* h_dst, int dst_dtype, int64_t n, int64_t chunk_samples,
+                          int ring);
 int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows, int64_t* bytes);
 int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
 int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3);
@@ -353,6 +374,8 @@ int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
 #define URH_FILTER_STFT 3
 #define URH_FILTER_DB 4
 #define URH_FILTER_IMAGES 5
+#define URH_FILTER_NOISE 6    /* urh_noise_chunk_stats_iq_stream (below) */
+#define URH_FILTER_CONVERT 7  /* urh_convert_iq_stream (below) */
 int urh_convolve_c128_stream(urh_ctx* ctx, const float* h_x, int64_t n, const double* h_taps, int m, int64_t offset, int64_t out_len,
                              int64_t chunk_samples, int ring, float* h_y);
 int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, const float* h_taps, int m, int64_t chunk_samples, int ring, float* h_y);

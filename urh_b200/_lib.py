@@ -20,10 +20,12 @@ DT_I8, DT_U8, DT_I16, DT_U16, DT_F32 = 0, 1, 2, 3, 4
 MOD_ASK, MOD_FSK, MOD_PSK, MOD_QAM, MOD_GFSK, MOD_OQPSK = 0, 1, 2, 3, 4, 5
 # streamed entry points (include/urh_b200.h)
 STREAM_AFP_DEMOD, STREAM_GRAB_PULSE_LENS, STREAM_DEMOD_DIGITIZE, STREAM_DEMOD_CENTER_DIGITIZE = 0, 1, 2, 3
+STREAM_SEGMENT_MESSAGES, STREAM_ESTIMATE = 4, 5
 STREAM_QAD_OUT, STREAM_RESIDENT, STREAM_QAD_ON_DEVICE = 0x10, 0x20, 0x40
 STREAM_PSK, STREAM_PSK4 = 0x80, 0x100
 STREAM_UPLOAD, STREAM_DOWNLOAD, STREAM_HALO = 1, 2, 4
 FILTER_CONVOLVE, FILTER_FIR, FILTER_DC, FILTER_STFT, FILTER_DB, FILTER_IMAGES = 0, 1, 2, 3, 4, 5
+FILTER_NOISE, FILTER_CONVERT = 6, 7
 
 _DTYPE_CODE = {
     np.dtype(np.int8): DT_I8,
@@ -169,6 +171,10 @@ SIGNATURES = {
                                                C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
     "urh_afp_demod_psk_stream": (i32, [vp, vp, i32, i64, f32, i32, f32, i64, i32, vp]),
     "urh_demod_digitize_psk_stream": (i32, [vp, vp, i32, i64, f32, f32, u16, u32, u8, f32, i64, i32, vp, C.POINTER(i64)]),
+    "urh_noise_chunk_stats_iq_stream": (i32, [vp, vp, i32, i64, i64, i32, i64, i32, vp, vp]),
+    "urh_segment_messages_iq_stream": (i32, [vp, vp, i32, i64, f32, i64, i32, C.POINTER(i64)]),
+    "urh_fetch_segments": (i32, [vp, vp, i64]),
+    "urh_convert_iq_stream": (i32, [vp, vp, i32, vp, i32, i64, i64, i32]),
     "urh_stream_footprint": (i32, [i64, i32, i32, i64, i32, i32, i64, C.POINTER(i64)]),
     "urh_stream_schedule": (i32, [i64, i64, i32, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_stats": (i32, [vp, vp]),

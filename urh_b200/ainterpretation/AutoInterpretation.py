@@ -92,18 +92,36 @@ def detect_noise_level(magnitudes):
     return _noise_from_chunk_stats(n, chunksize, sums, maxs, d.dtype)
 
 
+def noise_level_streams(n: int, dtype, budget: int) -> bool:
+    """whether detect_noise_level_iq streams a host capture of n samples: its resident call (the capture uploaded whole) does not
+    fit the device budget (signal_functions.filter_use_stream's rule)"""
+    if n <= 3:
+        return False
+    chunksize, nchunks = _chunking(n)
+    return signal_functions.filter_use_stream(_lib.FILTER_NOISE, n, 0, dtype, chunksize, nchunks, budget)
+
+
 def detect_noise_level_iq(iq):
     """detect_noise_level(IQArray(iq).magnitudes) without materialising the float64 magnitude array
-    (8 B/sample in the reference, SURVEY §5): `iq` is an (n,2) array (host or device)."""
+    (8 B/sample in the reference, SURVEY §5): `iq` is an (n,2) array (host or device).  A host capture whose upload does not fit
+    the device budget streams through the device (urh_noise_chunk_stats_iq_stream; the same sums and maxima)."""
     n = len(iq)
     if n <= 3:
         return 0
     on_device = isinstance(iq, DeviceArray)
     ctx = iq.ctx if on_device else _lib.default_context()
-    d = iq if on_device else to_device(np.ascontiguousarray(iq), ctx)
     chunksize, nchunks = _chunking(n)
     sums = np.empty(nchunks, dtype=np.float64)
     maxs = np.empty(nchunks, dtype=np.float64)
+    if not on_device:
+        iq = np.ascontiguousarray(iq)
+        if noise_level_streams(n, iq.dtype, signal_functions.device_budget(ctx)):
+            ctx.check(ctx.lib.urh_noise_chunk_stats_iq_stream(ctx.handle, iq.ctypes.data_as(C.c_void_p), _lib.dtype_code(iq.dtype), n,
+                                                              chunksize, nchunks, signal_functions.FILTER_STREAM_CHUNK,
+                                                              signal_functions.STREAM_RING, sums.ctypes.data_as(C.c_void_p),
+                                                              maxs.ctypes.data_as(C.c_void_p)))
+            return _noise_from_chunk_stats(n, chunksize, sums, maxs, np.float64)
+    d = iq if on_device else to_device(iq, ctx)
     ctx.check(ctx.lib.urh_noise_chunk_stats_iq(ctx.handle, C.c_void_p(d.ptr), _lib.dtype_code(d.dtype), n, chunksize, nchunks,
                                                sums.ctypes.data_as(C.c_void_p), maxs.ctypes.data_as(C.c_void_p)))
     return _noise_from_chunk_stats(n, chunksize, sums, maxs, np.float64)
@@ -112,6 +130,33 @@ def detect_noise_level_iq(iq):
 # ---- segmentation (AutoInterpretation.py:94-148) -----------------------------------------------------------------
 def segment_messages_from_magnitudes(magnitudes, noise_threshold: float):
     return c_auto_interpretation.segment_messages_from_magnitudes(magnitudes, noise_threshold)
+
+
+def segment_messages_iq(iq, noise_threshold: float) -> list:
+    """segment_messages_from_magnitudes(get_magnitudes(iq), noise_threshold) of an (n,2) capture (host or device): the float64
+    magnitudes estimate() segments.  A host capture whose resident call (capture, magnitudes, run tables) does not fit the device
+    budget streams through the device chunk by chunk (urh_segment_messages_iq_stream; the same segments)."""
+    n = len(iq)
+    if n == 0:
+        return []
+    on_device = isinstance(iq, DeviceArray)
+    ctx = iq.ctx if on_device else _lib.default_context()
+    if not on_device:
+        iq = np.ascontiguousarray(iq)
+        if signal_functions.use_stream(n, iq.dtype, 0, _lib.STREAM_SEGMENT_MESSAGES, signal_functions.device_budget(ctx)):
+            k = C.c_int64(0)
+            ctx.check(ctx.lib.urh_segment_messages_iq_stream(ctx.handle, iq.ctypes.data_as(C.c_void_p), _lib.dtype_code(iq.dtype), n,
+                                                             float(noise_threshold), signal_functions.STREAM_CHUNK,
+                                                             signal_functions.STREAM_RING, C.byref(k)))
+            seg = np.empty((k.value, 2), dtype=np.int64)
+            ctx.check(ctx.lib.urh_fetch_segments(ctx.handle, seg.ctypes.data_as(C.c_void_p), k.value))
+            return [(int(a), int(b)) for a, b in seg]
+    d_iq = iq if on_device else to_device(iq, ctx)
+    d_mag = util.get_magnitudes(d_iq)
+    try:
+        return segment_messages_from_magnitudes(d_mag, noise_threshold)
+    finally:
+        d_mag.free()
 
 
 def merge_message_segments_for_ook(segments: list):
@@ -185,11 +230,12 @@ def detect_modulation(data, wavelet_scale=4, median_filter_order=11) -> str:
 
 
 def detect_modulation_for_messages(signal, message_indices: list) -> str:
+    """each message converted from its own slice: the same complex64 values as slicing the whole capture's conversion (the
+    conversion is element-wise), without converting or uploading the rest of the capture"""
     max_messages = 100
     found = []
-    samples = signal.as_complex64()
     for start, end in message_indices[0:max_messages]:
-        mod = detect_modulation(samples[start:end])
+        mod = detect_modulation(signal.subarray(start, end).as_complex64())
         if mod is not None:
             found.append(mod)
     if len(found) == 0:
@@ -386,38 +432,67 @@ def get_bit_length_from_plateau_lengths(merged_plateau_lengths) -> int:
 
 
 # ---- orchestrator (AutoInterpretation.py:373-471) ------------------------------------------------------------------------
+def estimate_streams(n: int, dtype, budget: int) -> bool:
+    """whether estimate() takes its host path: the resident path's footprint (urh_stream_footprint, URH_STREAM_ENTRY_ESTIMATE:
+    capture, float64 magnitudes, the resident order-2 PSK demodulation, the largest of the three) exceeds the device budget"""
+    return signal_functions.stream_footprint(n, dtype, 0, _lib.STREAM_ESTIMATE | _lib.STREAM_RESIDENT) > budget
+
+
+def _demodulate(iq, noise, modulation):
+    if modulation in ("OOK", "ASK"):
+        return signal_functions.afp_demod(iq, noise, "ASK", 2)
+    if modulation in ("FSK", "PSK"):
+        return signal_functions.afp_demod(iq, noise, modulation, 2)
+    raise ValueError("Unsupported Modulation")
+
+
+def _center_and_plateaus(msg):
+    center = detect_center(msg)
+    if center is None:
+        return None, None
+    return center, c_auto_interpretation.get_plateau_lengths(msg, center, percentage=25)
+
+
 def estimate(iq_array, noise: float = None, modulation: str = None) -> dict:
+    """AutoInterpretation.py:373-471.  A capture whose resident path does not fit the device budget (estimate_streams) stays on the
+    host: the noise level and the segmentation stream through the device, afp_demod streams (ASK / FSK / PSK), and each message's
+    demodulated slice is uploaded once for its center and plateau lengths.  Both paths give the same dict.  Limit: a single message
+    whose per-message work does not fit the device raises MemoryError."""
     from ..signalprocessing.IQArray import IQArray
 
     if isinstance(iq_array, np.ndarray):
         iq_array = IQArray(iq_array)
     ctx = _lib.default_context()
-    d_iq = to_device(np.ascontiguousarray(iq_array._peek()), ctx)  # one upload, everything below stays in HBM
-    d_mag = util.get_magnitudes(d_iq)
-    noise = detect_noise_level(d_mag) if noise is None else noise
-    message_indices = segment_messages_from_magnitudes(d_mag, noise_threshold=noise)
-    d_mag.free()
+    host = np.ascontiguousarray(iq_array._peek())
+    on_host = estimate_streams(len(host), host.dtype, signal_functions.device_budget(ctx))
+    if on_host:
+        noise = detect_noise_level_iq(host) if noise is None else noise
+        message_indices = segment_messages_iq(host, noise)
+    else:
+        d_iq = to_device(host, ctx)  # one upload, everything below stays in HBM
+        d_mag = util.get_magnitudes(d_iq)
+        noise = detect_noise_level(d_mag) if noise is None else noise
+        message_indices = segment_messages_from_magnitudes(d_mag, noise_threshold=noise)
+        d_mag.free()
     modulation = detect_modulation_for_messages(iq_array, message_indices) if modulation is None else modulation
     if modulation is None:
         return None
     if modulation == "OOK":
         message_indices = merge_message_segments_for_ook(message_indices)
-    if modulation == "OOK" or modulation == "ASK":
-        data = signal_functions.afp_demod(d_iq, noise, "ASK", 2)
-    elif modulation == "FSK":
-        data = signal_functions.afp_demod(d_iq, noise, "FSK", 2)
-    elif modulation == "PSK":
-        data = signal_functions.afp_demod(d_iq, noise, "PSK", 2)
-    else:
-        raise ValueError("Unsupported Modulation")
+    data = _demodulate(host if on_host else d_iq, noise, modulation)
 
     centers, bit_lengths, tolerances = [], [], []
     for start, end in message_indices:
         msg = data[int(start):int(end)]
-        center = detect_center(msg)
+        if on_host:   # the message's qad uploaded once (freed with the DeviceArray)
+            try:
+                center, plateau_lengths = _center_and_plateaus(to_device(np.ascontiguousarray(msg), ctx))
+            except MemoryError as e:
+                raise MemoryError("estimate: the message [%d, %d) of %d samples does not fit the device" % (start, end, end - start)) from e
+        else:
+            center, plateau_lengths = _center_and_plateaus(msg)
         if center is None:
             continue
-        plateau_lengths = c_auto_interpretation.get_plateau_lengths(msg, center, percentage=25)
         tolerance = estimate_tolerance_from_plateau_lengths(plateau_lengths)
         if tolerance is None:
             tolerance = 0

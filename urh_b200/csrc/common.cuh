@@ -95,6 +95,8 @@ struct urh_ctx {
     int64_t stream_free_low, stream_chunks;
     size_t arena_live;   // bytes of the arena requests live since the last reset (released ones not counted)
     size_t arena_peak;   // the most arena_live reached since the last reset
+    // (start, end) pairs of the last urh_segment_messages_iq_stream call (urh_fetch_segments)
+    std::vector<int64_t> segments;
 };
 
 #define URH_CUDA(ctx, call)                                                                         \

@@ -1,7 +1,7 @@
 // Sample-format conversions of IQArray.convert_to (IQArray.py:127-200) on the GPU (SURVEY §8f row 2): the capture formats
 // cs8 / cu8 / cs16 / cu16 / float32 into each other, element by element, with numpy's integer wrap-around and C's
 // float -> int truncation.  One pass, 1..4 bytes read and written per element.
-#include "common.cuh"
+#include "stream_ring.cuh"
 
 #include <type_traits>
 
@@ -73,4 +73,26 @@ extern "C" int urh_convert_iq(urh_ctx* ctx, const void* d_in, int in_dtype, void
         case URH_DT_F32: return convert_from<float>(ctx, d_in, d_out, out_dtype, count, grid);
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "Data type not supported");
     }
+}
+
+// The same from a host capture of any size to a host output through the windowed ring (stream_ring.cuh): chunks of whole samples
+// (urh_filter_windows, URH_FILTER_CONVERT), each converted by urh_convert_iq, so every element is the resident call's.  n = samples.
+extern "C" int urh_convert_iq_stream(urh_ctx* ctx, const void* h_src, int src_dtype, void* h_dst, int dst_dtype, int64_t n,
+                                     int64_t chunk_samples, int ring) {
+    if (!h_src || !h_dst) URH_FAIL(ctx, URH_ERR_INVALID, "convert_iq_stream: bad arguments");
+    if (urh_iq_bytes(src_dtype) == 0 || urh_iq_bytes(dst_dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Data type not supported");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    if (n == 0) return URH_OK;
+    urh_arena_reset(ctx);   // the call takes no arena: its peak (urh_stream_stats) is 0, not a previous call's
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_CONVERT, n, n, dst_dtype, 0, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_CONVERT, n, n, src_dtype, dst_dtype, 0, 0, chunk_samples, L));
+    return stream_run_windows(ctx, win, R, (const char*)h_src, urh_iq_bytes(src_dtype), L.in, L.z.in_slot, true,
+                              [&](int64_t, const UrhWindow& w, int s) {
+                                  return urh_convert_iq(ctx, L.in + s * L.z.in_slot, src_dtype, L.out + s * L.z.out_slot, dst_dtype,
+                                                        2 * (w.k1 - w.k0));
+                              },
+                              contiguous_download(ctx, L, (char*)h_dst, urh_iq_bytes(dst_dtype)));
 }

@@ -613,9 +613,50 @@ static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_sam
     return z;
 }
 
+// Message segmentation from IQ (stats.cu urh_segment_messages_iq_stream): the arena of one pass of the sharded segmenter over `tiles`
+// tiles of float64 magnitudes (urh_segment_shard_pass: tile table, staging, closing-run scan; urh_shard_candidates: carries, heads,
+// counts, the candidates, at most one per 10 samples; the scans' aggregates)
+static int64_t segment_arena_bytes(int64_t tiles) {
+    const int64_t cap = URH_TILE / 10 + 2, cand = tiles * URH_TILE / 10 + 3;
+    return r256(tiles * (int64_t)sizeof(UrhTileSummary)) + r256(tiles * cap * 4) + 2 * r256(tiles * (int64_t)sizeof(RunCarry)) +
+           2 * r256(2 * (int64_t)sizeof(RunCarry)) + r256(tiles * 4) + r256(tiles * 8) + r256(32) + r256(cand * 8) + r256(cand * 2) +
+           3 * r256((tiles + 2) * 16);
+}
+SegmentStreamSizes urh_segment_stream_sizes(int64_t n, int dtype, int64_t chunk_samples) {
+    SegmentStreamSizes z;
+    z.cs = stream_chunk_samples(n, chunk_samples);
+    z.src_slot = r256(URH_STREAM_PAD + z.cs * urh_iq_bytes(dtype));
+    z.mag_bytes = r256(z.cs * 8);
+    z.arena = segment_arena_bytes(z.cs / URH_TILE);
+    return z;
+}
+
 extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows,
                                     int64_t* bytes) {
-    if (!bytes || n < 0 || tolerance < 0 || tolerance > 0xffff || (entry & 0xf) > URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE) return URH_ERR_INVALID;
+    if (!bytes || n < 0 || tolerance < 0 || tolerance > 0xffff || (entry & 0xf) > URH_STREAM_ENTRY_ESTIMATE) return URH_ERR_INVALID;
+    const int64_t arena_block = (int64_t)64 << 20;
+    if ((entry & 0xf) == URH_STREAM_ENTRY_SEGMENT_MESSAGES) {
+        if (urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
+        if (entry & URH_STREAM_RESIDENT) {   // the capture, its float64 magnitudes, urh_segment_messages' tables over all of it
+            *bytes = r256(n * urh_iq_bytes(dtype)) + r256(n * 8) + segment_arena_bytes(urh_div_up(n, URH_TILE)) + arena_block;
+            return URH_OK;
+        }
+        if (ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
+        const SegmentStreamSizes z = urh_segment_stream_sizes(n, dtype, chunk_samples);
+        *bytes = ring * z.src_slot + z.mag_bytes + 2 * z.arena + arena_block;   // arena: twice the requests plus one block
+        return URH_OK;
+    }
+    if ((entry & 0xf) == URH_STREAM_ENTRY_ESTIMATE) {
+        // AutoInterpretation.estimate's resident path: the capture, its float64 magnitudes, and the resident demodulation of order 2
+        // (capture, qad); PSK's Costas tables make that the largest of the three modulations, so one decision up front covers them all
+        if (!(entry & URH_STREAM_RESIDENT)) return URH_ERR_INVALID;
+        if (urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
+        int64_t demod = 0;
+        URH_CHECK(urh_stream_footprint(n, dtype, 0, chunk_samples, ring, URH_STREAM_ENTRY_AFP_DEMOD | URH_STREAM_PSK | URH_STREAM_RESIDENT,
+                                       -1, &demod));
+        *bytes = r256(n * 8) + demod;
+        return URH_OK;
+    }
     if (!(entry & URH_STREAM_RESIDENT) && (ring < 2 || ring > URH_STREAM_MAX_RING)) return URH_ERR_INVALID;
     if ((entry & 0xf) != URH_STREAM_ENTRY_GRAB_PULSE_LENS && urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
     if ((entry & URH_STREAM_PSK) && (entry & 0xf) != URH_STREAM_ENTRY_AFP_DEMOD && (entry & 0xf) != URH_STREAM_ENTRY_DEMOD_DIGITIZE)

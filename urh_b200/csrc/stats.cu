@@ -4,12 +4,15 @@
 //   message segmentation      — auto_interpretation.segment_messages_from_magnitudes (auto_interpretation.pyx:55-111)
 //   plateau lengths           — auto_interpretation.get_plateau_lengths (:179-208)
 //   median filter, dB         — auto_interpretation.median_filter (:211-240), util.arr2decibel (util.pyx:38-48)
+// Host captures too large for the device: the noise level (AutoInterpretation.py:60-104) and the segmentation of estimate()
+// (AutoInterpretation.py:373-471 over auto_interpretation.pyx:55-111) also stream through the rings of stream_ring.cuh, bit-identical.
 // The small, data-dependent decision logic (which chunks are quiet, which histogram bins are local maxima)
 // stays on the host in urh_b200/ainterpretation/AutoInterpretation.py, exactly as in the reference; the
 // sample-rate reductions run here.
 #include "dense_f32.cuh"
 #include "scan.cuh"
 #include "sparse.cuh"
+#include "stream_ring.cuh"
 
 #include <math.h>
 
@@ -58,13 +61,17 @@ extern "C" int urh_get_magnitudes(urh_ctx* ctx, const void* d_iq, int dtype, int
 // Chunks are counted from the END of the array (AutoInterpretation.py:66-72): chunk j covers
 // [n - (j+1)*cs, n - j*cs).  Each block reduces a slice of one chunk to (sum, max) in double; a second kernel
 // folds the slices in a fixed order, so the result is deterministic.
+// Block b reduces slice g0 + b in sample order (urh_filter_windows' URH_FILTER_NOISE numbering: chunk nchunks - 1 - g / 64, slice
+// g % 64) into that slice's slot chunk * 64 + slice, so a streamed window of slices computes each of them as the resident launch
+// (g0 = 0, every slice) does.
 #define STAT_BLOCK 256
-#define STAT_SLICES 64
+#define STAT_SLICES URH_NOISE_SLICES
 
 template <typename LOADER>
-__global__ void __launch_bounds__(STAT_BLOCK) k_chunk_partial(LOADER ld, int64_t n, int64_t cs, int nchunks,
+__global__ void __launch_bounds__(STAT_BLOCK) k_chunk_partial(LOADER ld, int64_t n, int64_t cs, int nchunks, int64_t g0,
                                                               double* __restrict__ psum, double* __restrict__ pmax) {
-    const int chunk = blockIdx.x / STAT_SLICES, slice = blockIdx.x % STAT_SLICES;
+    const int64_t g = g0 + blockIdx.x;
+    const int chunk = nchunks - 1 - (int)(g / STAT_SLICES), slice = (int)(g % STAT_SLICES);
     const int64_t c0 = n - (int64_t)(chunk + 1) * cs;
     const int64_t per = urh_div_up(cs, STAT_SLICES);
     const int64_t s0 = c0 + (int64_t)slice * per;
@@ -87,8 +94,8 @@ __global__ void __launch_bounds__(STAT_BLOCK) k_chunk_partial(LOADER ld, int64_t
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        psum[blockIdx.x] = s_sum[0];
-        pmax[blockIdx.x] = s_max[0];
+        psum[chunk * STAT_SLICES + slice] = s_sum[0];
+        pmax[chunk * STAT_SLICES + slice] = s_max[0];
     }
 }
 
@@ -124,7 +131,8 @@ static int chunk_stats(urh_ctx* ctx, LOADER ld, int64_t n, int64_t cs, int nchun
     URH_CHECK(urh_arena(ctx, (size_t)nchunks * STAT_SLICES, &pmax));
     URH_CHECK(urh_arena(ctx, (size_t)nchunks, &sum));
     URH_CHECK(urh_arena(ctx, (size_t)nchunks, &mx));
-    URH_LAUNCH(ctx, (k_chunk_partial<LOADER>), (unsigned)(nchunks * STAT_SLICES), STAT_BLOCK, 0, ld, n, cs, nchunks, psum, pmax);
+    URH_LAUNCH(ctx, (k_chunk_partial<LOADER>), (unsigned)(nchunks * STAT_SLICES), STAT_BLOCK, 0, ld, n, cs, nchunks, (int64_t)0, psum,
+               pmax);
     URH_LAUNCH(ctx, k_chunk_final, (unsigned)urh_div_up(nchunks, 128), 128, 0, psum, pmax, nchunks, sum, mx);
     URH_CUDA(ctx, cudaMemcpyAsync(h_sum, sum, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     URH_CUDA(ctx, cudaMemcpyAsync(h_max, mx, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -137,6 +145,50 @@ extern "C" int urh_noise_chunk_stats_iq(urh_ctx* ctx, const void* d_iq, int dtyp
                                         int nchunks, double* h_sum, double* h_max) {
     if (nchunks <= 0 || chunksize <= 0 || (int64_t)nchunks * chunksize > n) URH_FAIL(ctx, URH_ERR_INVALID, "bad chunking");
     URH_DISPATCH_DT(dtype, { LoadMagIQ<DT> ld; ld.iq = d_iq; URH_CHECK(chunk_stats(ctx, ld, n, chunksize, nchunks, h_sum, h_max)); });
+    return URH_OK;
+}
+
+// The same from a host capture of any size through the windowed ring (stream_ring.cuh): each window of whole slices
+// (urh_filter_windows, URH_FILTER_NOISE) is uploaded into its slot and reduced by k_chunk_partial through a pointer shifted back by
+// the window's first sample, so every slice's partial is the resident launch's word; the head before n - nchunks * cs is never read.
+template <int DT>
+static int noise_stream(urh_ctx* ctx, const void* h_iq, int64_t n, int64_t cs, int nchunks, int64_t chunk_samples, int ring,
+                        double* h_sum, double* h_max) {
+    urh_arena_reset(ctx);   // the call takes no arena: its peak (urh_stream_stats) is 0, not a previous call's
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_NOISE, n, 0, cs, nchunks, chunk_samples, nullptr, nullptr, 0, win));
+    StreamRing R;
+    FilterRingLayout L;
+    URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_NOISE, n, 0, DT, cs, nchunks, 0, chunk_samples, L));
+    const int64_t G = (int64_t)nchunks * STAT_SLICES;
+    double* psum = (double*)L.extra;
+    double* pmax = (double*)(L.extra + r256(G * 8));
+    double* sum = (double*)(L.extra + 2 * r256(G * 8));
+    double* mx = (double*)(L.extra + 2 * r256(G * 8) + r256((int64_t)nchunks * 8));
+    const int ib = urh_iq_bytes(DT);
+    auto no_download = [](int64_t, const UrhWindow&, int, cudaStream_t) { return URH_OK; };
+    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
+                                 [&](int64_t, const UrhWindow& w, int s) {
+                                     LoadMagIQ<DT> ld;
+                                     ld.iq = L.in + s * L.z.in_slot - w.a * ib;   // sample i of the capture at ld.iq + i
+                                     URH_LAUNCH(ctx, (k_chunk_partial<LoadMagIQ<DT>>), (unsigned)(w.k1 - w.k0), STAT_BLOCK, 0, ld, n, cs,
+                                                nchunks, w.k0, psum, pmax);
+                                     return URH_OK;
+                                 },
+                                 no_download));
+    URH_LAUNCH(ctx, k_chunk_final, (unsigned)urh_div_up(nchunks, 128), 128, 0, psum, pmax, nchunks, sum, mx);
+    URH_CUDA(ctx, cudaMemcpyAsync(h_sum, sum, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync(h_max, mx, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+
+extern "C" int urh_noise_chunk_stats_iq_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, int64_t chunksize, int nchunks,
+                                               int64_t chunk_samples, int ring, double* h_sum, double* h_max) {
+    if (!h_iq || !h_sum || !h_max) URH_FAIL(ctx, URH_ERR_INVALID, "noise_chunk_stats_iq_stream: bad arguments");
+    if (nchunks <= 0 || chunksize <= 0 || (int64_t)nchunks * chunksize > n) URH_FAIL(ctx, URH_ERR_INVALID, "bad chunking");
+    URH_CHECK(urh_filter_stream_check(ctx, n, ring));
+    URH_DISPATCH_DT(dtype, URH_CHECK(noise_stream<DT>(ctx, h_iq, n, chunksize, nchunks, chunk_samples, ring, h_sum, h_max)));
     return URH_OK;
 }
 int urh_chunk_sums_f32(urh_ctx* ctx, const float* d_a, int64_t n, int64_t len, int batch, float* d_out);   // pairwise.cu
@@ -303,6 +355,68 @@ extern "C" int urh_segment_messages(urh_ctx* ctx, const void* d_mags, int is_f64
     free(pos);
     free(cl);
     return rc;
+}
+
+// segment_messages_from_magnitudes(get_magnitudes(iq)) of a host capture of any size (stream_run: chunks of whole tiles).  Each chunk's
+// float64 magnitudes go into a scratch of one chunk, the sharded segmenter's dense pass runs over them, and urh_shard_candidates gives
+// its candidates with global positions from the run that ends right before the chunk (dist.py fold_carry's rule, folded here).  The
+// two-state machine then runs once over all candidates; the segments stay in the context for urh_fetch_segments, so a caller never
+// streams the capture twice to size its buffer.
+extern "C" int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_threshold,
+                                              int64_t chunk_samples, int ring, int64_t* k) {
+    if (!h_iq || !k) URH_FAIL(ctx, URH_ERR_INVALID, "segment_messages_iq_stream: bad arguments");
+    if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
+    if (n < 0 || ring < 2 || ring > URH_STREAM_MAX_RING) URH_FAIL(ctx, URH_ERR_INVALID, "segment_messages_iq_stream: bad n or ring");
+    *k = 0;
+    ctx->segments.clear();
+    if (n == 0) return URH_OK;
+    const SegmentStreamSizes z = urh_segment_stream_sizes(n, dtype, chunk_samples);
+    StreamRing R;
+    URH_CHECK(R.init(ctx, ring, ring * z.src_slot + z.mag_bytes));
+    double* d_mag = (double*)(R.mem + ring * z.src_slot);
+    std::vector<int64_t> pos;
+    std::vector<int16_t> cls;
+    int first_above = 0;
+    bool carry_valid = false;
+    int carry_cls = 0;
+    int64_t carry_len = 0;
+    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, R.mem, z.src_slot, nullptr, nullptr,
+                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
+                             URH_CHECK(urh_get_magnitudes(ctx, R.mem + s * z.src_slot + URH_STREAM_PAD, dtype, s1 - s0, d_mag));
+                             int64_t summary[4];
+                             URH_CHECK(urh_segment_shard_pass(ctx, d_mag, 1, s1 - s0, noise_threshold, summary));
+                             if (c == 0) first_above = (int)summary[3];
+                             int64_t count = 0;
+                             URH_CHECK(urh_shard_candidates(ctx, carry_valid ? 1 : 0, carry_cls, carry_len, s0, &count, nullptr, nullptr,
+                                                            nullptr));
+                             const size_t at = pos.size();
+                             pos.resize(at + (size_t)count);
+                             cls.resize(at + (size_t)count);
+                             URH_CHECK(urh_fetch_candidates(ctx, pos.data() + at, cls.data() + at, count));
+                             // the run that ends after this chunk: this chunk's closing run, continued from the carry if the chunk is one run
+                             if (carry_valid && summary[2] && summary[0] == carry_cls) {
+                                 carry_len += summary[1];
+                             } else {
+                                 carry_cls = (int)summary[0];
+                                 carry_len = summary[1];
+                             }
+                             carry_valid = true;
+                             return URH_OK;
+                         }));
+    int64_t m = 0;
+    URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, carry_cls, carry_len, n, nullptr, 0, &m));
+    ctx->segments.resize((size_t)(2 * m));
+    URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, carry_cls, carry_len, n, ctx->segments.data(),
+                                     m, &m));
+    *k = m;
+    return URH_OK;
+}
+
+// the segments of the last urh_segment_messages_iq_stream call: (start, end) pairs
+extern "C" int urh_fetch_segments(urh_ctx* ctx, int64_t* h_segments, int64_t k) {
+    if (k < 0 || 2 * k > (int64_t)ctx->segments.size()) URH_FAIL(ctx, URH_ERR_INVALID, "fetch_segments: k exceeds the last result");
+    if (k > 0) memcpy(h_segments, ctx->segments.data(), (size_t)(2 * k) * sizeof(int64_t));
+    return URH_OK;
 }
 
 // get_plateau_lengths (auto_interpretation.pyx:179-208): h_out capacity `cap`; *k = number of plateaus.

@@ -11,6 +11,7 @@
 #include "common.cuh"
 
 #define URH_STREAM_MAX_RING 8
+#define URH_NOISE_SLICES 64   // slices per noise chunk (stats.cu STAT_SLICES)
 #define URH_STREAM_PAD 256   // slot = [pad][halo][chunk]: the chunk starts 256 bytes in, the halo sample right before it
 enum { URH_OP_UPLOAD = 0, URH_OP_COMPUTE = 1, URH_OP_DOWNLOAD = 2 };
 
@@ -94,6 +95,13 @@ static int stream_run(urh_ctx* ctx, int64_t n, int64_t cs, StreamRing& R, const 
     URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return URH_OK;
 }
+
+// the slots of urh_segment_messages_iq_stream (stats.cu): chunk samples, one IQ slot ([pad][chunk], 256-byte multiple), the float64
+// magnitude scratch of one chunk, the arena requests of one chunk's segmenter pass (urh_stream_footprint, digitize.cu)
+struct SegmentStreamSizes {
+    int64_t cs, src_slot, mag_bytes, arena;
+};
+SegmentStreamSizes urh_segment_stream_sizes(int64_t n, int dtype, int64_t chunk_samples);
 
 // ---- the windowed ring ---------------------------------------------------------------------------------------------------------------
 // A chunk c is {k0, k1, a, b} (win[4 c ..]): it owns outputs [k0, k1) and reads input samples [a, b).  Slot s holds the window from its

@@ -9,6 +9,22 @@ static int64_t frames_per_chunk(int64_t cs, int64_t hop) { return cs / hop > 0 ?
 static int64_t frames_of(int64_t len, int64_t W, int64_t hop) { return len < W ? 1 : (len - W) / hop + 1; }
 static int64_t clamp64(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
+// The noise-chunk statistics (stats.cu) reduce each of the nchunks end-aligned chunks of cs samples in URH_NOISE_SLICES slices of
+// ceil(cs / URH_NOISE_SLICES) samples.  Slice g in sample order is slice g % 64 of chunk nchunks - 1 - g / 64 (chunk j covers
+// [n - (j + 1) cs, n - j cs)); its samples, clipped to its chunk (a slice past a short chunk's end is empty):
+static void noise_slice(int64_t n, int64_t cs, int64_t nchunks, int64_t g, int64_t* s0, int64_t* s1) {
+    const int64_t j = nchunks - 1 - g / URH_NOISE_SLICES, c0 = n - (j + 1) * cs, c1 = c0 + cs;
+    const int64_t per = urh_div_up(cs, URH_NOISE_SLICES);
+    *s0 = c0 + (g % URH_NOISE_SLICES) * per < c1 ? c0 + (g % URH_NOISE_SLICES) * per : c1;
+    *s1 = *s0 + per < c1 ? *s0 + per : c1;
+}
+// samples of the largest noise window: a chunk, or one slice when a slice is longer, never more than the chunks cover
+static int64_t noise_slot_samples(int64_t cs, int64_t nchunks, int64_t chunk_samples) {
+    const int64_t per = urh_div_up(cs, URH_NOISE_SLICES);
+    const int64_t w = filter_chunk(chunk_samples) > per ? filter_chunk(chunk_samples) : per;
+    return w < cs * nchunks ? w : cs * nchunks;
+}
+
 int urh_filter_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples, const int64_t* h_seg_start,
                        const int64_t* h_seg_len, int nseg, std::vector<UrhWindow>& out) {
     out.clear();
@@ -37,8 +53,27 @@ int urh_filter_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_
             return URH_OK;
         }
         case URH_FILTER_DC:
+        case URH_FILTER_CONVERT:
             for (int64_t k0 = 0; k0 < n; k0 += cs) out.push_back({k0, k0 + cs < n ? k0 + cs : n, k0, k0 + cs < n ? k0 + cs : n});
             return URH_OK;
+        case URH_FILTER_NOISE: {   // outputs: the slices in sample order (p0 = cs, p1 = nchunks); whole slices per window
+            const int64_t ccs = p0, nchunks = p1;
+            if (ccs < 1 || nchunks < 1 || ccs * nchunks > n) return URH_ERR_INVALID;
+            const int64_t G = nchunks * URH_NOISE_SLICES;
+            for (int64_t g0 = 0; g0 < G;) {
+                int64_t a, b, s0, s1;
+                noise_slice(n, ccs, nchunks, g0, &a, &b);
+                int64_t g1 = g0 + 1;
+                for (; g1 < G; g1++) {
+                    noise_slice(n, ccs, nchunks, g1, &s0, &s1);
+                    if (s1 - a > cs) break;
+                    b = s1;
+                }
+                out.push_back({g0, g1, a, b});
+                g0 = g1;
+            }
+            return URH_OK;
+        }
         case URH_FILTER_STFT:
         case URH_FILTER_DB: {   // frame f reads x[f hop .. f hop + W - 1]
             const int64_t W = p0, hop = p1;
@@ -181,6 +216,15 @@ FilterStreamSizes urh_filter_stream_sizes(int entry, int64_t n, int64_t out_len,
             z.out_slot = r256(cs * out_bytes_dc(dtype));
             z.work = 3 * r256(4096 * 16);   // column partials of up to 4096 blocks, the sums, the mean
             break;
+        case URH_FILTER_NOISE:   // the slot of the largest window; the slices' partials and the chunks' sums and maxima
+            z.in_slot = r256(noise_slot_samples(p0, p1, chunk_samples) * urh_iq_bytes(dtype));
+            z.out_slot = 0;
+            z.extra = 2 * r256(p1 * URH_NOISE_SLICES * 8) + 2 * r256(p1 * 8);
+            break;
+        case URH_FILTER_CONVERT:
+            z.in_slot = r256(cs * urh_iq_bytes(dtype));
+            z.out_slot = r256(cs * urh_iq_bytes((int)p0));
+            break;
         case URH_FILTER_STFT:
         case URH_FILTER_DB: {
             const int64_t fpc = frames_per_chunk(cs, p1);
@@ -211,6 +255,8 @@ static bool filter_args_ok(int entry, int64_t n, int64_t out_len, int dtype, int
         case URH_FILTER_CONVOLVE: return p0 >= 1 && p1 >= 0;
         case URH_FILTER_FIR: return p0 >= 0;
         case URH_FILTER_DC: return urh_iq_bytes(dtype) != 0;
+        case URH_FILTER_NOISE: return urh_iq_bytes(dtype) != 0 && p0 >= 1 && p1 >= 1 && p0 * p1 <= n;
+        case URH_FILTER_CONVERT: return urh_iq_bytes(dtype) != 0 && urh_iq_bytes((int)p0) != 0;
         case URH_FILTER_STFT:
         case URH_FILTER_DB: return p0 > 0 && p1 > 0;
         case URH_FILTER_IMAGES: return p0 > 0 && p1 > 0 && p2 > 0;
@@ -230,6 +276,9 @@ extern "C" int urh_stream_filter_footprint(int entry, int64_t n, int64_t out_len
             case URH_FILTER_CONVOLVE: b += r256(n * 8) + r256(out_len * 8) + r256(p0 * 16); break;
             case URH_FILTER_FIR: b += 2 * r256(n * 8) + r256((p0 > 1 ? p0 : 1) * 8); break;
             case URH_FILTER_DC: b += r256(n * urh_iq_bytes(dtype)) + r256(n * out_bytes_dc(dtype)) + 3 * r256(4096 * 16); break;
+            // the capture uploaded whole, the partials and results in the arena (urh_noise_chunk_stats_iq)
+            case URH_FILTER_NOISE: b += r256(n * urh_iq_bytes(dtype)) + 2 * r256(p1 * URH_NOISE_SLICES * 8) + 2 * r256(p1 * 8); break;
+            case URH_FILTER_CONVERT: b += r256(n * urh_iq_bytes(dtype)) + r256(n * urh_iq_bytes((int)p0)); break;
             case URH_FILTER_STFT:
             case URH_FILTER_DB:
                 b += r256(n * 8) + r256(out_len * p0 * (entry == URH_FILTER_STFT ? 16 : 4)) + r256(p0 * 8) + frames_work(p0, out_len);

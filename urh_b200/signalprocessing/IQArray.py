@@ -4,6 +4,7 @@ Same constructor, properties, dtype-conversion rules (pinned by the reference's 
 file formats.  `magnitudes` runs on the GPU (util.get_magnitudes); `device()` returns / caches the capture in HBM
 so that Signal, Filter and the demodulators do not re-upload it.
 """
+import ctypes
 import os
 import tarfile
 import tempfile
@@ -184,7 +185,28 @@ class IQArray(object):
             return self.__data
         if tgt not in [np.dtype(t) for t in _INT_TYPES + (np.float32,)]:
             raise ValueError("Data type {} not supported".format(target_dtype))
+        if self._device is None and len(self.__data) and self.__data.dtype in [np.dtype(t) for t in _INT_TYPES + (np.float32,)]:
+            converted = self._convert_streamed(tgt)
+            if converted is not None:
+                return converted
         return self.convert_to_device(tgt).get()
+
+    def _convert_streamed(self, tgt):
+        """the conversion of a host capture whose resident conversion (capture and output on the device) does not fit the device
+        budget, streamed through the device into a new host array (urh_convert_iq_stream, the same elements); else None"""
+        from .. import _lib
+        from ..cythonext import signal_functions as sf
+
+        ctx = _lib.default_context()
+        n = len(self.__data)
+        if not sf.filter_use_stream(_lib.FILTER_CONVERT, n, n, self.__data.dtype, _lib.dtype_code(tgt), 0, sf.device_budget(ctx)):
+            return None
+        src = np.ascontiguousarray(self.__data)
+        out = np.empty(src.shape, dtype=tgt)
+        ctx.check(ctx.lib.urh_convert_iq_stream(ctx.handle, src.ctypes.data_as(ctypes.c_void_p), _lib.dtype_code(src.dtype),
+                                                out.ctypes.data_as(ctypes.c_void_p), _lib.dtype_code(tgt), n, sf.FILTER_STREAM_CHUNK,
+                                                sf.STREAM_RING))
+        return out
 
     def convert_to_device(self, target_dtype):
         """the converted capture as a DeviceArray (no download)"""

@@ -107,7 +107,13 @@ class Signal(object):
             self.filename = filename
             default_noise_threshold = settings.read("default_noise_threshold", "automatic")
             if default_noise_threshold == "automatic":
-                self.noise_threshold = AutoInterpretation.detect_noise_level_iq(self.iq_array.device())
+                host = self.iq_array._peek()
+                if AutoInterpretation.noise_level_streams(len(host), host.dtype,
+                                                          signal_functions.device_budget(_lib.default_context())):
+                    # the capture does not fit the device: streamed, and no device copy is kept
+                    self.noise_threshold = AutoInterpretation.detect_noise_level_iq(host)
+                else:
+                    self.noise_threshold = AutoInterpretation.detect_noise_level_iq(self.iq_array.device())
             else:
                 self.noise_threshold = float(default_noise_threshold) / 100 * self.max_magnitude
 
