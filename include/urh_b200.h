@@ -257,8 +257,9 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
                                          int64_t chunk_samples, void* d_iq_scratch, float* d_qad_out, int64_t global_offset,
                                          int64_t n_total, double* center, int* center_state, int64_t* k);
 /* ---- streaming: host captures of any size through a ring of `ring` (2..8) device slots of chunk_samples each (digitize.cu,
- * DESIGN.md §4.11).  chunk_samples <= 0: 2^24; it is rounded down to a multiple of 2048 (at least 2048).  Host buffers may be pinned
- * (urh_host_alloc: copies overlap the kernels) or pageable, e.g. a memory-mapped file (correct, but each copy then blocks the host).
+ * DESIGN.md §4.11), in the chunks of urh_stream_windows with URH_FILTER_TILES.  chunk_samples <= 0: 2^24; it is rounded down to a
+ * multiple of 2048 (at least 2048).  Host buffers may be pinned (urh_host_alloc: copies overlap the kernels) or pageable, e.g. a
+ * memory-mapped file (correct, but each copy then blocks the host).
  * Results are bit-identical to the resident entry points named below.  ASK / FSK only; PSK raises URH_ERR_INVALID (PSK has entry
  * points of its own, below).
  * urh_afp_demod_stream: afp_demod (signal_functions.pyx:333-378) from host IQ into host qad h_qad[n].
@@ -280,9 +281,6 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
  *   URH_STREAM_PSK for a Costas loop of order 2 (also a bound for orders 1 and 3, which run the serial kernel), with
  *   URH_STREAM_PSK4 for order 4 or more.  rows: the pulse-table rows to budget for
  *   (-1: the bound n / (tolerance + 1) + 3 that no capture exceeds; -2: the n / 64 + 1024 rows the resident call reserves up front).
- * urh_stream_schedule: the order in which a call issues its copies and chunk computations, 6 int64 per op {kind (0 upload into
- *   the slot, 1 compute, 2 download from the slot), chunk, slot, first sample, end sample, 1 if the upload carries the halo sample
- *   first - 1}; host only.  flags: URH_STREAM_UPLOAD / DOWNLOAD / HALO.
  * urh_stream_stats: {lowest free device memory seen inside the last streamed call (after each chunk and each chunk's finish and
  *   while the pulse table grows; sampled only with urh_set_profiling on, else -1), chunks of its ring pass, the most bytes of
  *   scratch-arena requests live at once during it}.
@@ -298,7 +296,6 @@ int urh_shard_demod_center_digitize_host(urh_ctx* ctx, const void* h_iq, int dty
 #define URH_STREAM_PSK4 0x100         /* with URH_STREAM_PSK: Costas loop of order 4 */
 #define URH_STREAM_UPLOAD 1
 #define URH_STREAM_DOWNLOAD 2
-#define URH_STREAM_HALO 4
 int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, int64_t chunk_samples,
                          int ring, float* h_qad);
 int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qad_on_device, int64_t n, float center, uint16_t tolerance,
@@ -320,7 +317,7 @@ int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int
  * urh_noise_chunk_stats_iq_stream: urh_noise_chunk_stats_iq through the windowed ring; each window uploads whole slices of the noise
  *   chunks (urh_stream_windows with URH_FILTER_NOISE, p0 = chunksize, p1 = nchunks), the head before n - nchunks * chunksize is not read.
  * urh_segment_messages_iq_stream: urh_segment_messages over urh_get_magnitudes (float64) of the capture, chunk by chunk (chunks of whole
- *   tiles as urh_stream_schedule cuts them); *k = number of messages, fetched with urh_fetch_segments ((start, end) int64 pairs).
+ *   tiles, URH_FILTER_TILES); *k = number of messages, fetched with urh_fetch_segments ((start, end) int64 pairs).
  * urh_convert_iq_stream: urh_convert_iq of n samples (2 n elements) from host h_src into host h_dst through the windowed ring
  *   (URH_FILTER_CONVERT, p0 = dst_dtype).
  * Footprints: URH_FILTER_NOISE / URH_FILTER_CONVERT in urh_stream_filter_footprint, URH_STREAM_ENTRY_SEGMENT_MESSAGES in
@@ -337,7 +334,6 @@ int urh_fetch_segments(urh_ctx* ctx, int64_t* h_segments, int64_t k);
 int urh_convert_iq_stream(urh_ctx* ctx, const void* h_src, int src_dtype, void* h_dst, int dst_dtype, int64_t n, int64_t chunk_samples,
                           int ring);
 int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows, int64_t* bytes);
-int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);
 int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3);
 int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
 /* ---- streaming the filters and the spectrogram: the windowed ring (stream_window.cu, filter.cu, spectrogram.cu; DESIGN.md §4.11).
@@ -358,9 +354,11 @@ int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
  *   164-190) into host h_out; whole segments are grouped per chunk, a segment longer than a chunk is rendered in runs of frames.
  * urh_stream_windows: the chunks {k0, k1, a, b} (4 int64 each) of an entry URH_FILTER_*; host only.  Outputs: CONVOLVE samples of
  *   out_len (p0 = m, p1 = offset), FIR samples of n (p0 = m), DC rows of n, STFT / DB frames of out_len (p0 = W, p1 = hop), IMAGES the
- *   frames of all segments in order (p0 = W, p1 = hop, the segments; out_len unused).
- * urh_stream_window_schedule: the op order of the windowed ring, 7 int64 per op {kind, chunk, slot, k0, k1, a, b}, kinds and
- *   semantics as urh_stream_schedule; h_win: the chunks of urh_stream_windows.  flags: URH_STREAM_UPLOAD / DOWNLOAD; host only.
+ *   frames of all segments in order (p0 = W, p1 = hop, the segments; out_len unused), TILES samples of n in chunks of whole tiles
+ *   (p0 = 1: every later chunk also reads the sample before it, the FSK halo; p0 = 0: no halo).
+ * urh_stream_window_schedule: the order in which a streamed call issues its copies and chunk computations, 7 int64 per op {kind (0
+ *   upload of [a, b) into the slot, 1 compute, 2 download of the outputs), chunk, slot, k0, k1, a, b}; h_win: the chunks of
+ *   urh_stream_windows.  flags: URH_STREAM_UPLOAD / DOWNLOAD; host only.
  * urh_stream_filter_footprint: device bytes of the streamed entry (resident = 0) or of the resident entry fed from the host (resident
  *   != 0), without a device.  Parameters as urh_stream_windows; out_len is the output count for CONVOLVE, the frames for STFT / DB and
  *   the frames of all segments for IMAGES; p2 is the colormap's entry count for IMAGES (at least 1) and 0 otherwise; dtype matters for
@@ -376,6 +374,7 @@ int urh_mem_get_info(urh_ctx* ctx, size_t* free_bytes, size_t* total_bytes);
 #define URH_FILTER_IMAGES 5
 #define URH_FILTER_NOISE 6    /* urh_noise_chunk_stats_iq_stream (below) */
 #define URH_FILTER_CONVERT 7  /* urh_convert_iq_stream (below) */
+#define URH_FILTER_TILES 8    /* the demodulation and segmentation entries (above) */
 int urh_convolve_c128_stream(urh_ctx* ctx, const float* h_x, int64_t n, const double* h_taps, int m, int64_t offset, int64_t out_len,
                              int64_t chunk_samples, int ring, float* h_y);
 int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, const float* h_taps, int m, int64_t chunk_samples, int ring, float* h_y);

@@ -347,6 +347,6 @@ def test_device_memory_within_footprint(ctx):
 def test_arena_peak_independent_of_n(ctx):
     chunk = 1 << 18
     peaks = []
-    for n in (1 << 22, 1 << 24):   # whole chunks: the last chunk's segmenter pass is a full one in both
+    for n in (1 << 22, 1 << 24):   # the segmentation's peak is its largest chunk's: one full chunk's segmenter pass in both
         peaks.append([(call(), _stream_stats(ctx)[2])[1] for _, call in _runs(ctx, n, chunk)])
     assert peaks[0] == peaks[1], peaks

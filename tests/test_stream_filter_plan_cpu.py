@@ -3,7 +3,10 @@ choice) for the streamed band-pass, FIR and DC filters and the spectrogram, with
 
 Each chunk owns the outputs [k0, k1) and uploads the input window [a, b).  Checked here: the chunks cover every output once, each window
 is exactly the samples its outputs read, the windows equal the sharded plans of urh_b200/dist.py where the cut is a valid shard cut, and
-no slot is rewritten before its readers on a host model of the schedule's stream/event semantics."""
+no slot is rewritten before its readers on a host model of the schedule's stream/event semantics (stream_window.cu): uploads run on
+copy stream 0, chunk computations on the compute stream, downloads on copy stream 1, and every wait resolves to the last record of its
+event issued before it, as cudaStreamWaitEvent does.  The model also takes the tile chunks of the demodulation entries
+(URH_FILTER_TILES; their own plan is checked in tests/test_stream_plan_cpu.py)."""
 import ctypes as C
 
 import numpy as np
@@ -45,6 +48,7 @@ def shard_bounds_of(w):
 
 
 CS = 1000
+TILE = 2048
 
 
 @pytest.mark.parametrize("n", [1, CS - 1, CS, CS + 1, 3 * CS - 1, 3 * CS, 3 * CS + 1, 7 * CS + 13])
@@ -233,10 +237,15 @@ def _happens_before(ops, up, down):
 
 @pytest.mark.parametrize("ring", [2, 3, 4])
 @pytest.mark.parametrize("chunks", [1, 2, 3, 4, 5, 9])
-@pytest.mark.parametrize("up,down", [(True, True), (True, False)])
-def test_no_slot_overwritten_before_its_readers(L, ring, chunks, up, down):
-    n, m = chunks * CS - 7, 301
-    win = windows(L, L.FILTER_CONVOLVE, n, n, m, (m - 1) // 2, CS)
+@pytest.mark.parametrize("up,down,plan", [(True, True, "convolve"), (True, False, "convolve"), (True, True, "tiles"), (True, False, "tiles")],
+                         ids=["True-True", "True-False", "tiles-True-True", "tiles-True-False"])
+def test_no_slot_overwritten_before_its_readers(L, ring, chunks, up, down, plan):
+    if plan == "tiles":   # whole tiles, every later chunk with the sample before it (its halo is part of its own upload)
+        n = chunks * 3 * TILE - 5
+        win = windows(L, L.FILTER_TILES, n, n, 1, 0, 3 * TILE)
+    else:
+        n, m = chunks * CS - 7, 301
+        win = windows(L, L.FILTER_CONVOLVE, n, n, m, (m - 1) // 2, CS)
     assert len(win) == chunks
     flags = (L.STREAM_UPLOAD if up else 0) | (L.STREAM_DOWNLOAD if down else 0)
     ops = schedule(L, win, ring, flags)

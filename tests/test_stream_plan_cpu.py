@@ -1,8 +1,8 @@
-"""CPU: the plan of a streamed call (urh_stream_schedule, urh_stream_footprint, the shims' path choice) without a device.
+"""CPU: the plan of a streamed demodulation call (the tile chunks of urh_stream_windows with URH_FILTER_TILES in the order of
+urh_stream_window_schedule, urh_stream_footprint, the shims' path choice) without a device.
 
-The schedule is checked on a host model of its stream/event semantics (include/urh_b200.h, digitize.cu): uploads run on copy
-stream 0, chunk computations on the compute stream, qad downloads on copy stream 1, and every wait resolves to the last record of
-its event issued before it, as cudaStreamWaitEvent does."""
+That no slot is rewritten before its readers is checked, for these chunks as for the windowed entries', on the host model of the
+schedule in tests/test_stream_filter_plan_cpu.py."""
 import ctypes as C
 
 import numpy as np
@@ -19,12 +19,25 @@ def L():
     return _lib
 
 
-def schedule(L, n, cs, ring, flags):
+def tile_windows(L, n, cs, halo):
     lib = L.load_library()
     count = C.c_int64(0)
-    assert lib.urh_stream_schedule(n, cs, ring, flags, None, 0, C.byref(count)) == 0
-    ops = np.zeros((max(count.value, 1), 6), np.int64)
-    assert lib.urh_stream_schedule(n, cs, ring, flags, ops.ctypes.data_as(C.c_void_p), count.value, C.byref(count)) == 0
+    args = (L.FILTER_TILES, n, n, halo, 0, cs, None, None, 0)
+    assert lib.urh_stream_windows(*args, None, 0, C.byref(count)) == 0
+    win = np.zeros((max(count.value, 1), 4), np.int64)
+    assert lib.urh_stream_windows(*args, win.ctypes.data_as(C.c_void_p), count.value, C.byref(count)) == 0
+    return win[: count.value]
+
+
+def schedule(L, n, cs, ring, flags, halo):
+    """ops {kind, chunk, slot, k0, k1, a, b} of the tile chunks"""
+    lib = L.load_library()
+    win = tile_windows(L, n, cs, halo)
+    count = C.c_int64(0)
+    assert lib.urh_stream_window_schedule(win.ctypes.data_as(C.c_void_p), len(win), ring, flags, None, 0, C.byref(count)) == 0
+    ops = np.zeros((max(count.value, 1), 7), np.int64)
+    assert lib.urh_stream_window_schedule(win.ctypes.data_as(C.c_void_p), len(win), ring, flags, ops.ctypes.data_as(C.c_void_p),
+                                          count.value, C.byref(count)) == 0
     return ops[: count.value]
 
 
@@ -36,8 +49,8 @@ def footprint(L, n, dtype, tol, cs, ring, entry, rows=-1):
 
 @pytest.mark.parametrize("n", [1, 3, TILE - 1, TILE, TILE + 1, 5 * TILE, 7 * TILE + 3, 1_000_003])
 @pytest.mark.parametrize("cs", [0, 1, TILE, 3 * TILE, 5 * TILE + 17, 1 << 18])
-def test_chunks_cover_once_tile_aligned(L, n, cs):
-    ops = schedule(L, n, cs, 2, L.STREAM_UPLOAD | L.STREAM_HALO)
+def test_tile_windows_cover_once_tile_aligned(L, n, cs):
+    ops = schedule(L, n, cs, 2, L.STREAM_UPLOAD, 1)
     comp = ops[ops[:, 0] == 1]
     assert list(comp[:, 1]) == list(range(len(comp)))
     assert comp[0, 3] == 0 and comp[-1, 4] == n
@@ -48,70 +61,18 @@ def test_chunks_cover_once_tile_aligned(L, n, cs):
     assert comp[0, 4] - comp[0, 3] == min(eff, n)
     up = ops[ops[:, 0] == 0]
     assert sorted(up[:, 1]) == list(range(len(comp)))                      # every chunk uploaded once
-    assert (up[:, 5] == (up[:, 1] > 0)).all()                              # the halo (sample first - 1) comes with every later chunk
-    no_halo = schedule(L, n, cs, 2, L.STREAM_UPLOAD)
-    assert (no_halo[:, 5] == 0).all()
+    assert (up[:, 3] - up[:, 5] == (up[:, 1] > 0)).all()                   # the halo (sample k0 - 1) comes with every later chunk
+    assert (ops[:, 6] == ops[:, 4]).all()                                  # and nothing past the chunk's end
+    no_halo = schedule(L, n, cs, 2, L.STREAM_UPLOAD, 0)
+    assert (no_halo[:, 3] == no_halo[:, 5]).all()
 
 
-def _happens_before(L, ops, ring, up, down):
-    """edges of the model: program order per stream, and event waits resolved to the last record issued before the wait"""
-    stream_of = {0: "copy0", 1: "compute", 2: "copy1"}
-    last_on_stream, last_record = {}, {}
-    edges = {i: set() for i in range(len(ops))}
-    for i, (kind, c, s, *_rest) in enumerate(ops):
-        st = stream_of[kind]
-        if st in last_on_stream:
-            edges[i].add(last_on_stream[st])
-        waits = {0: [1], 1: ([0] if up else []) + ([2] if down else []), 2: [1]}[kind]
-        for w in waits:
-            if (w, s) in last_record:
-                edges[i].add(last_record[(w, s)])
-        last_on_stream[st] = i
-        last_record[(kind, s)] = i
-    memo = {}
-
-    def before(i):
-        if i not in memo:
-            acc = set()
-            for j in edges[i]:
-                acc.add(j)
-                acc |= before(j)
-            memo[i] = acc
-        return memo[i]
-
-    return before
-
-
-@pytest.mark.parametrize("ring", [2, 3, 4])
-@pytest.mark.parametrize("chunks", [1, 2, 3, 4, 5, 9])
-@pytest.mark.parametrize("down", [False, True])
-def test_no_slot_overwritten_before_its_readers(L, ring, chunks, down):
-    n = chunks * 3 * TILE - 5
-    flags = L.STREAM_UPLOAD | L.STREAM_HALO | (L.STREAM_DOWNLOAD if down else 0)
-    ops = schedule(L, n, 3 * TILE, ring, flags)
-    before = _happens_before(L, ops, ring, True, down)
-    idx = {(int(k), int(c)): i for i, (k, c, *_r) in enumerate(ops)}
-    assert len(idx) == len(ops)
-    for c in range(chunks):
-        assert ops[idx[(1, c)]][2] == c % ring
-        # the computation reads the upload of its own chunk
-        assert idx[(0, c)] in before(idx[(1, c)])
-        last_upload = max(i for i, o in enumerate(ops[: idx[(1, c)]]) if o[0] == 0 and o[2] == c % ring)
-        assert ops[last_upload][1] == c
-        # an upload into a slot waits for every computation that read the slot before (its halo is part of its own upload)
-        for c2 in range(c % ring, c, ring):
-            assert idx[(1, c2)] in before(idx[(0, c)])
-        if down:
-            assert idx[(1, c)] in before(idx[(2, c)])                      # qad leaves after it was written
-            for c2 in range(c % ring, c, ring):                            # and the qad slot is free again before it is rewritten
-                assert idx[(2, c2)] in before(idx[(1, c)])
-
-
-def test_schedule_rejects_bad_rings(L):
+def test_tile_schedule_rejects_bad_rings(L):
     lib = L.load_library()
     count = C.c_int64(0)
+    win = tile_windows(L, 100, TILE, 1)
     for ring in (0, 1, 9):
-        assert lib.urh_stream_schedule(100, TILE, ring, 1, None, 0, C.byref(count)) != 0
+        assert lib.urh_stream_window_schedule(win.ctypes.data_as(C.c_void_p), len(win), ring, 1, None, 0, C.byref(count)) != 0
 
 
 @pytest.mark.parametrize("tol", [0, 5, 100])

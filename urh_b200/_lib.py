@@ -23,9 +23,9 @@ STREAM_AFP_DEMOD, STREAM_GRAB_PULSE_LENS, STREAM_DEMOD_DIGITIZE, STREAM_DEMOD_CE
 STREAM_SEGMENT_MESSAGES, STREAM_ESTIMATE = 4, 5
 STREAM_QAD_OUT, STREAM_RESIDENT, STREAM_QAD_ON_DEVICE = 0x10, 0x20, 0x40
 STREAM_PSK, STREAM_PSK4 = 0x80, 0x100
-STREAM_UPLOAD, STREAM_DOWNLOAD, STREAM_HALO = 1, 2, 4
+STREAM_UPLOAD, STREAM_DOWNLOAD = 1, 2
 FILTER_CONVOLVE, FILTER_FIR, FILTER_DC, FILTER_STFT, FILTER_DB, FILTER_IMAGES = 0, 1, 2, 3, 4, 5
-FILTER_NOISE, FILTER_CONVERT = 6, 7
+FILTER_NOISE, FILTER_CONVERT, FILTER_TILES = 6, 7, 8
 
 _DTYPE_CODE = {
     np.dtype(np.int8): DT_I8,
@@ -176,7 +176,6 @@ SIGNATURES = {
     "urh_fetch_segments": (i32, [vp, vp, i64]),
     "urh_convert_iq_stream": (i32, [vp, vp, i32, vp, i32, i64, i64, i32]),
     "urh_stream_footprint": (i32, [i64, i32, i32, i64, i32, i32, i64, C.POINTER(i64)]),
-    "urh_stream_schedule": (i32, [i64, i64, i32, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_stats": (i32, [vp, vp]),
     "urh_mem_get_info": (i32, [vp, C.POINTER(szt), C.POINTER(szt)]),
     "urh_convolve_c128_stream": (i32, [vp, vp, i64, vp, i32, i64, i64, i64, i32, vp]),

@@ -89,10 +89,10 @@ extern "C" int urh_convert_iq_stream(urh_ctx* ctx, const void* h_src, int src_dt
     StreamRing R;
     FilterRingLayout L;
     URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_CONVERT, n, n, src_dtype, dst_dtype, 0, 0, chunk_samples, L));
-    return stream_run_windows(ctx, win, R, (const char*)h_src, urh_iq_bytes(src_dtype), L.in, L.z.in_slot, true,
-                              [&](int64_t, const UrhWindow& w, int s) {
-                                  return urh_convert_iq(ctx, L.in + s * L.z.in_slot, src_dtype, L.out + s * L.z.out_slot, dst_dtype,
-                                                        2 * (w.k1 - w.k0));
-                              },
-                              contiguous_download(ctx, L, (char*)h_dst, urh_iq_bytes(dst_dtype)));
+    return stream_run(ctx, win, R, (const char*)h_src, urh_iq_bytes(src_dtype), L.in, L.z.in_slot, true,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          return urh_convert_iq(ctx, L.in + s * L.z.in_slot, src_dtype, L.out + s * L.z.out_slot, dst_dtype,
+                                                2 * (w.k1 - w.k0));
+                      },
+                      contiguous_download(ctx, L.out, L.z.out_slot, (char*)h_dst, urh_iq_bytes(dst_dtype)));
 }

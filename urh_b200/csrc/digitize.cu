@@ -507,53 +507,15 @@ extern "C" int urh_demod_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int
 }
 
 // ---- streaming through a ring of device slots (DESIGN.md §4.11) -----------------------------------------------------------------
-// A chunk is a whole number of tiles (the last one excepted), so every tile has the bounds and the arithmetic it has in the resident
-// call.  IQ kernels see the slot through a pointer shifted back by the chunk's first sample: they index the capture globally, their
-// tile range is the chunk's, and the halo sample (uploaded with the chunk) sits where the resident buffer holds it.
+// A chunk is a whole number of tiles (the last one excepted; URH_FILTER_TILES), so every tile has the bounds and the arithmetic it
+// has in the resident call.  IQ kernels see the slot through a pointer shifted back by the chunk's first sample: they index the capture
+// globally, their tile range is the chunk's, and the halo sample (uploaded with the chunk) sits where the resident buffer holds it.
 int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
                      int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
                      int64_t rows_cap, int64_t* k);   // finish.cu
 
-static int64_t stream_chunk_samples(int64_t n, int64_t cs) {
-    if (cs <= 0) cs = (int64_t)1 << 24;
-    cs -= cs % URH_TILE;
-    if (cs < URH_TILE) cs = URH_TILE;
-    const int64_t whole = urh_div_up(n > 0 ? n : 1, URH_TILE) * URH_TILE;   // a capture shorter than a chunk: one slot of its size
-    return cs < whole ? cs : whole;
-}
 // rows one digitizer pass over n samples can produce: firings are >= tol + 1 samples apart, plus the head and the tail row
 static int64_t rows_bound(int64_t n, int tol) { return n / (tol + 1) + 3; }
-
-// Op semantics (the driver below and tests/test_stream_plan_cpu.py's model):
-//   upload(c, s)   copy stream 0: waits for the last compute recorded on slot s, copies, records "uploaded" on s
-//   compute(c, s)  compute stream: waits for "uploaded" on s (uploading calls) and for the last download recorded on s (downloading
-//                  calls), runs the chunk, records "computed" on s
-//   download(c, s) copy stream 1: waits for "computed" on s, copies qad out, records "downloaded" on s
-// Uploads run R - 1 chunks ahead: the upload of chunk c + R - 1 is issued before compute(c), into the slot compute(c - 1) released.
-extern "C" int urh_stream_schedule(int64_t n, int64_t chunk_samples, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count) {
-    if (!count || n < 0 || ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
-    const int64_t cs = stream_chunk_samples(n, chunk_samples);
-    const int64_t chunks = urh_div_up(n, cs);
-    const bool up = flags & URH_STREAM_UPLOAD, down = flags & URH_STREAM_DOWNLOAD, halo = flags & URH_STREAM_HALO;
-    int64_t k = 0;
-    auto emit = [&](int64_t kind, int64_t c) {
-        if (h_ops && k < cap) {
-            int64_t* o = h_ops + 6 * k;
-            o[0] = kind; o[1] = c; o[2] = c % ring; o[3] = c * cs; o[4] = (c + 1) * cs < n ? (c + 1) * cs : n;
-            o[5] = (kind == URH_OP_UPLOAD && halo && c > 0) ? 1 : 0;
-        }
-        k++;
-    };
-    if (up)
-        for (int64_t c = 0; c < ring - 1 && c < chunks; c++) emit(URH_OP_UPLOAD, c);
-    for (int64_t c = 0; c < chunks; c++) {
-        if (up && c + ring - 1 < chunks) emit(URH_OP_UPLOAD, c + ring - 1);
-        emit(URH_OP_COMPUTE, c);
-        if (down) emit(URH_OP_DOWNLOAD, c);
-    }
-    *count = k;
-    return (h_ops && k > cap) ? URH_ERR_INVALID : URH_OK;
-}
 
 // Device bytes of the ring (one cudaMallocAsync block) and of the arena requests of a call; the one place these sizes live.
 struct StreamSizes {
@@ -634,16 +596,15 @@ SegmentStreamSizes urh_segment_stream_sizes(int64_t n, int dtype, int64_t chunk_
 extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t chunk_samples, int ring, int entry, int64_t rows,
                                     int64_t* bytes) {
     if (!bytes || n < 0 || tolerance < 0 || tolerance > 0xffff || (entry & 0xf) > URH_STREAM_ENTRY_ESTIMATE) return URH_ERR_INVALID;
-    const int64_t arena_block = (int64_t)64 << 20;
     if ((entry & 0xf) == URH_STREAM_ENTRY_SEGMENT_MESSAGES) {
         if (urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
         if (entry & URH_STREAM_RESIDENT) {   // the capture, its float64 magnitudes, urh_segment_messages' tables over all of it
-            *bytes = r256(n * urh_iq_bytes(dtype)) + r256(n * 8) + segment_arena_bytes(urh_div_up(n, URH_TILE)) + arena_block;
+            *bytes = r256(n * urh_iq_bytes(dtype)) + r256(n * 8) + segment_arena_bytes(urh_div_up(n, URH_TILE)) + URH_ARENA_BLOCK;
             return URH_OK;
         }
         if (ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
         const SegmentStreamSizes z = urh_segment_stream_sizes(n, dtype, chunk_samples);
-        *bytes = ring * z.src_slot + z.mag_bytes + 2 * z.arena + arena_block;   // arena: twice the requests plus one block
+        *bytes = ring * z.src_slot + z.mag_bytes + stream_arena_bytes(z.arena);
         return URH_OK;
     }
     if ((entry & 0xf) == URH_STREAM_ENTRY_ESTIMATE) {
@@ -668,7 +629,7 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
     if (entry & URH_STREAM_RESIDENT) {
         // capture + qad, full-size digitizer tables, the pulse table as urh_ensure_pulses sizes it (1.25 x rows)
         const int64_t ntiles = urh_div_up(n, URH_TILE);
-        int64_t b = z.ring_bytes + ((int64_t)64 << 20);
+        int64_t b = z.ring_bytes + URH_ARENA_BLOCK;
         if (digitize)
             b += r256(ntiles * (int64_t)sizeof(UrhTileSummary)) + r256(ntiles * (int64_t)stage_cap_for(tolerance) * 4) +
                  finish_arena_bytes(ntiles, r + r / 4, true) + 16 * (r + r / 4);
@@ -679,10 +640,7 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
         *bytes = b;
         return URH_OK;
     }
-    int64_t b = z.ring_bytes;
-    // the arena grows in blocks of at least 64 MiB; a request that does not fit the current block's rest opens a new one, so new
-    // blocks hold at most twice the requests plus one block
-    b += 2 * z.arena + ((int64_t)64 << 20);
+    int64_t b = z.ring_bytes + stream_arena_bytes(z.arena);
     // look-back scan workspace (context.cu urhts::prepare): at least 8192 blocks, 256+ items each
     const int64_t nb = 2 * (z.scan_items / 256 + 1);
     b += 256 + (nb > 8192 ? nb : 8192) * (4 + 2 * 32);
@@ -889,11 +847,19 @@ static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype,
         scs = z.cs;
         URH_CHECK(ring.init(ctx, sc->ring, sc->ring * r256(z.src_slot)));
         const int64_t slot = r256(z.src_slot);
-        URH_CHECK(stream_run(ctx, n, scs, ring, (const char*)sc->h_iq, urh_iq_bytes(dtype), true, ring.mem, slot, sc->h_qad, d_qad_out,
-                             [&](int64_t, int64_t s0, int64_t s1, int s) {
-                                 return stream_dense_iq<false>(ctx, dtype, mod_type, ring.mem, slot, n, dp, d_qad_out, cls, 0, nullptr, s0, s1, s,
-                                                               ts, fine);
-                             }, true));
+        std::vector<UrhWindow> win;
+        URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, sc->chunk_samples, nullptr, nullptr, 0, win));
+        URH_CHECK(stream_run(ctx, win, ring, (const char*)sc->h_iq, urh_iq_bytes(dtype), ring.mem, slot, sc->h_qad != nullptr,
+                             [&](int64_t, const UrhWindow& w, int s) {
+                                 return stream_dense_iq<false>(ctx, dtype, mod_type, ring.mem, slot, n, dp, d_qad_out, cls, 0, nullptr, w.k0, w.k1,
+                                                               s, ts, fine);
+                             },
+                             [&](int64_t, const UrhWindow& w, int, cudaStream_t cp) {   // from the resident qad
+                                 URH_CUDA(ctx, cudaMemcpyAsync(sc->h_qad + w.k0, d_qad_out + w.k0, (size_t)(w.k1 - w.k0) * sizeof(float),
+                                                               cudaMemcpyDeviceToHost, cp));
+                                 return URH_OK;
+                             },
+                             place_after_pad, true));
     }
     // the digitizer's tables, filled by the qad digitizer after the center chain, and by the speculative pass before it
     cls.noise_value = urh_noise_value(mod_type);
@@ -1071,11 +1037,14 @@ extern "C" int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, i
     const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
     UrhClassify cls;
     memset(&cls, 0, sizeof(cls));
-    return stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), true, d_src, r256(z.src_slot), h_qad, d_qad,
-                      [&](int64_t, int64_t s0, int64_t s1, int s) {
-                          return stream_dense_iq<false>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp, d_qad + s * z.cs - s0, cls, 0,
-                                                        nullptr, s0, s1, s);
-                      });
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, chunk_samples, nullptr, nullptr, 0, win));
+    return stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, r256(z.src_slot), true,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          return stream_dense_iq<false>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp, d_qad + s * z.cs - w.k0, cls, 0,
+                                                        nullptr, w.k0, w.k1, s);
+                      },
+                      contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad, 4), place_after_pad);
 }
 
 extern "C" int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qad_on_device, int64_t n, float center, uint16_t tolerance,
@@ -1095,12 +1064,15 @@ extern "C" int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qa
     StreamDigitizer dz;
     URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
     char* d_src = R.mem;
-    URH_CHECK(stream_run(ctx, n, z.cs, R, qad_on_device ? nullptr : (const char*)qad, 4, false, d_src, r256(z.src_slot), nullptr, nullptr,
-                         [&](int64_t, int64_t s0, int64_t s1, int s) {
-                             const float* x = qad_on_device ? qad + s0 : (const float*)(d_src + s * r256(z.src_slot) + URH_STREAM_PAD);
-                             URH_CHECK(stream_dense_qad(ctx, x, s0, s1, cls, dz));
-                             return dz.finish(ctx, s0, s1);
-                         }));
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
+    URH_CHECK(stream_run(ctx, win, R, qad_on_device ? nullptr : (const char*)qad, 4, d_src, r256(z.src_slot), false,
+                         [&](int64_t, const UrhWindow& w, int s) {
+                             const float* x = qad_on_device ? qad + w.k0 : (const float*)(d_src + s * r256(z.src_slot) + URH_STREAM_PAD);
+                             URH_CHECK(stream_dense_qad(ctx, x, w.k0, w.k1, cls, dz));
+                             return dz.finish(ctx, w.k0, w.k1);
+                         },
+                         no_download, place_after_pad));
     *k = dz.rows;
     return URH_OK;
 }
@@ -1124,12 +1096,15 @@ extern "C" int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dty
     URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
     char* d_src = R.mem;
     float* d_qad = h_qad_out ? (float*)(R.mem + ring * r256(z.src_slot)) : nullptr;
-    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), true, d_src, r256(z.src_slot), h_qad_out, d_qad,
-                         [&](int64_t, int64_t s0, int64_t s1, int s) {
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, chunk_samples, nullptr, nullptr, 0, win));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, r256(z.src_slot), h_qad_out != nullptr,
+                         [&](int64_t, const UrhWindow& w, int s) {
                              URH_CHECK(stream_dense_iq<true>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp,
-                                                             d_qad ? d_qad + s * z.cs - s0 : nullptr, cls, tolerance, &dz, s0, s1, s));
-                             return dz.finish(ctx, s0, s1);
-                         }));
+                                                             d_qad ? d_qad + s * z.cs - w.k0 : nullptr, cls, tolerance, &dz, w.k0, w.k1, s));
+                             return dz.finish(ctx, w.k0, w.k1);
+                         },
+                         contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad_out, 4), place_after_pad));
     *k = dz.rows;
     return URH_OK;
 }
@@ -1162,12 +1137,15 @@ extern "C" int urh_afp_demod_psk_stream(urh_ctx* ctx, const void* h_iq, int dtyp
     UrhCostasStream cs;
     URH_CHECK(urh_costas_stream_begin(ctx, &cs));
     const UrhArenaMark mark = urh_arena_mark(ctx);
-    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, d_src, slot, h_qad, d_qad,
-                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, slot, true,
+                         [&](int64_t c, const UrhWindow& w, int s) {
                              urh_arena_release(ctx, mark);
-                             return urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, s1 - s0, dp.noise_sqrd,
+                             return urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, w.k1 - w.k0, dp.noise_sqrd,
                                                             mod_order, costas_loop_bandwidth, d_qad + s * z.cs);
-                         }));
+                         },
+                         contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad, 4), place_after_pad));
     return urh_costas_stream_end(ctx, &cs);
 }
 
@@ -1194,15 +1172,18 @@ extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int
     URH_CHECK(urh_costas_stream_begin(ctx, &cs));
     StreamDigitizer dz;
     URH_CHECK(dz.init(ctx, n, z.cs, tolerance, false, samples_per_symbol));
-    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, d_src, slot, h_qad_out, d_qad,
-                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, slot, h_qad_out != nullptr,
+                         [&](int64_t c, const UrhWindow& w, int s) {
                              urh_arena_release(ctx, dz.mark);
                              float* q = d_qad + s * z.cs;
-                             URH_CHECK(urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, s1 - s0, dp.noise_sqrd,
+                             URH_CHECK(urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, w.k1 - w.k0, dp.noise_sqrd,
                                                                mod_order, 0.1f, q));
-                             URH_CHECK(stream_dense_qad(ctx, q, s0, s1, cls, dz));
-                             return dz.finish(ctx, s0, s1);
-                         }));
+                             URH_CHECK(stream_dense_qad(ctx, q, w.k0, w.k1, cls, dz));
+                             return dz.finish(ctx, w.k0, w.k1);
+                         },
+                         contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad_out, 4), place_after_pad));
     *k = dz.rows;
     return urh_costas_stream_end(ctx, &cs);
 }

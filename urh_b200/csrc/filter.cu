@@ -502,12 +502,12 @@ extern "C" int urh_convolve_c128_stream(urh_ctx* ctx, const float* h_x, int64_t 
     URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_CONVOLVE, n, out_len, URH_DT_F32, m, offset, 0, chunk_samples, L));
     const double* d_taps = (const double*)L.extra;
     URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_taps, (size_t)m * 16, cudaMemcpyHostToDevice, ctx->stream));
-    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
-                              [&](int64_t, const UrhWindow& w, int s) {
-                                  return urh_convolve_c128(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, d_taps, m,
-                                                           w.k0 + offset - w.a, w.k1 - w.k0, (float*)(L.out + s * L.z.out_slot));
-                              },
-                              contiguous_download(ctx, L, (char*)h_y, 8));
+    return stream_run(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          return urh_convolve_c128(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, d_taps, m,
+                                                   w.k0 + offset - w.a, w.k1 - w.k0, (float*)(L.out + s * L.z.out_slot));
+                      },
+                      contiguous_download(ctx, L.out, L.z.out_slot, (char*)h_y, 8));
 }
 
 extern "C" int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, const float* h_taps, int m, int64_t chunk_samples, int ring,
@@ -521,13 +521,13 @@ extern "C" int urh_fir_filter_stream(urh_ctx* ctx, const float* h_x, int64_t n, 
     URH_CHECK(filter_ring_init(ctx, R, ring, URH_FILTER_FIR, n, n, URH_DT_F32, m, 0, 0, chunk_samples, L));
     const float* d_taps = (const float*)L.extra;
     if (m > 0) URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_taps, (size_t)m * 8, cudaMemcpyHostToDevice, ctx->stream));
-    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
-                              [&](int64_t, const UrhWindow& w, int s) {
-                                  // the slot starts at the first history sample: the chunk's own samples follow k0 - a samples in
-                                  const float* x = (const float*)(L.in + s * L.z.in_slot + (w.k0 - w.a) * 8);
-                                  return urh_fir_filter_shard(ctx, x, w.k1 - w.k0, w.k0 > 0, d_taps, m, (float*)(L.out + s * L.z.out_slot));
-                              },
-                              contiguous_download(ctx, L, (char*)h_y, 8));
+    return stream_run(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          // the slot starts at the first history sample: the chunk's own samples follow k0 - a samples in
+                          const float* x = (const float*)(L.in + s * L.z.in_slot + (w.k0 - w.a) * 8);
+                          return urh_fir_filter_shard(ctx, x, w.k1 - w.k0, w.k0 > 0, d_taps, m, (float*)(L.out + s * L.z.out_slot));
+                      },
+                      contiguous_download(ctx, L.out, L.z.out_slot, (char*)h_y, 8));
 }
 
 // Two passes: the column sums chunk by chunk (upload only), then the subtraction of the mean (upload, compute, download).  Both cut
@@ -552,29 +552,28 @@ extern "C" int urh_dc_correction_stream(urh_ctx* ctx, const void* h_iq, int dtyp
     float carry[2] = {0.0f, 0.0f};
     double dsum[2] = {0.0, 0.0};
     long long isum[2] = {0, 0};
-    auto no_download = [](int64_t, const UrhWindow&, int, cudaStream_t) { return URH_OK; };
-    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
-                                 [&](int64_t, const UrhWindow& w, int s) {
-                                     const void* x = L.in + s * L.z.in_slot;
-                                     if (!f32) {
-                                         int64_t part[2];
-                                         URH_CHECK(urh_dc_int_column_sums(ctx, x, dtype, w.b - w.a, part));
-                                         isum[0] += part[0];
-                                         isum[1] += part[1];
-                                         return URH_OK;
-                                     }
-                                     double part[2];
-                                     URH_CHECK(urh_dc_column_sums(ctx, (const float*)x, w.b - w.a, exact_order, exact_order ? carry : nullptr, part));
-                                     if (exact_order) {   // float32 accumulators carried in doubles: exact
-                                         carry[0] = (float)part[0];
-                                         carry[1] = (float)part[1];
-                                     } else {
-                                         dsum[0] += part[0];
-                                         dsum[1] += part[1];
-                                     }
-                                     return URH_OK;
-                                 },
-                                 no_download));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
+                         [&](int64_t, const UrhWindow& w, int s) {
+                             const void* x = L.in + s * L.z.in_slot;
+                             if (!f32) {
+                                 int64_t part[2];
+                                 URH_CHECK(urh_dc_int_column_sums(ctx, x, dtype, w.b - w.a, part));
+                                 isum[0] += part[0];
+                                 isum[1] += part[1];
+                                 return URH_OK;
+                             }
+                             double part[2];
+                             URH_CHECK(urh_dc_column_sums(ctx, (const float*)x, w.b - w.a, exact_order, exact_order ? carry : nullptr, part));
+                             if (exact_order) {   // float32 accumulators carried in doubles: exact
+                                 carry[0] = (float)part[0];
+                                 carry[1] = (float)part[1];
+                             } else {
+                                 dsum[0] += part[0];
+                                 dsum[1] += part[1];
+                             }
+                             return URH_OK;
+                         },
+                         no_download));
     float mean32[2];
     double mean64[2];
     if (f32 && exact_order) {
@@ -588,13 +587,13 @@ extern "C" int urh_dc_correction_stream(urh_ctx* ctx, const void* h_iq, int dtyp
         mean64[1] = (double)isum[1] / (double)n;
     }
     const int64_t ob = f32 ? 8 : 16;
-    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, true,
-                                 [&](int64_t, const UrhWindow& w, int s) {
-                                     const void* x = L.in + s * L.z.in_slot;
-                                     void* y = L.out + s * L.z.out_slot;
-                                     if (f32) return urh_dc_subtract(ctx, (const float*)x, w.b - w.a, mean32[0], mean32[1], (float*)y);
-                                     return urh_dc_int_subtract(ctx, x, dtype, w.b - w.a, mean64[0], mean64[1], (double*)y);
-                                 },
-                                 contiguous_download(ctx, L, (char*)h_out, ob)));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, true,
+                         [&](int64_t, const UrhWindow& w, int s) {
+                             const void* x = L.in + s * L.z.in_slot;
+                             void* y = L.out + s * L.z.out_slot;
+                             if (f32) return urh_dc_subtract(ctx, (const float*)x, w.b - w.a, mean32[0], mean32[1], (float*)y);
+                             return urh_dc_int_subtract(ctx, x, dtype, w.b - w.a, mean64[0], mean64[1], (double*)y);
+                         },
+                         contiguous_download(ctx, L.out, L.z.out_slot, (char*)h_out, ob)));
     return URH_OK;
 }

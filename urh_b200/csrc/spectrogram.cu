@@ -709,12 +709,12 @@ static int stft_stream(urh_ctx* ctx, const float* h_x, int64_t n, int W, int hop
     URH_CHECK(filter_ring_init(ctx, R, ring, entry, n, num_frames, URH_DT_F32, W, hop, 0, chunk_samples, L));
     const double* d_window = (const double*)L.extra;
     URH_CUDA(ctx, cudaMemcpyAsync(L.extra, h_window, (size_t)W * 8, cudaMemcpyHostToDevice, ctx->stream));
-    return stream_run_windows(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
-                              [&](int64_t, const UrhWindow& w, int s) {
-                                  return stft_run(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, W, hop, d_window, w.k1 - w.k0,
-                                                  L.out + s * L.z.out_slot, mode);
-                              },
-                              contiguous_download(ctx, L, (char*)h_out, (int64_t)W * (mode == 0 ? 16 : 4)));
+    return stream_run(ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          return stft_run(ctx, (const float*)(L.in + s * L.z.in_slot), w.b - w.a, W, hop, d_window, w.k1 - w.k0,
+                                          L.out + s * L.z.out_slot, mode);
+                      },
+                      contiguous_download(ctx, L.out, L.z.out_slot, (char*)h_out, (int64_t)W * (mode == 0 ? 16 : 4)));
 }
 
 extern "C" int urh_stft_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window, int64_t num_frames,
@@ -758,7 +758,7 @@ extern "C" int urh_spectrogram_bgra_stream(urh_ctx* ctx, const float* h_x, int64
         *piece = w.k1 <= cum[s + 1];
         return s;
     };
-    return stream_run_windows(
+    return stream_run(
         ctx, win, R, (const char*)h_x, 8, L.in, L.z.in_slot, true,
         [&](int64_t, const UrhWindow& w, int slot) {
             bool piece;

@@ -166,16 +166,15 @@ static int noise_stream(urh_ctx* ctx, const void* h_iq, int64_t n, int64_t cs, i
     double* sum = (double*)(L.extra + 2 * r256(G * 8));
     double* mx = (double*)(L.extra + 2 * r256(G * 8) + r256((int64_t)nchunks * 8));
     const int ib = urh_iq_bytes(DT);
-    auto no_download = [](int64_t, const UrhWindow&, int, cudaStream_t) { return URH_OK; };
-    URH_CHECK(stream_run_windows(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
-                                 [&](int64_t, const UrhWindow& w, int s) {
-                                     LoadMagIQ<DT> ld;
-                                     ld.iq = L.in + s * L.z.in_slot - w.a * ib;   // sample i of the capture at ld.iq + i
-                                     URH_LAUNCH(ctx, (k_chunk_partial<LoadMagIQ<DT>>), (unsigned)(w.k1 - w.k0), STAT_BLOCK, 0, ld, n, cs,
-                                                nchunks, w.k0, psum, pmax);
-                                     return URH_OK;
-                                 },
-                                 no_download));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, ib, L.in, L.z.in_slot, false,
+                         [&](int64_t, const UrhWindow& w, int s) {
+                             LoadMagIQ<DT> ld;
+                             ld.iq = L.in + s * L.z.in_slot - w.a * ib;   // sample i of the capture at ld.iq + i
+                             URH_LAUNCH(ctx, (k_chunk_partial<LoadMagIQ<DT>>), (unsigned)(w.k1 - w.k0), STAT_BLOCK, 0, ld, n, cs,
+                                        nchunks, w.k0, psum, pmax);
+                             return URH_OK;
+                         },
+                         no_download));
     URH_LAUNCH(ctx, k_chunk_final, (unsigned)urh_div_up(nchunks, 128), 128, 0, psum, pmax, nchunks, sum, mx);
     URH_CUDA(ctx, cudaMemcpyAsync(h_sum, sum, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     URH_CUDA(ctx, cudaMemcpyAsync(h_max, mx, nchunks * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
@@ -380,14 +379,16 @@ extern "C" int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, in
     bool carry_valid = false;
     int carry_cls = 0;
     int64_t carry_len = 0;
-    URH_CHECK(stream_run(ctx, n, z.cs, R, (const char*)h_iq, urh_iq_bytes(dtype), false, R.mem, z.src_slot, nullptr, nullptr,
-                         [&](int64_t c, int64_t s0, int64_t s1, int s) {
-                             URH_CHECK(urh_get_magnitudes(ctx, R.mem + s * z.src_slot + URH_STREAM_PAD, dtype, s1 - s0, d_mag));
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
+    URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), R.mem, z.src_slot, false,
+                         [&](int64_t c, const UrhWindow& w, int s) {
+                             URH_CHECK(urh_get_magnitudes(ctx, R.mem + s * z.src_slot + URH_STREAM_PAD, dtype, w.k1 - w.k0, d_mag));
                              int64_t summary[4];
-                             URH_CHECK(urh_segment_shard_pass(ctx, d_mag, 1, s1 - s0, noise_threshold, summary));
+                             URH_CHECK(urh_segment_shard_pass(ctx, d_mag, 1, w.k1 - w.k0, noise_threshold, summary));
                              if (c == 0) first_above = (int)summary[3];
                              int64_t count = 0;
-                             URH_CHECK(urh_shard_candidates(ctx, carry_valid ? 1 : 0, carry_cls, carry_len, s0, &count, nullptr, nullptr,
+                             URH_CHECK(urh_shard_candidates(ctx, carry_valid ? 1 : 0, carry_cls, carry_len, w.k0, &count, nullptr, nullptr,
                                                             nullptr));
                              const size_t at = pos.size();
                              pos.resize(at + (size_t)count);
@@ -402,7 +403,8 @@ extern "C" int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, in
                              }
                              carry_valid = true;
                              return URH_OK;
-                         }));
+                         },
+                         no_download, place_after_pad));
     int64_t m = 0;
     URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, carry_cls, carry_len, n, nullptr, 0, &m));
     ctx->segments.resize((size_t)(2 * m));

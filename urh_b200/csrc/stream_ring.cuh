@@ -1,24 +1,27 @@
 // The ring of device slots that streamed calls move a host capture through (DESIGN.md §4.11), shared by the demodulation entries
-// (digitize.cu) and the filter and spectrogram entries (filter.cu, spectrogram.cu).
+// (digitize.cu), the filter and spectrogram entries (filter.cu, spectrogram.cu) and the auto-interpretation entries (stats.cu,
+// convert.cu).
 //
-// Two runners drive it:
-//   stream_run          chunks of whole tiles with at most a one-sample halo; qad downloaded into h_qad (urh_stream_schedule)
-//   stream_run_windows  chunks that own the outputs [k0, k1) and upload the input window [a, b) those outputs read, halos of any
-//                       length included, straight from host memory; each chunk's outputs leave through a caller-given download
-//                       (urh_stream_windows, urh_stream_window_schedule)
-// Both issue their ops in the order their schedule lists, with the same op semantics (include/urh_b200.h).
+// A chunk owns the outputs [k0, k1) and uploads the input window [a, b) those outputs read, halos included, straight from host memory,
+// so no chunk reads another chunk's slot.  urh_filter_windows cuts a capture into such chunks (two plans: whole tiles with at most a
+// one-sample halo, URH_FILTER_TILES; the windows of the filter, spectrogram, noise and conversion entries), urh_stream_window_schedule
+// orders their copies and computations (op semantics there), and stream_run issues that order.
 #pragma once
 #include "common.cuh"
 
 #define URH_STREAM_MAX_RING 8
 #define URH_NOISE_SLICES 64   // slices per noise chunk (stats.cu STAT_SLICES)
-#define URH_STREAM_PAD 256   // slot = [pad][halo][chunk]: the chunk starts 256 bytes in, the halo sample right before it
+#define URH_STREAM_PAD 256   // tile-chunk slot = [pad][halo][chunk]: the chunk starts 256 bytes in, the halo sample right before it
+#define URH_ARENA_BLOCK ((int64_t)64 << 20)   // the scratch arena grows in blocks of at least 64 MiB (context.cu urh_arena_alloc)
 enum { URH_OP_UPLOAD = 0, URH_OP_COMPUTE = 1, URH_OP_DOWNLOAD = 2 };
 
 static inline int64_t r256(int64_t b) { return (b + 255) & ~(int64_t)255; }
+// device bytes the arena may take for a streamed call's requests: a request that does not fit the current block's rest opens a new
+// block, so new blocks hold at most twice the requests plus one block
+static inline int64_t stream_arena_bytes(int64_t requests) { return 2 * requests + URH_ARENA_BLOCK; }
 
 // The ring of one streamed call: the block, its events, and the copy streams drained before the block is freed on every exit path.
-// arena_peak: the most scratch-arena bytes live at once over every chunk the runners computed (a chunk's window call may reset the
+// arena_peak: the most scratch-arena bytes live at once over every chunk stream_run computed (a chunk's computation may reset the
 // arena, which restarts ctx->arena_peak).
 struct StreamRing {
     urh_ctx* ctx = nullptr;
@@ -51,51 +54,6 @@ struct StreamRing {
     }
 };
 
-// Runs the schedule: compute(c, s0, s1, slot) enqueues chunk c's work on the compute stream (it may synchronise).  h_src: host source
-// of src_b bytes per sample uploaded into slots of src_slot bytes at d_src (NULL: the computation reads device data); h_qad: host
-// destination of the qad slots at d_qad (cs floats each; NULL: none).
-template <typename F>
-static int stream_run(urh_ctx* ctx, int64_t n, int64_t cs, StreamRing& R, const char* h_src, int src_b, bool halo, char* d_src,
-                      int64_t src_slot, float* h_qad, float* d_qad, F&& compute, bool qad_resident = false) {
-    const int flags = (h_src ? URH_STREAM_UPLOAD : 0) | (h_qad ? URH_STREAM_DOWNLOAD : 0) | (halo ? URH_STREAM_HALO : 0);
-    int64_t count = 0;
-    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, nullptr, 0, &count));
-    std::vector<int64_t> ops((size_t)(6 * count));
-    URH_CHECK(urh_stream_schedule(n, cs, R.ring, flags, ops.data(), count, &count));
-    bool recorded[3][URH_STREAM_MAX_RING] = {};
-    ctx->stream_chunks = 0;
-    for (int64_t i = 0; i < count; i++) {
-        const int64_t* o = &ops[(size_t)(6 * i)];
-        const int kind = (int)o[0], s = (int)o[2];
-        const int64_t c = o[1], s0 = o[3], s1 = o[4], h = o[5];
-        if (kind == URH_OP_UPLOAD) {
-            cudaStream_t cp = ctx->copy_stream[0];
-            if (recorded[URH_OP_COMPUTE][s]) URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
-            URH_CUDA(ctx, cudaMemcpyAsync(d_src + s * src_slot + URH_STREAM_PAD - h * src_b, h_src + (s0 - h) * src_b,
-                                          (size_t)((s1 - s0 + h) * src_b), cudaMemcpyHostToDevice, cp));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_UPLOAD][s], cp));
-        } else if (kind == URH_OP_COMPUTE) {
-            if (h_src) URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_UPLOAD][s], 0));
-            if (h_qad && !qad_resident && recorded[URH_OP_DOWNLOAD][s])
-                URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_DOWNLOAD][s], 0));
-            URH_CHECK(compute(c, s0, s1, s));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_COMPUTE][s], ctx->stream));
-            urh_stream_sample_free(ctx);
-            ctx->stream_chunks++;
-        } else {
-            cudaStream_t cp = ctx->copy_stream[1];
-            URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
-            URH_CUDA(ctx, cudaMemcpyAsync(h_qad + s0, d_qad + (qad_resident ? s0 : (int64_t)s * cs), (size_t)(s1 - s0) * sizeof(float),
-                                          cudaMemcpyDeviceToHost, cp));
-            URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_DOWNLOAD][s], cp));
-        }
-        recorded[kind][s] = true;
-    }
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->copy_stream[1]));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return URH_OK;
-}
-
 // the slots of urh_segment_messages_iq_stream (stats.cu): chunk samples, one IQ slot ([pad][chunk], 256-byte multiple), the float64
 // magnitude scratch of one chunk, the arena requests of one chunk's segmenter pass (urh_stream_footprint, digitize.cu)
 struct SegmentStreamSizes {
@@ -103,22 +61,35 @@ struct SegmentStreamSizes {
 };
 SegmentStreamSizes urh_segment_stream_sizes(int64_t n, int dtype, int64_t chunk_samples);
 
-// ---- the windowed ring ---------------------------------------------------------------------------------------------------------------
-// A chunk c is {k0, k1, a, b} (win[4 c ..]): it owns outputs [k0, k1) and reads input samples [a, b).  Slot s holds the window from its
-// first byte: d_src + s * src_slot = sample a.  compute(c, w, s) enqueues chunk c's work on the compute stream (it may synchronise);
-// download(c, w, s, copy_stream) enqueues the copies of its outputs to the host.  h_src NULL: no upload (the computation reads device
-// data); down false: no download (the computation keeps its results).
+// chunk c of a streamed call: it owns outputs [k0, k1) and reads input samples [a, b) (win[4 c ..] of urh_stream_windows)
 struct UrhWindow {
     int64_t k0, k1, a, b;
 };
 
-// the windows of a streamed filter / spectrogram entry (URH_FILTER_*; urh_stream_windows without the C wrapper)
+// the chunks of a streamed entry (URH_FILTER_*; urh_stream_windows without the C wrapper)
 int urh_filter_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples, const int64_t* h_seg_start,
                        const int64_t* h_seg_len, int nseg, std::vector<UrhWindow>& out);
+// samples per chunk of the tile plan: chunk_samples (<= 0: 2^24) rounded down to whole tiles, at least one; a capture shorter than a
+// chunk is one chunk of its whole tiles
+int64_t stream_chunk_samples(int64_t n, int64_t chunk_samples);
 
+// Where a chunk's window lands in its slot, in bytes from the slot's start (src_b bytes per sample): the windowed entries at the start;
+// a tile chunk so that its sample k0 sits at byte URH_STREAM_PAD and its halo right before it (the IQ kernels' vector loads rely on the
+// 256-byte alignment).
+typedef int64_t (*UrhPlace)(const UrhWindow& w, int src_b);
+static int64_t place_at_start(const UrhWindow&, int) { return 0; }
+static int64_t place_after_pad(const UrhWindow& w, int src_b) { return URH_STREAM_PAD - (w.k0 - w.a) * src_b; }
+
+// Runs the chunks win through the ring R in the order urh_stream_window_schedule gives.  h_src: host source of src_b bytes per sample;
+// chunk c's window is uploaded into slot s at d_src + s * src_slot + place(w, src_b) (h_src NULL: no upload, the computation reads
+// device data).  compute(c, w, s) enqueues chunk c's work on the compute stream (it may synchronise); download(c, w, s, copy_stream)
+// enqueues the copies of its outputs to the host (down false: none, the computation keeps its results).  download_resident: the
+// downloads read device data no later chunk rewrites, so a computation does not wait for the download before it on its slot.
+// ctx->arena_peak after the run: the most over its chunks.
 template <typename Compute, typename Download>
-static int stream_run_windows(urh_ctx* ctx, const std::vector<UrhWindow>& win, StreamRing& R, const char* h_src, int src_b, char* d_src,
-                              int64_t src_slot, bool down, Compute&& compute, Download&& download) {
+static int stream_run(urh_ctx* ctx, const std::vector<UrhWindow>& win, StreamRing& R, const char* h_src, int src_b, char* d_src,
+                      int64_t src_slot, bool down, Compute&& compute, Download&& download, UrhPlace place = place_at_start,
+                      bool download_resident = false) {
     const int flags = (h_src ? URH_STREAM_UPLOAD : 0) | (down ? URH_STREAM_DOWNLOAD : 0);
     const int64_t chunks = (int64_t)win.size();
     int64_t count = 0;
@@ -136,11 +107,13 @@ static int stream_run_windows(urh_ctx* ctx, const std::vector<UrhWindow>& win, S
             cudaStream_t cp = ctx->copy_stream[0];
             if (recorded[URH_OP_COMPUTE][s]) URH_CUDA(ctx, cudaStreamWaitEvent(cp, R.ev[URH_OP_COMPUTE][s], 0));
             if (w.b > w.a)
-                URH_CUDA(ctx, cudaMemcpyAsync(d_src + s * src_slot, h_src + w.a * src_b, (size_t)((w.b - w.a) * src_b), cudaMemcpyHostToDevice, cp));
+                URH_CUDA(ctx, cudaMemcpyAsync(d_src + s * src_slot + place(w, src_b), h_src + w.a * src_b, (size_t)((w.b - w.a) * src_b),
+                                              cudaMemcpyHostToDevice, cp));
             URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_UPLOAD][s], cp));
         } else if (kind == URH_OP_COMPUTE) {
             if (h_src) URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_UPLOAD][s], 0));
-            if (down && recorded[URH_OP_DOWNLOAD][s]) URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_DOWNLOAD][s], 0));
+            if (down && !download_resident && recorded[URH_OP_DOWNLOAD][s])
+                URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, R.ev[URH_OP_DOWNLOAD][s], 0));
             URH_CHECK(compute(c, w, s));
             URH_CUDA(ctx, cudaEventRecord(R.ev[URH_OP_COMPUTE][s], ctx->stream));
             if (ctx->arena_peak > R.arena_peak) R.arena_peak = ctx->arena_peak;
@@ -187,10 +160,12 @@ static int filter_ring_init(urh_ctx* ctx, StreamRing& R, int ring, int entry, in
     L.extra = L.out + ring * L.z.out_slot;
     return URH_OK;
 }
-// contiguous outputs of ob bytes each: chunk c's [k0, k1) from its output slot to h_out
-static auto contiguous_download(urh_ctx* ctx, const FilterRingLayout& L, char* h_out, int64_t ob) {
-    return [ctx, &L, h_out, ob](int64_t, const UrhWindow& w, int s, cudaStream_t cp) {
-        URH_CUDA(ctx, cudaMemcpyAsync(h_out + w.k0 * ob, L.out + s * L.z.out_slot, (size_t)((w.k1 - w.k0) * ob), cudaMemcpyDeviceToHost, cp));
+// contiguous outputs of ob bytes each: chunk c's [k0, k1) from its output slot at d_out + s * out_slot to h_out
+static auto contiguous_download(urh_ctx* ctx, const char* d_out, int64_t out_slot, char* h_out, int64_t ob) {
+    return [ctx, d_out, out_slot, h_out, ob](int64_t, const UrhWindow& w, int s, cudaStream_t cp) {
+        URH_CUDA(ctx, cudaMemcpyAsync(h_out + w.k0 * ob, d_out + s * out_slot, (size_t)((w.k1 - w.k0) * ob), cudaMemcpyDeviceToHost, cp));
         return URH_OK;
     };
 }
+// the download of a call whose chunks keep their results on the device (down false)
+static int no_download(int64_t, const UrhWindow&, int, cudaStream_t) { return URH_OK; }

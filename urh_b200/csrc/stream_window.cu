@@ -1,6 +1,7 @@
-// The windowed ring's plan (DESIGN.md §4.11, "The windowed ring"): which outputs each chunk of a streamed filter or spectrogram call
-// owns, which input window it uploads, the order of its copies and computations, and the device bytes of the streamed and the
-// resident form of each entry.  Host code only: everything here runs without a device.
+// The plan of a streamed call (DESIGN.md §4.11): which outputs each chunk owns and which input window it uploads, the order of its
+// copies and computations, and the device bytes of the streamed and the resident form of each windowed entry.  Host code only:
+// everything here runs without a device.
+#include "dense.cuh"   // URH_TILE
 #include "stream_ring.cuh"
 
 static int64_t filter_chunk(int64_t cs) { return cs > 0 ? cs : (int64_t)1 << 24; }
@@ -8,6 +9,14 @@ static int64_t frames_per_chunk(int64_t cs, int64_t hop) { return cs / hop > 0 ?
 // frames of a segment of len samples, as Spectrogram.stft and urh_spectrogram_bgra count them (short segments: one frame)
 static int64_t frames_of(int64_t len, int64_t W, int64_t hop) { return len < W ? 1 : (len - W) / hop + 1; }
 static int64_t clamp64(int64_t v, int64_t lo, int64_t hi) { return v < lo ? lo : (v > hi ? hi : v); }
+
+int64_t stream_chunk_samples(int64_t n, int64_t cs) {
+    if (cs <= 0) cs = (int64_t)1 << 24;
+    cs -= cs % URH_TILE;
+    if (cs < URH_TILE) cs = URH_TILE;
+    const int64_t whole = urh_div_up(n > 0 ? n : 1, URH_TILE) * URH_TILE;   // a capture shorter than a chunk: one slot of its size
+    return cs < whole ? cs : whole;
+}
 
 // The noise-chunk statistics (stats.cu) reduce each of the nchunks end-aligned chunks of cs samples in URH_NOISE_SLICES slices of
 // ceil(cs / URH_NOISE_SLICES) samples.  Slice g in sample order is slice g % 64 of chunk nchunks - 1 - g / 64 (chunk j covers
@@ -49,6 +58,15 @@ int urh_filter_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_
             for (int64_t k0 = 0; k0 < n; k0 += cs) {
                 const int64_t k1 = k0 + cs < n ? k0 + cs : n;
                 out.push_back({k0, k1, k0 > 0 ? k0 - h : 0, k1});
+            }
+            return URH_OK;
+        }
+        case URH_FILTER_TILES: {   // whole tiles, so every tile keeps its resident bounds; p0 = 1: later chunks read the sample before them
+            if (p0 != 0 && p0 != 1) return URH_ERR_INVALID;
+            cs = stream_chunk_samples(n, chunk_samples);
+            for (int64_t k0 = 0; k0 < n; k0 += cs) {
+                const int64_t k1 = k0 + cs < n ? k0 + cs : n;
+                out.push_back({k0, k1, k0 > 0 ? k0 - p0 : 0, k1});
             }
             return URH_OK;
         }
@@ -151,7 +169,13 @@ extern "C" int urh_stream_windows(int entry, int64_t n, int64_t out_len, int64_t
     return URH_OK;
 }
 
-// The op order of urh_stream_schedule (uploads R - 1 chunks ahead, each compute followed by its download), 7 int64 per op.
+// The op order of a streamed call, 7 int64 per op {kind, chunk, slot, k0, k1, a, b}.  Op semantics (stream_run and the host model of
+// tests/test_stream_filter_plan_cpu.py):
+//   upload(c, s)   copy stream 0: waits for the last compute recorded on slot s, copies, records "uploaded" on s
+//   compute(c, s)  compute stream: waits for "uploaded" on s (uploading calls) and for the last download recorded on s (calls whose
+//                  downloads read the slot), runs the chunk, records "computed" on s
+//   download(c, s) copy stream 1: waits for "computed" on s, copies the chunk's outputs out, records "downloaded" on s
+// Uploads run R - 1 chunks ahead: the upload of chunk c + R - 1 is issued before compute(c), into the slot compute(c - 1) released.
 extern "C" int urh_stream_window_schedule(const int64_t* h_win, int64_t chunks, int ring, int flags, int64_t* h_ops, int64_t cap,
                                           int64_t* count) {
     if (!count || chunks < 0 || (chunks > 0 && !h_win) || ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
@@ -269,9 +293,8 @@ extern "C" int urh_stream_filter_footprint(int entry, int64_t n, int64_t out_len
                                            int64_t chunk_samples, int ring, int resident, int64_t* bytes) {
     if (!bytes || !filter_args_ok(entry, n, out_len, dtype, p0, p1, p2)) return URH_ERR_INVALID;
     if (!resident && (ring < 2 || ring > URH_STREAM_MAX_RING)) return URH_ERR_INVALID;
-    const int64_t arena_block = (int64_t)64 << 20;   // the arena grows in blocks of at least 64 MiB
     if (resident) {
-        int64_t b = arena_block;
+        int64_t b = URH_ARENA_BLOCK;
         switch (entry) {
             case URH_FILTER_CONVOLVE: b += r256(n * 8) + r256(out_len * 8) + r256(p0 * 16); break;
             case URH_FILTER_FIR: b += 2 * r256(n * 8) + r256((p0 > 1 ? p0 : 1) * 8); break;
@@ -292,8 +315,7 @@ extern "C" int urh_stream_filter_footprint(int entry, int64_t n, int64_t out_len
         return URH_OK;
     }
     const FilterStreamSizes z = urh_filter_stream_sizes(entry, n, out_len, dtype, p0, p1, p2, chunk_samples);
-    // arena requests: at most twice what is asked plus one block (urh_stream_footprint's rule)
-    *bytes = ring * (z.in_slot + z.out_slot) + z.extra + 2 * z.work + arena_block;
+    *bytes = ring * (z.in_slot + z.out_slot) + z.extra + stream_arena_bytes(z.work);
     return URH_OK;
 }
 
