@@ -187,3 +187,33 @@ def test_oracle_costas_pinned_to_reference(oracle, request):
         cases += 1
     c.close()
     assert cases == 5 * 3 * 8 + 9 * 2
+
+
+def test_oracle_dense_edges_pinned_to_reference(oracle, request):
+    """The oracle's ASK/FSK afp_demod against the reference's compiled afp_demod on float32 captures with infinite, NaN, huge,
+    subnormal and zero samples of every sign, each after and before neighbours with zero and nonzero parts (tests/dense_edge_cases.py),
+    at noise 0 and 0.05.  An infinite part takes the reference's Annex G recovery of the float complex FSK product.  Words are
+    compared with NaN folded (the payload is not pinned).  The reference's answers are recorded in tests/golden/ref_dense_edges.json;
+    with oracle/_ref built the pin also runs live."""
+    from dense_edge_cases import REFERENCE_TABLE, folded, pinned_captures
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette, same
+
+    c = Cassette("dense_edges", request.node.name)
+    sf = ref_loader.load_kernels()[0] if (RECORD or ref_loader.kernels_available()) else None
+    cases = 0
+    for name, iq in pinned_captures():
+        for mod in ("ASK", "FSK"):
+            for noise in (0.0, 0.05):
+                mine = folded(oracle.afp_demod(iq, noise, mod, 2))
+                want = c.want(lambda: folded(sf.afp_demod(iq, noise, mod, 2)))
+                assert same(mine, want), (name, mod, noise)
+                if sf is not None:
+                    assert np.array_equal(mine, folded(sf.afp_demod(iq, noise, mod, 2))), (name, mod, noise)
+                cases += 1
+    c.close()
+    assert cases == 2 * 2 * 2
+    # the recovery by value: (predecessor, sample) -> the reference's angle
+    for prev, cur, word in REFERENCE_TABLE:
+        q = oracle.afp_demod(np.array([(1.0, 1.0), prev, cur], np.float32), 0.05, "FSK", 2)
+        assert q[2].view(np.uint32) == word, (prev, cur, hex(q[2].view(np.uint32)))

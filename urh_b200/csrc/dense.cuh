@@ -260,10 +260,11 @@ __device__ __forceinline__ UrhFskTerms urh_fsk_terms(float re, float im) {
     t.B = __fsub_rn(0.0f, t.D);
     return t;
 }
-// atan2f(imag, real) of (A + iB)(C + iD), bit-faithful to signal_functions.pyx:375-376
+// atan2f(imag, real) of (A + iB)(C + iD), bit-faithful to signal_functions.pyx:375-376: the product is the reference's
+// float complex one, so a sample with an infinite part takes the Annex G recovery (urh_cmulf) and gives a finite angle
 __device__ __forceinline__ float urh_fsk_angle(float A, float B, float C, float D) {
-    const float xr = __fsub_rn(__fmul_rn(A, C), __fmul_rn(B, D));
-    const float xi = __fadd_rn(__fmul_rn(A, D), __fmul_rn(B, C));
+    float xr, xi;
+    urh_cmulf(A, B, C, D, xr, xi);
     return urh_atan2f_v2(xi, xr);
 }
 
