@@ -217,3 +217,42 @@ def test_oracle_dense_edges_pinned_to_reference(oracle, request):
     for prev, cur, word in REFERENCE_TABLE:
         q = oracle.afp_demod(np.array([(1.0, 1.0), prev, cur], np.float32), 0.05, "FSK", 2)
         assert q[2].view(np.uint32) == word, (prev, cur, hex(q[2].view(np.uint32)))
+
+
+def _center_bits(c):
+    """a center as comparable bits: None stays None, a value becomes its float64 word"""
+    return None if c is None else int(np.float64(c).view(np.uint64))
+
+
+def test_oracle_center_edges_pinned_to_reference(oracle, request):
+    """The oracle's detect_center against the reference's own AutoInterpretation.detect_center on the named arrays of
+    tests/center_edge_cases.py: the keep rule at -4 and at non-finite samples, huge / subnormal / all-equal windows, windows of
+    0..3 kept samples, samples on bin edges, rank windows at tile boundaries and cut by max_size, levels far from zero.  Centers
+    are compared as float64 words, None as None.  The reference's answers are recorded in tests/golden/ref_center_edges.json;
+    with oracle/_ref built the pin also runs live."""
+    import warnings
+
+    from center_edge_cases import cases
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette
+
+    c = Cassette("center_edges", request.node.name)
+    live = RECORD or ref_loader.python_layer_available()
+    AIref = ref_loader.load_python_layer().AutoInterpretation if live else None
+    got = {}
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)   # np.var / np.mean of empty and overflowing windows
+        for name, x, max_size in cases():
+            mine = _center_bits(oracle.detect_center(x, max_size))
+            want = c.want(lambda: [name, _center_bits(AIref.detect_center(x, max_size))])
+            assert want == [name, mine], (name, want, mine)
+            if AIref is not None:
+                assert _center_bits(AIref.detect_center(x, max_size)) == mine, name
+            assert name not in got
+            got[name] = mine
+    c.close()
+    assert len(got) >= 50
+    # the cases reach both outcomes and the keep rule's corners
+    assert got["posinf_in_window"] is None and got["posinf_trimmed"] is not None
+    assert got["posinf_first_window_rank"] is None and got["posinf_last_trimmed_rank"] is not None
+    assert got["kept_2"] is None and got["kept_3"] is not None

@@ -336,17 +336,36 @@ def demod_detect_center(iq, noise_mag: float, mod_type: str, max_size=None, out=
     kept = C.c_int64(0)
     ctx.check(ctx.lib.urh_afp_demod_tiles(ctx.handle, C.c_void_p(d_iq.ptr), _lib.dtype_code(d_iq.dtype), n, float(noise_mag),
                                           code, C.c_void_p(qad.ptr), 0, C.byref(kept)))
-    r0, r1 = center_rank_window(kept.value, max_size)
+    st = fused_window_stats(ctx, qad, n, kept.value, max_size, bitwise)
+    return qad, _center_from_stats(ctx, qad, n, st, ctx.lib.urh_center_histogram_tiles)
+
+
+# The fused steps take np.var(rect) from the demodulator's double tile sums, (Σx² - n·mean²) / n.  numpy's float32 variance of
+# the same window differs from that by about the square of its float32 mean's error, which is up to ~2^-19 of |mean| (pairwise
+# sums, n up to 2^30).  Below var = mean² · 2^-14 (a strong, nearly constant level) that difference outgrows the variance's own
+# float32 rounding and moves the bin width, so there the steps replay numpy's variance instead (k_center_plan: state 2).
+FUSED_VAR_MIN_RATIO = 2.0 ** -14
+
+
+def fused_variance_stands(st):
+    """whether the double tile-sum variance in st (center_stats_from_window) may stand in for numpy's float32 np.var"""
+    return bool(st[6] >= st[5] * st[5] * FUSED_VAR_MIN_RATIO)
+
+
+def fused_window_stats(ctx, qad, n, kept, max_size=None, bitwise=False):
+    """detect_center's window statistics of qad from the tile table in the arena: the double tile-sum variance, or numpy's float32
+    variance replayed bit for bit (pairwise.cu) with ``bitwise`` or where the double one may not stand in for it"""
+    r0, r1 = center_rank_window(kept, max_size)
     w = np.zeros(5, dtype=np.float64)
     ctx.check(ctx.lib.urh_center_window_stats(ctx.handle, C.c_void_p(qad.ptr), n, r0, r1, w.ctypes.data_as(C.c_void_p)))
-    st = center_stats_from_window(kept.value, r0, r1, w)
-    if bitwise and r1 > r0:
+    st = center_stats_from_window(kept, r0, r1, w)
+    if int(st[2]) > int(st[1]) and (bitwise or not fused_variance_stands(st)):
         # np.var(rect) as numpy computes it (float32 pairwise sums replayed on the device): two more passes over the window,
         # and the center is bit-identical to the reference's instead of agreeing to ~1e-6
         mv = np.zeros(2, dtype=np.float64)
         ctx.check(ctx.lib.urh_center_window_var(ctx.handle, C.c_void_p(qad.ptr), n, r0, r1, mv.ctypes.data_as(C.c_void_p)))
         st[5], st[6] = mv[0], mv[1]
-    return qad, _center_from_stats(ctx, qad, n, st, ctx.lib.urh_center_histogram_tiles)
+    return st
 
 
 def center_rank_window(kept: int, max_size=None):

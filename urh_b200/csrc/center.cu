@@ -569,6 +569,7 @@ extern "C" int urh_center_histogram(urh_ctx* ctx, const float* d_x, int64_t n, i
 #include "tilescan.cuh"
 
 #define CEN_MAX_BINS 6000
+#define CEN_VAR_MIN_RATIO 0x1p-14   // the double tile-sum variance stands in for numpy's only down to var = mean^2 * 2^-14
 
 struct __align__(16) CenterPlan {
     long long total, offset;   // kept samples of the capture / of the preceding shards
@@ -739,7 +740,11 @@ __global__ void __launch_bounds__(256) k_center_plan(const CenStats* __restrict_
             const double hstep = (double)__double2float_rn(var);   // np.var of a float32 array is a float32
             hmin = (double)mn;
             const double stop = __dadd_rn((double)mx, hstep);
-            if (hstep != 0.0) {
+            // numpy's float32 mean is off by up to ~2^-19 of |mean|, so its variance moves by up to mean^2 * 2^-38: below
+            // var = mean^2 * 2^-14 (and for non-finite sums) that outgrows the variance's own float32 rounding, and the host
+            // path replays numpy's variance instead (CEN_VAR_MIN_RATIO, AutoInterpretation.FUSED_VAR_MIN_RATIO)
+            if (!(var >= __dmul_rn(__dmul_rn(mean, mean), CEN_VAR_MIN_RATIO))) state = 2;
+            else if (hstep != 0.0) {
                 const double val = __ddiv_rn(__dsub_rn(stop, hmin), hstep);
                 if (val == val && fabs(val) < 9.0e18) {
                     const long long len = (long long)ceil(val);

@@ -304,10 +304,7 @@ def _demod_center_digitize_stream(ctx, samples, noise_mag, code, tolerance, samp
                                                        _host_ptr(host) if host is not None else None, C.byref(center), C.byref(state),
                                                        C.byref(kept), C.byref(k)))
     if state.value == 2:
-        r0, r1 = AI.center_rank_window(kept.value, max_size)
-        w = np.zeros(5, dtype=np.float64)
-        ctx.check(ctx.lib.urh_center_window_stats(ctx.handle, C.c_void_p(qad.ptr), n, r0, r1, w.ctypes.data_as(C.c_void_p)))
-        st = AI.center_stats_from_window(kept.value, r0, r1, w)
+        st = AI.fused_window_stats(ctx, qad, n, kept.value, max_size)
         c = AI._center_from_stats(ctx, qad, n, st, ctx.lib.urh_center_histogram_tiles)
         rows = np.zeros((0, 2), dtype=np.int64)
         if c is not None:
