@@ -11,7 +11,7 @@
 //   a table that starts with a pause skips that row but keeps its length in `total`                          (:335-339)
 // Every step is a map or a prefix sum over rows; the bits are then expanded with one thread per output bit.
 #include "common.cuh"
-#include "scan.cuh"
+#include "tilescan.cuh"
 
 enum { PP_SKIP = 0, PP_DATA = 1, PP_ZERO = 2, PP_LONG = 3 };
 
@@ -51,9 +51,26 @@ __global__ void k_pp_mark(const int64_t* __restrict__ seg, const uint8_t* __rest
     if (i < k && has_data[i]) seg_has[seg[i]] = 1;
 }
 
-__global__ void k_pp_effective(const int64_t* __restrict__ seg, const int64_t* __restrict__ seg_has, int64_t k, int64_t* __restrict__ nbits) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < k && !seg_has[seg[i]]) nbits[i] = 0;
+// scan elements: in[i]; out[i] = exclusive prefix (in == out: in place)
+struct PpPrefix {
+    const int64_t* in;
+    int64_t* out;
+    __device__ __forceinline__ int64_t load(int64_t i) const { return in[i]; }
+    __device__ __forceinline__ void post(int64_t i, const int64_t& excl, const int64_t&) const { out[i] = excl; }
+};
+// a row's bits count only if its segment is a message; nbits[i] becomes the row's bit offset
+struct PpBitOffsets {
+    const int64_t* seg;
+    const int64_t* seg_has;
+    int64_t* nbits;
+    __device__ __forceinline__ int64_t load(int64_t i) const { return seg_has[seg[i]] ? nbits[i] : 0; }
+    __device__ __forceinline__ void post(int64_t i, const int64_t& excl, const int64_t&) const { nbits[i] = excl; }
+};
+// 8 items per thread: on a table of 10^7 rows that runs each scan about a fifth faster than 16 (H100)
+static int pp_scan(urh_ctx* ctx, const int64_t* in, int64_t* out, int64_t k, int64_t* d_total) {
+    PpPrefix f;
+    f.in = in; f.out = out;
+    return urhts::scan<int64_t, urhts::AddI64, PpPrefix, 8>(ctx, k, (int64_t)0, urhts::AddI64(), f, d_total);
 }
 
 // mailbox: {n_msgs, total_bits, final_open, n_long}
@@ -147,14 +164,14 @@ extern "C" int urh_ppseq_to_bits(urh_ctx* ctx, const int64_t* d_rows, int64_t k,
     URH_CHECK(urh_arena(ctx, (size_t)k, &has_data));
     const unsigned g = (unsigned)urh_div_up(k, 256);
     URH_LAUNCH(ctx, k_pp_rows, g, 256, 0, d_rows, k, (double)samples_per_symbol, (int)bits_per_symbol, pause_threshold, total, nbits, seg, type, has_data);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, total, k, urhscan::AddI64(), (int64_t)0, true, d_cnt + 0)));
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, seg, k, urhscan::AddI64(), (int64_t)0, true, d_cnt + 1)));
+    URH_CHECK(pp_scan(ctx, total, total, k, d_cnt + 0));
+    URH_CHECK(pp_scan(ctx, seg, seg, k, d_cnt + 1));
     URH_CUDA(ctx, cudaMemsetAsync(seg_has, 0, ((size_t)k + 2) * sizeof(int64_t), ctx->stream));
     URH_LAUNCH(ctx, k_pp_mark, g, 256, 0, seg, has_data, k, seg_has);
-    URH_CUDA(ctx, cudaMemcpyAsync(seg_msg, seg_has, ((size_t)k + 1) * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, seg_msg, k + 1, urhscan::AddI64(), (int64_t)0, true, d_cnt + 2)));
-    URH_LAUNCH(ctx, k_pp_effective, g, 256, 0, seg, seg_has, k, nbits);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, nbits, k, urhscan::AddI64(), (int64_t)0, true, d_cnt + 3)));
+    URH_CHECK(pp_scan(ctx, seg_has, seg_msg, k + 1, d_cnt + 2));
+    PpBitOffsets fb;
+    fb.seg = seg; fb.seg_has = seg_has; fb.nbits = nbits;
+    URH_CHECK((urhts::scan<int64_t, urhts::AddI64, PpBitOffsets, 8>(ctx, k, (int64_t)0, urhts::AddI64(), fb, d_cnt + 3)));
     URH_LAUNCH(ctx, k_pp_counts, 1, 1, 0, seg_has, d_cnt + 1, d_cnt + 2, d_cnt + 3, mail);
     int64_t h[4], total_end = 0;
     URH_CHECK(urh_read_i64(ctx, mail, 4, h));

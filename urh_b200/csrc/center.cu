@@ -12,7 +12,7 @@
 //   3. histogram: ONE pass over qad.  Bin edges become float thresholds (exact, see k_hist_edges), every thread counts
 //      its currently popular bins in registers and only misses touch the shared-memory histogram.
 #include "dense.cuh"
-#include "scan.cuh"
+#include "tilescan.cuh"
 
 #include <math.h>
 #include <stdlib.h>
@@ -62,9 +62,21 @@ k_tile_stats_f32(const float* __restrict__ x, int64_t n, int64_t ntiles, UrhTile
 }
 
 // ---- 2. rank prefix, window tiles, window statistics --------------------------------------------------------------------
-__global__ void k_tile_counts(const UrhTileStats* __restrict__ ts, int64_t ntiles, int64_t* __restrict__ prefix) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < ntiles) prefix[t] = ts[t].cnt;
+struct ScanKept {
+    const UrhTileStats* ts;
+    int64_t* prefix;
+    __device__ __forceinline__ int64_t load(int64_t t) const { return ts[t].cnt; }
+    __device__ __forceinline__ void post(int64_t t, const int64_t& excl, const int64_t&) const { prefix[t] = excl; }
+};
+struct CenAddI64 {
+    __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; }
+};
+
+// prefix[t] = kept samples of the tiles before t, prefix[ntiles] = all of them (ntiles >= 1).  Enqueued only, no synchronisation.
+static int kept_prefix(urh_ctx* ctx, const UrhTileStats* ts, int64_t ntiles, int64_t* prefix) {
+    ScanKept fk;
+    fk.ts = ts; fk.prefix = prefix;
+    return urhts::scan<int64_t, CenAddI64, ScanKept>(ctx, ntiles, (int64_t)0, CenAddI64(), fk, prefix + ntiles);
 }
 
 // Tile t holds ranks [prefix[t], prefix[t+1]).  win[0] = tile of rank r0, win[1] = tile of rank r1-1 (r0 < r1 <= total);
@@ -185,13 +197,10 @@ __global__ void __launch_bounds__(256) k_center_fold(const CenStats* __restrict_
 // Rank prefix over a tile table; leaves {x, ts, prefix, n} in ctx for the window / histogram calls.
 int urh_center_tiles_begin(urh_ctx* ctx, const float* d_x, const UrhTileStats* ts, int64_t n, int64_t* h_total) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
-    int64_t *prefix, *d_total;
+    int64_t* prefix;
     URH_CHECK(urh_arena(ctx, (size_t)ntiles + 1, &prefix));
-    URH_CHECK(urh_arena(ctx, 4, &d_total));
-    URH_LAUNCH(ctx, k_tile_counts, (unsigned)urh_div_up(ntiles, 256), 256, 0, ts, ntiles, prefix);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, prefix, ntiles, urhscan::AddI64(), (int64_t)0, true, d_total)));
-    URH_CUDA(ctx, cudaMemcpyAsync(prefix + ntiles, d_total, sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
-    URH_CHECK(urh_read_i64(ctx, d_total, 1, h_total));
+    URH_CHECK(kept_prefix(ctx, ts, ntiles, prefix));
+    URH_CHECK(urh_read_i64(ctx, prefix + ntiles, 1, h_total));
     ctx->center_prefix = prefix;
     ctx->center_ts = ts;
     ctx->center_n = n;
@@ -566,8 +575,6 @@ extern "C" int urh_center_histogram(urh_ctx* ctx, const float* d_x, int64_t n, i
 //     which peak is taken hands the decision back to the host path (state 2), as do more than CEN_MAX_BINS bins.
 // Sharded captures: the kept counts, the window partials and the histogram are exchanged with NCCL on the context stream.
 // =============================================================================================================================
-#include "tilescan.cuh"
-
 #define CEN_MAX_BINS 6000
 #define CEN_VAR_MIN_RATIO 0x1p-14   // the double tile-sum variance stands in for numpy's only down to var = mean^2 * 2^-14
 
@@ -588,16 +595,6 @@ struct __align__(16) CenterPlan {
     int certified;             // 1: k_center_certify decided the center from the fine histogram (no histogram pass over qad)
     long long straddle;        // U - L of the two deciding bins (k_center_certify)
     long long pad;
-};
-
-struct ScanKept {
-    const UrhTileStats* ts;
-    int64_t* prefix;
-    __device__ __forceinline__ int64_t load(int64_t t) const { return ts[t].cnt; }
-    __device__ __forceinline__ void post(int64_t t, const int64_t& excl, const int64_t&) const { prefix[t] = excl; }
-};
-struct CenAddI64 {
-    __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; }
 };
 
 // counts: this shard's kept total (world == 1) or the gathered totals of all ranks
@@ -1057,9 +1054,7 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
         URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &cert_lo));
         URH_CHECK(urh_arena(ctx, (size_t)CEN_MAX_BINS, &cert_hi));
     }
-    ScanKept fk;
-    fk.ts = ts; fk.prefix = prefix;
-    URH_CHECK((urhts::scan<int64_t, CenAddI64, ScanKept>(ctx, ntiles, (int64_t)0, CenAddI64(), fk, prefix + ntiles)));
+    URH_CHECK(kept_prefix(ctx, ts, ntiles, prefix));
     const int64_t* counts = prefix + ntiles;
     if (world > 1) {
         URH_TL_MARK(ctx, "x1 kept counts: enter");

@@ -82,7 +82,7 @@ struct urh_ctx {
     void* nccl_stage;
     void* nccl_hstage;  // pinned twin of nccl_stage
     int nccl_rank, nccl_world;
-    // tilescan.cuh workspace (look-back scans over tile tables)
+    // tilescan.cuh workspace (the look-back scans)
     void* ts_mem;
     int64_t ts_cap_blocks;
     unsigned long long ts_issued;

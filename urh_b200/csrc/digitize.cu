@@ -3,7 +3,7 @@
 // Reference: src/urh/cythonext/signal_functions.pyx:333-378 (afp_demod), :392-495 (grab_pulse_lens).
 // See dense.cuh for the dense pass and DESIGN.md for the run/candidate restatement of the digitizer.
 #include "dense.cuh"
-#include "scan.cuh"
+#include "tilescan.cuh"
 #include "sparse.cuh"
 #include "fsk_fast.cuh"
 #include "dense_f32.cuh"
@@ -527,6 +527,12 @@ struct StreamSizes {
     int64_t scan_items;  // largest table a look-back scan of the call runs over
     int64_t rows_chunk;  // bound of one chunk's rows
 };
+// workspace of the look-back scans (context.cu urhts::prepare) after tables of up to `items` elements: twice the blocks of the
+// largest launch (256+ items each), at least 8192
+static int64_t scan_workspace_bytes(int64_t items) {
+    const int64_t nb = 2 * (items / 256 + 1);
+    return 256 + (nb > 8192 ? nb : 8192) * (4 + 2 * (int64_t)urhts::SLOT);
+}
 static int64_t finish_arena_bytes(int64_t tiles, int64_t rows_cap, bool ask) {
     return r256(tiles * (int64_t)sizeof(RunCarry)) + 2 * r256(tiles * 4) + 2 * r256(tiles * 8) + r256((32 + 8) * 8) +
            (ask ? r256(rows_cap * 16) : 0);
@@ -576,13 +582,12 @@ static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_sam
 }
 
 // Message segmentation from IQ (stats.cu urh_segment_messages_iq_stream): the arena of one pass of the sharded segmenter over `tiles`
-// tiles of float64 magnitudes (urh_segment_shard_pass: tile table, staging, closing-run scan; urh_shard_candidates: carries, heads,
-// counts, the candidates, at most one per 10 samples; the scans' aggregates)
+// tiles of float64 magnitudes (urh_segment_shard_pass: tile table, staging, closing-run total; urh_shard_candidates: heads, offsets,
+// counts, the candidates, at most one per 10 samples).  Its scans use the look-back workspace (scan_workspace_bytes), not the arena.
 static int64_t segment_arena_bytes(int64_t tiles) {
     const int64_t cap = URH_TILE / 10 + 2, cand = tiles * URH_TILE / 10 + 3;
-    return r256(tiles * (int64_t)sizeof(UrhTileSummary)) + r256(tiles * cap * 4) + 2 * r256(tiles * (int64_t)sizeof(RunCarry)) +
-           2 * r256(2 * (int64_t)sizeof(RunCarry)) + r256(tiles * 4) + r256(tiles * 8) + r256(32) + r256(cand * 8) + r256(cand * 2) +
-           3 * r256((tiles + 2) * 16);
+    return r256(tiles * (int64_t)sizeof(UrhTileSummary)) + r256(tiles * cap * 4) + 2 * r256(2 * (int64_t)sizeof(RunCarry)) +
+           r256(tiles * 4) + r256(tiles * 8) + r256(32) + r256(cand * 8) + r256(cand * 2);
 }
 SegmentStreamSizes urh_segment_stream_sizes(int64_t n, int dtype, int64_t chunk_samples) {
     SegmentStreamSizes z;
@@ -599,12 +604,13 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
     if ((entry & 0xf) == URH_STREAM_ENTRY_SEGMENT_MESSAGES) {
         if (urh_iq_bytes(dtype) == 0) return URH_ERR_DTYPE;
         if (entry & URH_STREAM_RESIDENT) {   // the capture, its float64 magnitudes, urh_segment_messages' tables over all of it
-            *bytes = r256(n * urh_iq_bytes(dtype)) + r256(n * 8) + segment_arena_bytes(urh_div_up(n, URH_TILE)) + URH_ARENA_BLOCK;
+            const int64_t ntiles = urh_div_up(n, URH_TILE);
+            *bytes = r256(n * urh_iq_bytes(dtype)) + r256(n * 8) + segment_arena_bytes(ntiles) + URH_ARENA_BLOCK + scan_workspace_bytes(ntiles);
             return URH_OK;
         }
         if (ring < 2 || ring > URH_STREAM_MAX_RING) return URH_ERR_INVALID;
         const SegmentStreamSizes z = urh_segment_stream_sizes(n, dtype, chunk_samples);
-        *bytes = ring * z.src_slot + z.mag_bytes + stream_arena_bytes(z.arena);
+        *bytes = ring * z.src_slot + z.mag_bytes + stream_arena_bytes(z.arena) + scan_workspace_bytes(z.cs / URH_TILE);
         return URH_OK;
     }
     if ((entry & 0xf) == URH_STREAM_ENTRY_ESTIMATE) {
@@ -641,9 +647,7 @@ extern "C" int urh_stream_footprint(int64_t n, int dtype, int tolerance, int64_t
         return URH_OK;
     }
     int64_t b = z.ring_bytes + stream_arena_bytes(z.arena);
-    // look-back scan workspace (context.cu urhts::prepare): at least 8192 blocks, 256+ items each
-    const int64_t nb = 2 * (z.scan_items / 256 + 1);
-    b += 256 + (nb > 8192 ? nb : 8192) * (4 + 2 * 32);
+    b += scan_workspace_bytes(z.scan_items);
     // pulse table: grown with its rows kept (old and new table alive during the copy, the new one up to twice the old)
     if (digitize) b += 3 * 16 * (r + z.rows_chunk);
     *bytes = b;

@@ -61,20 +61,8 @@ struct FireOp {
 };
 
 // ---- A ---------------------------------------------------------------------------------------------------------------
-struct ScanRunCarry {
-    const UrhTileSummary* tiles;
-    int64_t n;
+struct ScanRunCarry : TileRuns {
     RunCarry* carry;
-    __device__ __forceinline__ RunCarry load(int64_t t) const {
-        const int64_t rem = n - t * URH_TILE;
-        const int tile_len = rem < URH_TILE ? (int)rem : URH_TILE;
-        const UrhTileSummary s = tiles[t];
-        RunCarry r;
-        r.len = s.tail_len;
-        r.cls = s.last_cls;
-        r.flags = (s.head_len == tile_len) ? 1 : 0;
-        return r;
-    }
     __device__ __forceinline__ void post(int64_t t, const RunCarry& excl, const RunCarry&) const { carry[t] = excl; }
 };
 

@@ -13,7 +13,7 @@
 // cuFFT is used for the FFTs only.  Parity: the float32 FFT differs from pocketfft in rounding, so features agree to ~1e-5
 // relative; the tests compare features with that tolerance and the decisions on the golden captures exactly.
 #include "common.cuh"
-#include "scan.cuh"
+#include "tilescan.cuh"
 
 #include <cufft.h>
 #include <math.h>
@@ -32,13 +32,14 @@
 // data[np.abs(data) > 0]: a NaN magnitude compares false, so (NaN, 0) is dropped while (inf, NaN), whose hypot is inf, stays
 __device__ __forceinline__ bool urh_mod_keep(float2 v) { return hypotf(v.x, v.y) > 0.0f; }
 
-__global__ void k_mod_flags(const float2* __restrict__ x, int64_t n, int64_t* __restrict__ flag) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) {
-        const float2 v = x[i];
-        flag[i] = urh_mod_keep(v) ? 1 : 0;
-    }
-}
+// scan element: 1 for a kept sample; off[i] = kept samples before i (k_mod_compact's destination).  Scanned with 8 items per
+// thread, as the per-row tables of bits.cu: faster than 16 on a per-sample table
+struct ModKeepOffsets {
+    const float2* x;
+    int64_t* off;
+    __device__ __forceinline__ int64_t load(int64_t i) const { return urh_mod_keep(x[i]) ? 1 : 0; }
+    __device__ __forceinline__ void post(int64_t i, const int64_t& excl, const int64_t&) const { off[i] = excl; }
+};
 
 __global__ void k_mod_compact(const float2* __restrict__ x, int64_t n, const int64_t* __restrict__ off, float2* __restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -252,19 +253,20 @@ extern "C" int urh_modulation_features(urh_ctx* ctx, const float* d_data, int64_
     if (wavelet_scale < 1 || median_k < 1 || median_k > 64) URH_FAIL(ctx, URH_ERR_INVALID, "wavelet_scale >= 1 and 1 <= median k <= 64 required");
     urh_arena_reset(ctx);
     const float2* x = (const float2*)d_data;
-    int64_t *flag, *d_cnt;
-    URH_CHECK(urh_arena(ctx, (size_t)n, &flag));
+    int64_t *off, *d_cnt;
+    URH_CHECK(urh_arena(ctx, (size_t)n, &off));
     URH_CHECK(urh_arena(ctx, 4, &d_cnt));
     const unsigned g = (unsigned)urh_div_up(n, 256);
-    URH_LAUNCH(ctx, k_mod_flags, g, 256, 0, x, n, flag);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, flag, n, urhscan::AddI64(), (int64_t)0, true, d_cnt)));
+    ModKeepOffsets fk;
+    fk.x = x; fk.off = off;
+    URH_CHECK((urhts::scan<int64_t, urhts::AddI64, ModKeepOffsets, 8>(ctx, n, (int64_t)0, urhts::AddI64(), fk, d_cnt)));
     int64_t nz = 0;
     URH_CHECK(urh_read_i64(ctx, d_cnt, 1, &nz));
     h_feat[0] = (double)nz;
     if (nz == 0 || n - nz > 3) return URH_OK;   // None / "OOK" without looking further (AutoInterpretation.py:154-159)
     float2* data;
     URH_CHECK(urh_arena(ctx, (size_t)nz, &data));
-    URH_LAUNCH(ctx, k_mod_compact, g, 256, 0, x, n, flag, data);
+    URH_LAUNCH(ctx, k_mod_compact, g, 256, 0, x, n, off, data);
     // |max(data)|: lexicographic maximum, then float32 hypot
     const int nb = (int)min((int64_t)ctx->sm_count * 2, urh_div_up(nz, 256));
     float2* pmax;

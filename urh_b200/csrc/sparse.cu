@@ -1,35 +1,46 @@
 // Run stitching and candidate collection over a tile table: the segmenter's and the plateau RLE's candidate tables and a shard's
 // closing run (see sparse.cuh, DESIGN.md §4.2).
 #include "sparse.cuh"
-#include "scan.cuh"
+#include "tilescan.cuh"
 
-// ---- run stitching across tiles (RunCarry / RunCarryOp: sparse.cuh) -------------------------------------
-__global__ void k_tile_elems(const UrhTileSummary* __restrict__ tiles, int64_t ntiles, int64_t n, RunCarry* __restrict__ e) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ntiles) return;
-    const int64_t rem = n - t * URH_TILE;
-    const int tile_len = rem < URH_TILE ? (int)rem : URH_TILE;
-    const UrhTileSummary s = tiles[t];
-    RunCarry r;
-    r.len = s.tail_len;
-    r.cls = s.last_cls;
-    r.flags = (s.head_len == tile_len) ? 1 : 0;
-    e[t] = r;
-}
+// ---- run stitching across tiles (RunCarry / RunCarryOp / TileRuns: sparse.cuh) -----------------------------------
+// only the total: the run that ends the table
+struct RunTotal : TileRuns {
+    __device__ __forceinline__ void post(int64_t, const RunCarry&, const RunCarry&) const {}
+};
 
-// head candidate of each tile from the carry of all preceding tiles
-__global__ void k_tile_heads(const UrhTileSummary* __restrict__ tiles, const RunCarry* __restrict__ carry,
-                             int64_t ntiles, int tol, int32_t* __restrict__ head_rel, int64_t* __restrict__ total) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ntiles) return;
-    const UrhTileSummary s = tiles[t];
-    const RunCarry c = carry[t];
-    int64_t start_len = 0;
-    if (!(c.flags & 2) && c.cls == s.first_cls) start_len = c.len;
-    int32_t rel = -1;
-    if (start_len <= tol && (int64_t)tol < start_len + s.head_len) rel = (int32_t)(tol - start_len);
-    head_rel[t] = rel;
-    total[t] = (int64_t)s.ncand + (rel >= 0 ? 1 : 0);
+// head candidate of each tile from the carry of all preceding tiles (and of the preceding shards, if any)
+struct RunHeads : TileRuns {
+    int tol;
+    int has_in;
+    RunCarry in;
+    int32_t* head_rel;
+    __device__ __forceinline__ void post(int64_t t, const RunCarry& excl, const RunCarry&) const {
+        const RunCarry c = has_in ? RunCarryOp()(in, excl) : excl;
+        const UrhTileSummary s = tiles[t];
+        int64_t start_len = 0;
+        if (!(c.flags & 2) && c.cls == s.first_cls) start_len = c.len;
+        int32_t rel = -1;
+        if (start_len <= tol && (int64_t)tol < start_len + s.head_len) rel = (int32_t)(tol - start_len);
+        head_rel[t] = rel;
+    }
+};
+
+// candidates of each tile (its head candidate and the staged ones) -> offset of the tile's first candidate in the table
+struct CandOffsets {
+    const UrhTileSummary* tiles;
+    const int32_t* head_rel;
+    int64_t* offset;
+    __device__ __forceinline__ int64_t load(int64_t t) const { return (int64_t)tiles[t].ncand + (head_rel[t] >= 0 ? 1 : 0); }
+    __device__ __forceinline__ void post(int64_t t, const int64_t& excl, const int64_t&) const { offset[t] = excl; }
+};
+
+static RunCarry run_identity() {
+    RunCarry ident;
+    ident.len = 0;
+    ident.cls = 0;
+    ident.flags = 2 | 1;
+    return ident;
 }
 
 // one warp per tile: head candidate first, then the staged interior candidates
@@ -58,22 +69,13 @@ __global__ void k_gather(const UrhTileSummary* __restrict__ tiles, const uint32_
     }
 }
 
-__global__ void k_apply_carry(RunCarry* __restrict__ carry, int64_t ntiles, RunCarry in) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ntiles) return;
-    carry[t] = RunCarryOp()(in, carry[t]);
-}
-
 int urh_shard_run_total(urh_ctx* ctx, int64_t n, const UrhTileSummary* tiles, int64_t* h_out) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
-    RunCarry* carry;
     RunCarry* d_total_run;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &carry));
     URH_CHECK(urh_arena(ctx, 2, &d_total_run));
-    URH_LAUNCH(ctx, k_tile_elems, (unsigned)urh_div_up(ntiles, 256), 256, 0, tiles, ntiles, n, carry);
-    RunCarry ident;
-    ident.len = 0; ident.cls = 0; ident.flags = 2 | 1;
-    URH_CHECK((urhscan::device_scan<RunCarry, RunCarryOp>(ctx, carry, ntiles, RunCarryOp(), ident, true, d_total_run)));
+    RunTotal f;
+    f.tiles = tiles; f.n = n;
+    URH_CHECK((urhts::scan<RunCarry, RunCarryOp, RunTotal>(ctx, ntiles, run_identity(), RunCarryOp(), f, d_total_run)));
     int64_t raw[2];
     URH_CHECK(urh_read_i64(ctx, (const int64_t*)d_total_run, 2, raw));
     RunCarry tr;
@@ -94,30 +96,23 @@ int urh_collect_candidates(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummar
 int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummary* tiles, const uint32_t* staging,
                                  int stage_cap, UrhShardCarry carry_in, int64_t global_offset, UrhCandidates* out) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
-    RunCarry* carry;
     int32_t* head_rel;
-    int64_t* total;
+    int64_t* offset;
     int64_t* d_count;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &carry));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &head_rel));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &total));
-    URH_CHECK(urh_arena(ctx, 4, &d_count));
-    const unsigned g = (unsigned)urh_div_up(ntiles, 256);
-    URH_LAUNCH(ctx, k_tile_elems, g, 256, 0, tiles, ntiles, n, carry);
-    RunCarry ident;
-    ident.len = 0;
-    ident.cls = 0;
-    ident.flags = 2 | 1;
     RunCarry* d_total_run;
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &head_rel));
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &offset));
+    URH_CHECK(urh_arena(ctx, 4, &d_count));
     URH_CHECK(urh_arena(ctx, 2, &d_total_run));
-    URH_CHECK((urhscan::device_scan<RunCarry, RunCarryOp>(ctx, carry, ntiles, RunCarryOp(), ident, true, d_total_run)));
-    if (carry_in.valid) {
-        RunCarry in;
-        in.len = carry_in.len; in.cls = carry_in.cls; in.flags = 0;
-        URH_LAUNCH(ctx, k_apply_carry, g, 256, 0, carry, ntiles, in);
-    }
-    URH_LAUNCH(ctx, k_tile_heads, g, 256, 0, tiles, carry, ntiles, tol, head_rel, total);
-    URH_CHECK((urhscan::device_scan<int64_t, urhscan::AddI64>(ctx, total, ntiles, urhscan::AddI64(), (int64_t)0, true, d_count)));
+    RunHeads fh;
+    fh.tiles = tiles; fh.n = n; fh.tol = tol; fh.head_rel = head_rel;
+    fh.has_in = carry_in.valid ? 1 : 0;
+    fh.in.len = carry_in.len; fh.in.cls = carry_in.cls; fh.in.flags = 0;
+    // the total is the shard's own closing run, without the carry of the preceding shards
+    URH_CHECK((urhts::scan<RunCarry, RunCarryOp, RunHeads>(ctx, ntiles, run_identity(), RunCarryOp(), fh, d_total_run)));
+    CandOffsets fc;
+    fc.tiles = tiles; fc.head_rel = head_rel; fc.offset = offset;
+    URH_CHECK((urhts::scan<int64_t, urhts::AddI64, CandOffsets>(ctx, ntiles, (int64_t)0, urhts::AddI64(), fc, d_count)));
     int64_t C = 0;
     URH_CHECK(urh_read_i64(ctx, d_count, 1, &C));
     {
@@ -135,6 +130,6 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
     URH_CHECK(urh_arena(ctx, (size_t)C, &out->pos));
     URH_CHECK(urh_arena(ctx, (size_t)C, &out->cls));
     const unsigned gg = (unsigned)urh_div_up(ntiles * 32, 256);
-    URH_LAUNCH(ctx, k_gather, gg, 256, 0, tiles, staging, stage_cap, head_rel, total, ntiles, global_offset, out->pos, out->cls);
+    URH_LAUNCH(ctx, k_gather, gg, 256, 0, tiles, staging, stage_cap, head_rel, offset, ntiles, global_offset, out->pos, out->cls);
     return URH_OK;
 }

@@ -28,6 +28,22 @@ struct RunCarryOp {
     }
 };
 
+// The look-back scan's element (tilescan.cuh) for run stitching over a tile table of n samples: tile t's closing run, whole if
+// the tile is one run.  Callers add the post hook that consumes the carries.
+struct TileRuns {
+    const UrhTileSummary* tiles;
+    int64_t n;
+    __device__ __forceinline__ RunCarry load(int64_t t) const {
+        const int64_t rem = n - t * URH_TILE;
+        const int tile_len = rem < URH_TILE ? (int)rem : URH_TILE;
+        const UrhTileSummary s = tiles[t];
+        RunCarry r;
+        r.len = s.tail_len;
+        r.cls = s.last_cls;
+        r.flags = (s.head_len == tile_len) ? 1 : 0;
+        return r;
+    }
+};
 
 // Chunks of one capture digitized one after another on the same GPU (streaming, finish.cu): what the finish of chunk c needs from
 // the chunks before it, left in device memory by their finishes.  The same three totals a shard receives from its predecessors.

@@ -10,7 +10,6 @@
 // stays on the host in urh_b200/ainterpretation/AutoInterpretation.py, exactly as in the reference; the
 // sample-rate reductions run here.
 #include "dense_f32.cuh"
-#include "scan.cuh"
 #include "sparse.cuh"
 #include "stream_ring.cuh"
 

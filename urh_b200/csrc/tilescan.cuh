@@ -1,12 +1,13 @@
-// Single-launch scan over a table with one element per TILE (decoupled look-back), for any associative — not
-// necessarily commutative — operator.  The tables scanned here have n/2048 entries (the run-carry, candidate and
-// firing summaries of the dense pass's tiles), so one launch of a few hundred blocks replaces the
-// reduce / scan-of-aggregates / apply triple of scan.cuh and, with the `post` hook, the element-wise kernels
-// around it.
+// Single-launch exclusive scan over a device table (decoupled look-back), for any associative — not necessarily
+// commutative — operator; the library's one device-wide scan.  Most tables have one entry per TILE (the run-carry,
+// candidate, firing and kept-count summaries of the dense pass's tiles); others have one per pulse row or per sample
+// (ppseq_to_bits, detect_modulation's compaction).  The `load` and `post` hooks fold the element-wise kernels that
+// would produce a scan's input or consume its output into the scan itself.  `post` may write the table `load` reads:
+// a thread loads all its elements before it posts any, and no other thread touches them.
 //
 //   F::load(i)                  -> element i (computed on the fly from other tables)
 //   F::post(i, excl, elem)      called for every i < n with its EXCLUSIVE prefix (identity for i == 0)
-//   *d_total (optional)         the reduction of all elements
+//   *d_total (optional)         the reduction of all elements (n <= 0: nothing is launched or written)
 //
 // Blocks take their chunk index from a monotonic counter in arrival order, so a block only ever waits for blocks
 // that are already running (forward progress without co-residency assumptions).  The per-block status words carry
@@ -171,8 +172,13 @@ __global__ void __launch_bounds__(BLOCK) k_scan(int64_t n, T identity, Op op, F 
     }
 }
 
-// host side (context.cu): workspace for `nblocks` blocks of the next launch
+// host side (context.cu): workspace for `nblocks` blocks of the next launch.  The workspace starts at 8192 blocks (a table of
+// 2^25 elements at ITEMS = 16, 2^24 at 8); a larger launch grows it once, which synchronises the context stream and reallocates.
 int prepare(urh_ctx* ctx, int64_t nblocks, Ws* out);
+
+struct AddI64 {
+    __device__ __forceinline__ int64_t operator()(int64_t a, int64_t b) const { return a + b; }
+};
 
 template <typename T, typename Op, typename F, int ITEMS = 16>
 static inline int scan(urh_ctx* ctx, int64_t n, T identity, Op op, F f, T* d_total) {
