@@ -476,6 +476,16 @@ int64_t urh_costas_last_redone(urh_ctx* ctx);
 int urh_costas_stitch_stats(urh_ctx* ctx, int64_t* h_out4);
 /* paired (float2) division used by the FSK fast path vs __fdiv_rn on `count` random operand pairs */
 int urh_selftest_packed_div(urh_ctx* ctx, uint64_t seed, int64_t count, int64_t* mismatches, int64_t* tested);
+/* test entry point of the look-back scan (tilescan.cuh): d_excl[i] = exclusive prefix of d_in[0:n] (d_excl may be d_in),
+ * d_elem[i] = d_in[i] as the scan loaded it (NULL: not written), *d_total = the reduction (NULL: not written; n <= 0: nothing is
+ * launched).  op 0: int64 sum; 1: RunCarry {int64 len, int32 cls, int32 flags} under RunCarryOp (sparse.cuh); 2: 2x2 uint64
+ * matrix (row-major, 32 bytes) product mod 2^64.  items: 4, 8 or 16 elements per thread (a scan block covers 256 * items).
+ * delay_chunk >= 0: that scan block waits (bounded, at most about 2 ms) for the next 33 blocks to publish their aggregates, then
+ * spins about 50 us before loading, so the blocks after it take the look-back path past it; *d_held (NULL: not written) = 1 if
+ * all of those blocks had published while it waited (the 33rd then went on to a second look-back round), 0 if not.  Enqueues the
+ * scan on the context stream and returns without synchronising. */
+int urh_selftest_scan(urh_ctx* ctx, int op, int items, const void* d_in, int64_t n, void* d_excl, void* d_elem, void* d_total,
+                      int64_t delay_chunk, int* d_held);
 /* synthetic phase-continuous 2-FSK bursts + AWGN + noise-only gaps generated in HBM (SURVEY 8d recipe) */
 int urh_synth_fsk(urh_ctx* ctx, float* d_iq, int64_t n, int64_t global_offset, int sps, const int8_t* d_sym_bit,
                   const int32_t* d_sym_sum, double dev_ratio, float amplitude, float sigma, uint64_t seed,

@@ -13,10 +13,13 @@ def _oracle_ppseq_to_bits(*a, **k):
 
 
 def model(rows, sps, bps, pt):
+    """the restatement in flat arrays, as urh_fetch_bits returns them: (bits uint8[B], msg_off int64[M+1], pauses int64[M],
+    pos int64[P]); message m is bits[msg_off[m]:msg_off[m+1]] with positions pos[msg_off[m] + 2m : msg_off[m+1] + 2m + 2]
+    (one fewer for a last message that no pause row closes).  Loop-free, so it serves tables of millions of rows."""
     rows = np.asarray(rows, np.int64).reshape(-1, 2)
     k = len(rows)
     if k == 0:
-        return [], [], []
+        return np.zeros(0, np.uint8), np.zeros(1, np.int64), np.zeros(0, np.int64), np.zeros(0, np.int64)
     kind, ns = rows[:, 0], rows[:, 1]
     first = 1 if kind[0] == -1 else 0
     f = ns / float(sps)
@@ -43,28 +46,33 @@ def model(rows, sps, bps, pt):
     msg_off = np.zeros(M + 1, np.int64)
     pauses = np.zeros(M, np.int64)
     pos = np.zeros(B + 2 * M, np.int64)
-    for i in np.nonzero(long_)[0]:
-        if seg_has[seg[i]]:
-            m = seg_msg[seg[i]]
-            msg_off[m + 1] = bitoff[i]
-            pauses[m] = ns[i]
-            pos[bitoff[i] + 2 * m] = total[i]
-            pos[bitoff[i] + 2 * m + 1] = total[i] + ns[i]
+    # a long pause closes its segment's message
+    i = np.nonzero(long_ & (seg_has[seg] == 1))[0]
+    m = seg_msg[seg[i]]
+    msg_off[m + 1] = bitoff[i]
+    pauses[m] = ns[i]
+    pos[bitoff[i] + 2 * m] = total[i]
+    pos[bitoff[i] + 2 * m + 1] = total[i] + ns[i]
     if final_open:
         msg_off[M] = B
         pauses[M - 1] = ns[-1] if kind[-1] == -1 else 0
         pos[B + 2 * (M - 1)] = total[k]
-    bits = np.zeros(B, np.uint8)
+    # every bit: its row, its index inside the row, the row's symbol digits MSB first
+    r = np.repeat(idx, eff)
+    b = np.arange(B, dtype=np.int64) - bitoff[r]
+    bits = np.where(data[r], (kind[r] >> (bps - 1 - b % bps)) & 1, 0).astype(np.uint8)
     spb = int(sps / bps)
-    for g in range(B):
-        i = int(np.searchsorted(bitoff[:k], g, side="right")) - 1
-        b = g - bitoff[i]
-        if data[i]:
-            bits[g] = (kind[i] >> (bps - 1 - b % bps)) & 1
-        pos[g + 2 * seg_msg[seg[i]]] = total[i] + b * spb
+    pos[np.arange(B, dtype=np.int64) + 2 * seg_msg[seg[r]]] = total[r] + b * spb
     P = B + 2 * M - (1 if final_open else 0)
+    return bits, msg_off, pauses, pos[:P]
+
+
+def as_messages(flat):
+    """model()'s flat arrays -> per-message lists, the shape the sequential port returns"""
+    bits, msg_off, pauses, pos = flat
+    M = len(pauses)
     out_bits = [bits[msg_off[m]:msg_off[m + 1]].tolist() for m in range(M)]
-    out_pos = [pos[msg_off[m] + 2 * m: min(msg_off[m + 1] + 2 * m + 2, P)].tolist() for m in range(M)]
+    out_pos = [pos[msg_off[m] + 2 * m: min(msg_off[m + 1] + 2 * m + 2, len(pos))].tolist() for m in range(M)]
     return out_bits, pauses.tolist(), out_pos
 
 
@@ -79,7 +87,7 @@ def test_model_equals_sequential_port():
         ns = np.where(rng.random(k) < 0.15, rng.integers(9, 30, k) * sps, rng.integers(0, 5 * sps + 1, k))
         rows = np.stack([kinds, ns], axis=1).astype(np.int64)
         hb, hp, hpos = _oracle_ppseq_to_bits(rows, sps, bps, pause_threshold=pt)
-        mb, mp, mpos = model(rows, sps, bps, pt)
+        mb, mp, mpos = as_messages(model(rows, sps, bps, pt))
         assert [list(x) for x in hb] == mb, (trial, rows.tolist())
         assert list(hp) == mp, (trial, rows.tolist())
         assert [list(x) for x in hpos] == mpos, (trial, rows.tolist())

@@ -127,7 +127,7 @@ def test_demod_detect_center_matches_two_step_golden(AI, name):
         assert float(exact) == gc
 
 
-@pytest.mark.parametrize("n", [3, 2047, 2048, 2049, 70001, 1 << 20])
+@pytest.mark.parametrize("n", [3, 2047, 2048, 2049, 70001, 1 << 20, 2 * 4096 * 2048 + 4097])
 @pytest.mark.parametrize("max_size", [None, 5000])
 def test_demod_detect_center_sizes(AI, n, max_size):
     from urh_b200.cythonext import signal_functions as sf

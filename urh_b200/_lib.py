@@ -154,6 +154,7 @@ SIGNATURES = {
     "urh_costas_last_redone": (i64, [vp]),
     "urh_costas_stitch_stats": (i32, [vp, vp]),
     "urh_selftest_packed_div": (i32, [vp, C.c_uint64, i64, C.POINTER(i64), C.POINTER(i64)]),
+    "urh_selftest_scan": (i32, [vp, i32, i32, vp, i64, vp, vp, vp, i64, vp]),
     "urh_bgra_lookup": (i32, [vp, vp, i64, i64, vp, i32, f32, f32, i32, vp]),
     "urh_spectrogram_bgra": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, f32, f32, i32, vp]),
     "urh_gather_samples": (i32, [vp, vp, i64, i64, i64, i64, vp]),
