@@ -118,7 +118,7 @@ def main():
                 ref = Filter.dc_correction(xd)
             if not same(got, ref):
                 failures.append(("dc", nd, np.dtype(dtype).name))
-    # ---- dB map: radix-16 1024/512, 256 at overlap 0.75, cuFFT-composed 1000/500; shard edges not multiples of hop
+    # ---- dB map: k_stft_r16 at 1024 / 512 and at 256 with overlap 0.75, cuFFT-composed 1000 / 500; shard edges not multiples of hop
     for W, overlap in [(1024, 0.5), (256, 0.75), (1000, 0.5)]:
         first, db = udist.spectrogram_db_sharded(ctx, hx, sb, bounds, W, overlap)
         firsts = hx.allgather(first)

@@ -2,12 +2,12 @@
 the same operation (oracle/oracle.py, numpy), at the sizes where the dispatch switches and the kernels' tiles end.
 
 Paths (DESIGN 4.5 / 4.6):
-  STFT     W = 256 / 1024 / 4096: k_stft_r16;  other powers of two 128 .. 4096 (or $URH_B200_STFT_RADIX4): k_stft_fused;
-           everything else (or $URH_B200_STFT_CUFFT): k_stft_window -> cuFFT Z2Z -> k_stft_scale / k_stft_db, in 512 MiB batches
+  STFT     powers of two 128 .. 4096: k_stft_r16 (radix-16 passes + one radix-2 / 4 / 8 pass);
+           everything else: k_stft_window -> cuFFT Z2Z -> k_stft_scale / k_stft_db, in 512 MiB batches
   band-pass  m <= 768 taps: k_conv_c128_tiled;  more: k_conv_c128
   DC       n <= Filter.EXACT_DC_MAX: k_dc_mean_serial (numpy's float32 chain);  more: k_dc_mean_partial + k_dc_mean_fold (double)
 
-Run with -s to see the largest error each path showed."""
+Run with -s to see the largest error each path showed (the STFT and dB map per window size)."""
 import numpy as np
 import pytest
 
@@ -17,7 +17,6 @@ pytestmark = pytest.mark.gpu
 
 STFT_SIZES = [64, 128, 256, 512, 1000, 1001, 1024, 2048, 3000, 4096, 8192]
 OVERLAPS = [0, 0.5, 0.75, 0.3]
-PATH_ENV = {"default": {}, "radix4": {"URH_B200_STFT_RADIX4": "1"}, "cufft": {"URH_B200_STFT_CUFFT": "1"}}
 STFT_REL = 1e-12    # per frame: max|got - ref| <= STFT_REL * max|ref frame|   (a double FFT is ~1e-15; float twiddles ~3e-8)
 DB_ABS = 1e-3       # dB, in every bin within DB_RANGE of its frame's peak (DESIGN 4.6)
 DB_RANGE = 150.0
@@ -44,22 +43,8 @@ def asymmetric(w):
 WINDOWS = {"hanning": np.hanning, "asymmetric": asymmetric}
 
 
-def stft_paths(W):
-    """the override variables matter only where the fused kernels serve W"""
-    return ["default", "radix4", "cufft"] if (W & (W - 1)) == 0 and 128 <= W <= 4096 else ["default"]
-
-
-def stft_kernel(W, path):
-    if path == "cufft" or (W & (W - 1)) or not 128 <= W <= 4096:
-        return "cufft"
-    return "k_stft_r16" if path == "default" and W in (256, 1024, 4096) else "k_stft_fused"
-
-
-def use_path(monkeypatch, path):
-    for var in ("URH_B200_STFT_RADIX4", "URH_B200_STFT_CUFFT"):
-        monkeypatch.delenv(var, raising=False)
-    for var, value in PATH_ENV[path].items():
-        monkeypatch.setenv(var, value)   # read by getenv() on every call (spectrogram.cu)
+def stft_kernel(W):
+    return "k_stft_r16" if (W & (W - 1)) == 0 and 128 <= W <= 4096 else "cufft"
 
 
 def lengths(W, hop):
@@ -87,7 +72,7 @@ def check_stft(got, ref, key):
     assert len(bad) == 0, (key, "frames", bad[:8], err[bad[:8]], peak[bad[:8]])
     nz = peak > 0
     if nz.any():
-        _record("stft rel err  " + key[0], (err[nz] / peak[nz]).max())
+        _record("stft rel err  %s W=%d" % key[:2], (err[nz] / peak[nz]).max())
 
 
 def check_db(got, ref, key):
@@ -108,15 +93,14 @@ def check_db(got, ref, key):
     inf_ok = np.isneginf(g) | (g < floor)
     assert np.all(inf_ok | ~np.isneginf(r)), (key, "-inf in the reference", np.argwhere(~(inf_ok | ~np.isneginf(r)))[:8])
     if strong.any():
-        _record("dB |delta|    " + key[0], d.max())
+        _record("dB |delta|    %s W=%d" % key[:2], d.max())
 
 
 # ---- 1. STFT (complex128) ----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("window", sorted(WINDOWS))
 @pytest.mark.parametrize("W", STFT_SIZES)
-def test_stft_matches_float64_reference(oracle, monkeypatch, W, window):
-    """Spectrogram.stft on every kernel that serves W == oracle.stft (complex128, not rounded) to STFT_REL per frame; the
-    kernels agree with one another to the same bar"""
+def test_stft_matches_float64_reference(oracle, W, window):
+    """Spectrogram.stft on the kernel that serves W == oracle.stft (complex128, not rounded) to STFT_REL per frame"""
     from urh_b200.signalprocessing.Spectrogram import Spectrogram
 
     wf = WINDOWS[window]
@@ -125,21 +109,14 @@ def test_stft_matches_float64_reference(oracle, monkeypatch, W, window):
         for n in lengths(W, hop):
             x = capture(n, W)
             ref = oracle.stft(x, W, ov, wf)
-            outs = {}
-            for path in stft_paths(W):
-                use_path(monkeypatch, path)
-                outs[path] = Spectrogram(x, W, ov, wf).stft(x)
-                check_stft(outs[path], ref, (stft_kernel(W, path), W, ov, n, window))
-            peak = np.abs(ref).max(axis=1, keepdims=True)
-            for path, got in outs.items():
-                assert np.all(np.abs(got - outs["default"]) <= STFT_REL * peak), ("paths disagree", path, W, ov, n, window)
+            check_stft(Spectrogram(x, W, ov, wf).stft(x), ref, (stft_kernel(W), W, ov, n, window))
 
 
 # ---- 2. dB map (float32) -----------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("window", sorted(WINDOWS))
 @pytest.mark.parametrize("W", STFT_SIZES)
-def test_spectrogram_db_matches_float64_reference(oracle, monkeypatch, W, window):
-    """Spectrogram.calculate_spectrogram (fftshift, complex64 cast, dB, fliplr) on every kernel that serves W == oracle.spectrogram_db
+def test_spectrogram_db_matches_float64_reference(oracle, W, window):
+    """Spectrogram.calculate_spectrogram (fftshift, complex64 cast, dB, fliplr) on the kernel that serves W == oracle.spectrogram_db
     (check_db); odd W on cuFFT exercises k_stft_db's fftshift, the only place where it differs from W / 2"""
     from urh_b200.signalprocessing.Spectrogram import Spectrogram
 
@@ -149,16 +126,12 @@ def test_spectrogram_db_matches_float64_reference(oracle, monkeypatch, W, window
         for n in lengths(W, hop):
             x = capture(n, W)
             ref = oracle.spectrogram_db(x, W, ov, window_function=wf)
-            for path in stft_paths(W):
-                use_path(monkeypatch, path)
-                check_db(Spectrogram(x, W, ov, wf).calculate_spectrogram(), ref, (stft_kernel(W, path), W, ov, n, window))
+            check_db(Spectrogram(x, W, ov, wf).calculate_spectrogram(), ref, (stft_kernel(W), W, ov, n, window))
         zeros = np.zeros(W + 5 * hop, np.complex64)
         ref = oracle.spectrogram_db(zeros, W, ov, window_function=wf)
         assert np.all(np.isneginf(ref))
-        for path in stft_paths(W):
-            use_path(monkeypatch, path)
-            got = Spectrogram(zeros, W, ov, wf).calculate_spectrogram()
-            assert got.shape == ref.shape and np.all(np.isneginf(got)), (path, W, ov)
+        got = Spectrogram(zeros, W, ov, wf).calculate_spectrogram()
+        assert got.shape == ref.shape and np.all(np.isneginf(got)), (W, ov)
 
 
 # ---- 3. cuFFT batching and the plan cache ------------------------------------------------------------------------------------
@@ -168,13 +141,12 @@ def frame_db(oracle, x, W, hop, f, window):
     return np.fliplr(oracle.arr2decibel(np.fft.fftshift(X)[None].astype(np.complex64)))
 
 
-def test_spectrogram_cufft_batches_and_plan_cache(oracle, monkeypatch):
+def test_spectrogram_cufft_batches_and_plan_cache(oracle):
     """W = 5000 (cuFFT), hop 2500: 6710 frames fill one 512 MiB batch, 6717 frames leave a last batch of 7 (ensure_plan rebuilds
     the plan).  Frames on either side of the batch boundary match the reference; a call of the last batch's 7 frames reuses the
     cached plan and repeats them bit for bit; after a call of another frame count rebuilt the plan, so does the first call"""
     from urh_b200.signalprocessing.Spectrogram import Spectrogram
 
-    use_path(monkeypatch, "default")
     W, ov = 5000, 0.5
     hop = W - int(ov * W)
     max_batch = (512 << 20) // (W * 16)
@@ -190,13 +162,13 @@ def test_spectrogram_cufft_batches_and_plan_cache(oracle, monkeypatch):
     first = spec.calculate_spectrogram(x)
     assert first.shape == (frames, W)
     for f in (0, max_batch - 1, max_batch, max_batch + 1, frames - 1):
-        check_db(first[f:f + 1], frame_db(oracle, x, W, hop, f, window), ("cufft batched", f))
+        check_db(first[f:f + 1], frame_db(oracle, x, W, hop, f, window), ("cufft batched", W, f))
     tail = spec.calculate_spectrogram(x[max_batch * hop: max_batch * hop + W + 6 * hop])   # the last batch's frames, same plan
     assert tail.shape == (7, W) and bits_equal(tail, first[max_batch:]) == 0
     other = spec.calculate_spectrogram(x[: W + 99 * hop])   # 100 frames: plan rebuilt
     assert other.shape == (100, W)
     for f in (0, 99):
-        check_db(other[f:f + 1], frame_db(oracle, x, W, hop, f, window), ("cufft batched", f))
+        check_db(other[f:f + 1], frame_db(oracle, x, W, hop, f, window), ("cufft batched", W, f))
     again = spec.calculate_spectrogram(x)
     assert bits_equal(again, first) == 0
 

@@ -1,8 +1,8 @@
 """GPU: spectrogram images (urh_spectrogram_bgra: STFT -> dB -> colormap in one launch for every segment) and the streamed FTA
 export (urh_fta_records), against the two device stages they fuse, the reference's own Spectrogram class and the FTA restatement.
 
-Paths (DESIGN 4.6): W = 256 / 1024 / 4096: k_stft_r16 mode 2;  other powers of two 128 .. 4096 (or $URH_B200_STFT_RADIX4):
-k_stft_fused mode 2;  everything else: urh_spectrogram_db's kernels + k_bgra_place (composed)."""
+Paths (DESIGN 4.6): powers of two 128 .. 4096: k_stft_r16 mode 2;  everything else: urh_spectrogram_db's kernels + k_bgra_place
+(composed)."""
 import ctypes as C
 import os
 
@@ -16,13 +16,6 @@ pytestmark = pytest.mark.gpu
 OVERLAPS = [0, 0.3, 0.5, 0.75]
 RANGES = [(-140, 10), (-80, 10), (-60, -60)]
 WINDOW_SIZES = [128, 256, 512, 1024, 2048, 4096, 1000, 1001]
-
-
-def use_path(monkeypatch, path):
-    for var in ("URH_B200_STFT_RADIX4", "URH_B200_STFT_CUFFT"):
-        monkeypatch.delenv(var, raising=False)
-    if path == "radix4":
-        monkeypatch.setenv("URH_B200_STFT_RADIX4", "1")
 
 
 def colormap(entries, seed=0):
@@ -62,17 +55,16 @@ def composed(spec, x, transpose, cmap):
 
 
 @pytest.mark.parametrize("W", WINDOW_SIZES)
-def test_fused_image_equals_db_map_then_lookup(monkeypatch, W):
-    """create_spectrogram_image == urh_bgra_lookup(urh_spectrogram_db(...)) bit for bit on every kernel that serves W, every overlap,
+def test_fused_image_equals_db_map_then_lookup(W):
+    """create_spectrogram_image == urh_bgra_lookup(urh_spectrogram_db(...)) bit for bit on the kernel that serves W, every overlap,
     1 .. ~20 frames (n < W included), both layouts, three (min, max) ranges (one with min = max) and colormaps of 256 / 1024 (shared
     memory) and 1025 (global memory) entries; each length includes frames of zeros once it is long enough"""
     from urh_b200.signalprocessing.Spectrogram import Spectrogram
 
-    paths = ["default", "radix4"] if (W & (W - 1)) == 0 else ["default"]
+    paths = ["default"]
     combos = [(t, r, L) for t in (False, True) for r in RANGES for L in CMAPS]
     k = 0
     for path in paths:
-        use_path(monkeypatch, path)
         for ov in OVERLAPS:
             hop = W - int(ov * W)
             ns = lengths(W, hop)

@@ -86,7 +86,7 @@ def main():
     total = ms_fir + ms_demod + ms_spec
     print(json.dumps({"config": "configs[2]: ASK capture -> 101-tap band-pass -> ASK demod -> STFT(1024, hop 512) dB", "samples": n2,
                       "ms": {"band-pass (complex128 taps, double accumulation)": ms_fir, "afp_demod ASK": ms_demod,
-                             "spectrogram dB (cuFFT Z2Z)": ms_spec, "total": total},
+                             "spectrogram dB (k_stft_r16)": ms_spec, "total": total},
                       "MSamples_per_s": n2 / total / 1e3, "envelope_matches_bits": ok2}), flush=True)
     del d_cap, d_filt, d_qad, d_db
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Spectrogram STFT -> dB (W = 1024, hop 512): the fused shared-memory-FFT kernel against the cuFFT path (URH_B200_STFT_CUFFT=1),
-and their agreement; create_image_segments, fused image kernel against the composed dB map + look-up; FTA record generation and
-export.   python tools/bench_stft.py [--log2n 28]"""
+"""Spectrogram at 2^log2n samples, hop W/2, for each window size W: the dB map (urh_spectrogram_db) and the images of every
+create_image_segments segment in one call (urh_spectrogram_bgra), CUDA events; FTA record generation and export.
+   python tools/bench_stft.py [--log2n 28] [--windows 128 256 512 1024 2048 4096]"""
 import argparse
 import ctypes as C
 import json
@@ -18,6 +18,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--log2n", type=int, default=28)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--windows", type=int, nargs="+", default=[128, 256, 512, 1024, 2048, 4096])
     args = ap.parse_args()
     from urh_b200 import _lib
     from urh_b200.device import DeviceArray, to_device
@@ -33,39 +34,26 @@ def main():
     d_c = to_device(chunk, ctx)
     for i in range(n >> 20):
         ctx.check(lib.urh_memcpy_d2d(ctx.handle, C.c_void_p(d_x.ptr + i * chunk.nbytes), C.c_void_p(d_c.ptr), chunk.nbytes))
-    W, hop = 1024, 512
-    frames = (n - W) // hop + 1
-    d_w = to_device(np.hanning(W), ctx)
-    out = {}
-    res = {}
-    for name, env in (("fused", None), ("cufft", "1")):
-        if env:
-            os.environ["URH_B200_STFT_CUFFT"] = env
-        else:
-            os.environ.pop("URH_B200_STFT_CUFFT", None)
-        d_db = DeviceArray(ctx, (frames, W), np.float32)
-        ms = []
-        for rep in range(args.reps + 1):
-            ctx.timer_start()
-            ctx.check(lib.urh_spectrogram_db(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr), frames, C.c_void_p(d_db.ptr)))
-            t = ctx.timer_stop()
-            if rep:
-                ms.append(t)
-        out[name + "_ms"] = float(np.median(ms))
-        res[name] = d_db[:4096].get()
-        d_db.free()
-    peak = res["cufft"].max()
-    mask = res["cufft"] > peak - 100
-    out["max_abs_dB_diff_within_100dB_of_peak"] = float(np.abs(res["fused"] - res["cufft"])[mask].max())
-    out["samples"] = n
-    out["algorithmic_GBps_fused"] = 16.0 * n / out["fused_ms"] / 1e6
-    os.environ.pop("URH_B200_STFT_CUFFT", None)
-    out.update(bench_images(ctx, d_x, n, W, hop, d_w, args.reps))
+    out = {"samples": n}
+    for W in args.windows:
+        out.update(bench_window(ctx, d_x, n, W, args.reps))
     out.update(bench_fta(ctx, args.reps))
     info = ctx.device_info()
     out["device"] = info["name"]
     out["power_limit_W"] = power_limit()
     print(json.dumps(out))
+
+
+def timed(ctx, reps, call):
+    """median over reps calls, after one warm-up call, of the CUDA-event time of call()"""
+    ms = []
+    for rep in range(reps + 1):
+        ctx.timer_start()
+        call()
+        t = ctx.timer_stop()
+        if rep:
+            ms.append(t)
+    return float(np.median(ms))
 
 
 def power_limit():
@@ -79,46 +67,34 @@ def power_limit():
         return None
 
 
-def bench_images(ctx, d_x, n, W, hop, d_w, reps):
-    """create_image_segments at n samples: the fused image kernel (one launch for every segment) against the composed stages
-    (urh_spectrogram_db then urh_bgra_lookup, per segment, as the reference's generator calls them), CUDA events"""
+def bench_window(ctx, d_x, n, W, reps):
+    """at window size W, hop W/2: the dB map of every frame, and the images of create_image_segments' segments in one call (256
+    colormap entries, (min, max) = (-140, 10), the scene view's layout)"""
     from urh_b200.device import DeviceArray, to_device
     from urh_b200.signalprocessing.Spectrogram import Spectrogram
 
     lib = ctx.lib
-    spec = Spectrogram(d_x, W, 0.5)
-    bounds = spec.segment_bounds()
+    hop = W // 2
+    frames = (n - W) // hop + 1
+    d_w = to_device(np.hanning(W), ctx)
+    d_db = DeviceArray(ctx, (frames, W), np.float32)
+    db_ms = timed(ctx, reps, lambda: ctx.check(lib.urh_spectrogram_db(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr),
+                                                                      frames, C.c_void_p(d_db.ptr))))
+    d_db.free()
+    bounds = Spectrogram.segment_bounds_of(n, W, hop)
     cmap = np.zeros((256, 4), np.uint8)
     cmap[:, 0] = np.arange(256)
     d_map = to_device(cmap, ctx)
     starts = np.array([s for s, _, _ in bounds], np.int64)
     lens = np.array([e - s for s, e, _ in bounds], np.int64)
-    pixels = sum(f for _, _, f in bounds) * W
-    d_img = DeviceArray(ctx, (pixels * 4,), np.uint8)
-    max_f = max(f for _, _, f in bounds)
-    d_db = DeviceArray(ctx, (max_f, W), np.float32)
-    res = {"fused": [], "composed": []}
-    for rep in range(reps + 1):
-        ctx.timer_start()
-        ctx.check(lib.urh_spectrogram_bgra(ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr), starts.ctypes.data_as(C.c_void_p),
-                                           lens.ctypes.data_as(C.c_void_p), len(bounds), C.c_void_p(d_map.ptr), 256, -140.0, 10.0, 0,
-                                           C.c_void_p(d_img.ptr)))
-        t_fused = ctx.timer_stop()
-        ctx.timer_start()
-        off = 0
-        for s, e, f in bounds:
-            ctx.check(lib.urh_spectrogram_db(ctx.handle, C.c_void_p(d_x.ptr + 8 * s), e - s, W, hop, C.c_void_p(d_w.ptr), f, C.c_void_p(d_db.ptr)))
-            ctx.check(lib.urh_bgra_lookup(ctx.handle, C.c_void_p(d_db.ptr), f, W, C.c_void_p(d_map.ptr), 256, -140.0, 10.0, 1,
-                                          C.c_void_p(d_img.ptr + off)))
-            off += f * W * 4
-        t_comp = ctx.timer_stop()
-        if rep:
-            res["fused"].append(t_fused)
-            res["composed"].append(t_comp)
-    out = {"image_segments": len(bounds), "image_fused_ms": float(np.median(res["fused"])),
-           "image_composed_ms": float(np.median(res["composed"]))}
-    out["image_fused_GBps_8B_per_sample"] = 8.0 * n / out["image_fused_ms"] / 1e6
-    return out
+    d_img = DeviceArray(ctx, (sum(f for _, _, f in bounds) * W * 4,), np.uint8)
+    image_ms = timed(ctx, reps, lambda: ctx.check(lib.urh_spectrogram_bgra(
+        ctx.handle, C.c_void_p(d_x.ptr), n, W, hop, C.c_void_p(d_w.ptr), starts.ctypes.data_as(C.c_void_p),
+        lens.ctypes.data_as(C.c_void_p), len(bounds), C.c_void_p(d_map.ptr), 256, -140.0, 10.0, 0, C.c_void_p(d_img.ptr))))
+    d_img.free()
+    k = "W%d_" % W
+    return {k + "db_ms": db_ms, k + "db_GBps_16B_per_sample": 16.0 * n / db_ms / 1e6, k + "image_segments": len(bounds),
+            k + "image_ms": image_ms, k + "image_GBps_8B_per_sample": 8.0 * n / image_ms / 1e6}
 
 
 def bench_fta(ctx, reps, log2n=23, sample_rate=2e6):

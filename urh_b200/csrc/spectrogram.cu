@@ -3,16 +3,15 @@
 //
 // The reference multiplies complex frames by np.hanning in float64 and runs numpy's complex128 FFT, then casts
 // to complex64 and takes 10*log10f(|X|^2) in float32.  To keep the weak bins (down to ~-100 dB below the peak)
-// within the stated 1e-3 dB, the FFT is done in double.  Power-of-two windows (URH's: 1024) take ONE fused kernel (window ->
-// shared-memory FFT -> scale / fftshift / cast / dB / flip, see k_stft_fused); other sizes use cuFFT Z2Z — for the FFT only, as
-// the north_star prescribes — between two hand-written kernels, in batches that bound the working set.
+// within the stated 1e-3 dB, the FFT is done in double.  Power-of-two windows of 128 .. 4096 points (URH's: 1024) take ONE fused
+// kernel (window -> shared-memory FFT -> scale / fftshift / cast / dB / flip, see k_stft_r16); other sizes use cuFFT Z2Z — for the
+// FFT only, as the north_star prescribes — between two hand-written kernels, in batches that bound the working set.
 #include "common.cuh"
 #include "stream_ring.cuh"
 
 #include <cufft.h>
 #include <limits.h>
 #include <math.h>
-#include <stdlib.h>
 
 #include <algorithm>
 
@@ -73,11 +72,11 @@ __global__ void k_stft_db(const double2* __restrict__ X, int W, int64_t nframes,
     }
 }
 
-// ---- fused path (power-of-two windows): window -> FFT in shared memory -> scale / fftshift / dB, one block per frame ----------
+// ---- fused path (power-of-two windows): window -> FFT in shared memory -> scale / fftshift / dB, W / 16 threads per frame ------
 // The cuFFT path above moves every frame through HBM three times as complex128 (window kernel -> Z2Z -> dB kernel: 36 GB for
 // 2^28 samples at W = 1024, hop = 512).  Here a frame is read once as complex64 (the 50 % overlap with its neighbour comes from
-// L2), transformed in double in shared memory (Stockham autosort, radix-4 stages + one radix-2 stage when log2 W is odd) and
-// written once as float32 dB (or complex128 for urh_stft): 8 + 8 B/sample at the reference's parameters.
+// L2), transformed in double in shared memory (Stockham autosort, radix-16 passes + one radix-2 / 4 / 8 pass, see k_stft_r16)
+// and written once as float32 dB (or complex128 for urh_stft): 8 + 8 B/sample at the reference's parameters.
 // tw[q] = exp(-2 pi i q / W), q < W, built once per window size with sincospi (double).
 __global__ void k_fft_twiddles(int W, double2* __restrict__ tw) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -105,6 +104,13 @@ __device__ __forceinline__ double2 cmul(double2 a, double2 b) {
 //                  computed, coalesced.
 // padded shared-memory index of the radix-16 kernel (one element every 16; see k_stft_r16)
 __device__ __forceinline__ int stft_pad(int i) { return i + (i >> 4); }
+// k_stft_r16 runs W / 16 threads per frame; its blocks hold several frames where that is less than a warp (W = 128, 256)
+constexpr int stft_frames(int W) { return W / 16 >= 32 ? 1 : 32 / (W / 16); }
+// the thread's frame within its block, and its lane among that frame's W / 16 threads
+template <int W>
+__device__ __forceinline__ int stft_group() { return stft_frames(W) > 1 ? (int)(threadIdx.x / (W / 16)) : 0; }
+template <int W>
+__device__ __forceinline__ int stft_lane() { return stft_frames(W) > 1 ? (int)(threadIdx.x % (W / 16)) : (int)threadIdx.x; }
 constexpr int STFT_IMG_FPB = 8;
 struct StftImage {
     const int64_t* seg;
@@ -124,11 +130,12 @@ __device__ __forceinline__ int bgra_index(float v, float data_min, float range, 
     return (int)k;
 }
 
-// fft(base, end) runs one frame's FFT (samples base .. base + W - 1, zeros at and past end) and returns the buffer holding X, the
-// stride of which PAD says (stft_pad or none); `tail` is the shared memory after the FFT buffers
-template <int W, int NT, bool PAD, typename Fft>
+// fft(base, end) runs the FFT of the thread's frame (samples base .. base + W - 1, zeros at and past end) and returns the (padded)
+// buffer holding X; `tail` is the shared memory after the FFT buffers
+template <int W, typename Fft>
 __device__ __forceinline__ void stft_image_block(const StftImage& img, int hop, Fft fft, unsigned char* tail, uint32_t* __restrict__ out) {
     constexpr int FPB = STFT_IMG_FPB;
+    constexpr int T = W / 16, G = stft_frames(W), NT = G * T;
     const int64_t blk = blockIdx.x;
     int lo = 0, hi = img.nseg - 1;   // the last segment whose first block is <= blk
     while (lo < hi) {
@@ -151,19 +158,22 @@ __device__ __forceinline__ void stft_image_block(const StftImage& img, int hop, 
     const float scale = (float)(img.entries - 1);
     constexpr int shift = (W + 1) / 2;
     const double inv = 1.0 / (double)W;
-    for (int k = 0; k < nf; k++) {
+    for (int k0 = 0; k0 < nf; k0 += G) {   // G frames at a time, one per group of T threads
+        const int k = k0 + stft_group<W>();  // k >= nf (the last block of a segment): transformed, not written
         const double2* a = fft(start + (f0 + k) * hop, end);
-        for (int r = threadIdx.x; r < W; r += NT) {
-            const int j = img.transpose ? W - 1 - r : r;            // dB column (fliplr order)
-            const int src = ((W - 1 - j) + shift) & (W - 1);        // fliplr, then fftshift
-            const double2 v = a[PAD ? stft_pad(src) : src];
-            const float re = (float)(v.x * inv), im = (float)(v.y * inv);
-            const float db = __fmul_rn(10.0f, log10f(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im))));
-            const int idx = bgra_index(db, img.data_min, img.range, scale, img.entries, 1);
-            if (img.transpose) o[(f0 + k) * W + r] = map[idx];
-            else s_idx[r * FPB + k] = (uint16_t)idx;
+        if (G == 1 || k < nf) {
+            for (int r = stft_lane<W>(); r < W; r += T) {
+                const int j = img.transpose ? W - 1 - r : r;            // dB column (fliplr order)
+                const int src = ((W - 1 - j) + shift) & (W - 1);        // fliplr, then fftshift
+                const double2 v = a[stft_pad(src)];
+                const float re = (float)(v.x * inv), im = (float)(v.y * inv);
+                const float db = __fmul_rn(10.0f, log10f(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im))));
+                const int idx = bgra_index(db, img.data_min, img.range, scale, img.entries, 1);
+                if (img.transpose) o[(f0 + k) * W + r] = map[idx];
+                else s_idx[r * FPB + k] = (uint16_t)idx;
+            }
         }
-        __syncthreads();   // the next frame's load overwrites the FFT buffers
+        __syncthreads();   // the next frames' loads overwrite the FFT buffers
     }
     if (!img.transpose) {
         for (int t = threadIdx.x; t < W * FPB; t += NT) {
@@ -173,119 +183,12 @@ __device__ __forceinline__ void stft_image_block(const StftImage& img, int hop, 
     }
 }
 
-// frame at x[base ..], samples at and past n are zeros: window -> Stockham FFT; returns the buffer holding X (natural order)
-template <int LOG2W, int THREADS>
-__device__ __forceinline__ const double2* stft_fused_fft(const float2* __restrict__ x, int64_t n, int64_t base,
-                                                         const double* __restrict__ window, const double2* __restrict__ tw,
-                                                         double2* s_buf) {
-    constexpr int W = 1 << LOG2W;
-    constexpr int PER = W / THREADS;          // elements per thread in the load / store phases
-    constexpr int BPT = (W / 4) / THREADS > 0 ? (W / 4) / THREADS : 1;   // radix-4 butterflies per thread and stage
-    double2* a = s_buf;
-    double2* b = s_buf + W;
-    {
-        float2 sm[PER];
-        double g[PER];
-#pragma unroll
-        for (int r = 0; r < PER; r++) {
-            const int w = threadIdx.x + r * THREADS;
-            const int64_t i = base + w;
-            sm[r] = (i < n) ? x[i] : make_float2(0.0f, 0.0f);
-            g[r] = window[w];
-        }
-#pragma unroll
-        for (int r = 0; r < PER; r++) a[threadIdx.x + r * THREADS] = make_double2((double)sm[r].x * g[r], (double)sm[r].y * g[r]);
-    }
-    __syncthreads();
-    if (LOG2W & 1) {   // one radix-2 stage first
-#pragma unroll
-        for (int r = 0; r < (W / 2) / THREADS; r++) {
-            const int j = threadIdx.x + r * THREADS;
-            const double2 u = a[j], v = a[j + W / 2];
-            b[2 * j] = make_double2(u.x + v.x, u.y + v.y);
-            b[2 * j + 1] = make_double2(u.x - v.x, u.y - v.y);
-        }
-        __syncthreads();
-        double2* t = a; a = b; b = t;
-    }
-#pragma unroll
-    for (int st = 0; st < LOG2W / 2; st++) {
-        const int ns = 1 << (2 * st + (LOG2W & 1));   // length of the sub-transforms finished so far (compile-time after unrolling)
-        constexpr int quarter = W / 4;
-        const int tstep = W / (4 * ns);               // exp(-2 pi i r k / (4 ns)) = tw[r * k * tstep]
-#pragma unroll
-        for (int r = 0; r < BPT; r++) {
-            const int j = threadIdx.x + r * THREADS;
-            if (j < quarter) {
-                const int k = j & (ns - 1);
-                double2 v0 = a[j], v1 = a[j + quarter], v2 = a[j + 2 * quarter], v3 = a[j + 3 * quarter];
-                if (ns > 1) {
-                    v1 = cmul(v1, tw[k * tstep]);
-                    v2 = cmul(v2, tw[2 * k * tstep]);
-                    v3 = cmul(v3, tw[3 * k * tstep]);
-                }
-                // DFT of length 4 (forward: -i rotation)
-                const double2 s02 = make_double2(v0.x + v2.x, v0.y + v2.y), d02 = make_double2(v0.x - v2.x, v0.y - v2.y);
-                const double2 s13 = make_double2(v1.x + v3.x, v1.y + v3.y), d13 = make_double2(v1.x - v3.x, v1.y - v3.y);
-                const int j0 = ((j - k) << 2) + k;   // (j / ns) * 4 ns + k
-                b[j0] = make_double2(s02.x + s13.x, s02.y + s13.y);
-                b[j0 + ns] = make_double2(d02.x + d13.y, d02.y - d13.x);      // d02 - i d13
-                b[j0 + 2 * ns] = make_double2(s02.x - s13.x, s02.y - s13.y);
-                b[j0 + 3 * ns] = make_double2(d02.x - d13.y, d02.y + d13.x);  // d02 + i d13
-            }
-        }
-        __syncthreads();
-        double2* t = a; a = b; b = t;
-    }
-    return a;
-}
-
-// MODE 0: out = complex128 [F][W] = X / W;  MODE 1: out = float32 [F][W] dB map (fftshift + fliplr + complex64 cast + 10 log10f);
-// MODE 2: the image (img, see StftImage)
-// W = 2^LOG2W and the thread count are compile-time: every loop below is fully unrolled (the W / THREADS loads of a thread are
-// in flight together — the first version, with run-time W, was bound by the latency of one load after the other — and the index
-// arithmetic of the stages is shifts and masks).
-template <int LOG2W, int THREADS, int MODE>
-__global__ void __launch_bounds__(THREADS) k_stft_fused(const float2* __restrict__ x, int64_t n, int hop,
-                                                       const double* __restrict__ window, const double2* __restrict__ tw,
-                                                       int64_t nframes, void* __restrict__ out_, StftImage img) {
-    constexpr int W = 1 << LOG2W;
-    constexpr int PER = W / THREADS;
-    extern __shared__ double2 s_buf[];        // two W-element buffers (MODE 2: then the image staging)
-    if (MODE == 2) {
-        stft_image_block<W, THREADS, false>(
-            img, hop, [&](int64_t base, int64_t end) { return stft_fused_fft<LOG2W, THREADS>(x, end, base, window, tw, s_buf); },
-            (unsigned char*)(s_buf + 2 * W), (uint32_t*)out_);
-        return;
-    }
-    const int64_t f = blockIdx.x;
-    const double2* a = stft_fused_fft<LOG2W, THREADS>(x, n, f * hop, window, tw, s_buf);
-    const double inv = 1.0 / (double)W;   // W is a power of two: multiplying by 1/W IS the division by W, bit for bit
-    if (MODE == 0) {
-        double2* out = (double2*)out_ + f * W;
-#pragma unroll
-        for (int r = 0; r < PER; r++) {
-            const int w = threadIdx.x + r * THREADS;
-            out[w] = make_double2(a[w].x * inv, a[w].y * inv);
-        }
-    } else {
-        float* out = (float*)out_ + f * W;
-        constexpr int shift = (W + 1) / 2;
-#pragma unroll
-        for (int r = 0; r < PER; r++) {
-            const int j = threadIdx.x + r * THREADS;
-            const int src = ((W - 1 - j) + shift) & (W - 1);   // fliplr, then fftshift
-            const double2 v = a[src];
-            const float re = (float)(v.x * inv), im = (float)(v.y * inv);   // complex128 / W, then astype(complex64)
-            out[j] = __fmul_rn(10.0f, log10f(__fadd_rn(__fmul_rn(re, re), __fmul_rn(im, im))));
-        }
-    }
-}
-
-// ---- radix-16 variant (W = 256, 1024, 4096): two radix-4 levels per pass held in registers, so a frame crosses shared memory
-// three times (1024 = 16 * 16 * 4) instead of five: the radix-4 kernel above is bound by shared-memory bandwidth.
-// One thread owns 16 points of a pass; W / 16 threads per frame.  Both buffers are padded by one element every 16 (P(i)) so that
-// the stride-16 stores of the first pass do not pile onto the same banks.
+// ---- the FFT (W = 2^LOG2W, 128 .. 4096): LOG2W / 4 radix-16 passes, each two radix-4 levels held in registers, then one closing
+// pass of radix 2^(LOG2W mod 4) (radix-8 for 128 and 2048, radix-2 for 512, radix-4 for 1024, none for 256 and 4096), so a frame
+// crosses shared memory three times at W = 1024 (16 * 16 * 4).  One thread owns 16 points of every pass; W / 16 threads per frame
+// (stft_frames frames per block).
+// Both buffers are padded by one element every 16 (stft_pad) so that the stride-16 stores of the first pass do not pile onto the
+// same banks.
 __device__ __forceinline__ double2 cadd(double2 a, double2 b) { return make_double2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ double2 csub(double2 a, double2 b) { return make_double2(a.x - b.x, a.y - b.y); }
 __device__ __forceinline__ double2 cmul_mi(double2 a) { return make_double2(a.y, -a.x); }   // a * (-i)
@@ -293,6 +196,25 @@ __device__ __forceinline__ double2 cmul_mi(double2 a) { return make_double2(a.y,
 __device__ __forceinline__ void dft4(double2& x0, double2& x1, double2& x2, double2& x3) {
     const double2 s02 = cadd(x0, x2), d02 = csub(x0, x2), s13 = cadd(x1, x3), d13 = cmul_mi(csub(x1, x3));
     x0 = cadd(s02, s13); x1 = cadd(d02, d13); x2 = csub(s02, s13); x3 = csub(d02, d13);
+}
+// forward DFT of length 2, in place
+__device__ __forceinline__ void dft2(double2& x0, double2& x1) {
+    const double2 s = cadd(x0, x1), d = csub(x0, x1);
+    x0 = s; x1 = d;
+}
+// forward DFT of length 8, in place: v[c + 2 m] -> columns (DFT4 over m), twiddle w8^(c r), rows (DFT2 over c); natural order out
+__device__ __forceinline__ void dft8(double2 (&v)[8]) {
+    const double H = 0.70710678118654752440;
+    dft4(v[0], v[2], v[4], v[6]);   // now v[c + 2 r] = u_c[r]
+    dft4(v[1], v[3], v[5], v[7]);
+    v[1 + 2] = cmul(v[1 + 2], make_double2(H, -H));    // c=1, r=1: w8^1
+    v[1 + 4] = cmul_mi(v[1 + 4]);                      // w8^2 = -i
+    v[1 + 6] = cmul(v[1 + 6], make_double2(-H, -H));   // w8^3
+#pragma unroll
+    for (int r = 0; r < 4; r++) dft2(v[2 * r], v[2 * r + 1]);   // v[2 r + s] = y[r + 4 s]
+    const double2 y[8] = {v[0], v[2], v[4], v[6], v[1], v[3], v[5], v[7]};
+#pragma unroll
+    for (int i = 0; i < 8; i++) v[i] = y[i];
 }
 // forward DFT of length 16, in place: v[c + 4 r'] -> columns, twiddle w16^(c r), rows; output y[r + 4 s] (natural order)
 __device__ __forceinline__ void dft16(double2 (&v)[16]) {
@@ -324,7 +246,7 @@ __device__ __forceinline__ const double2* stft_r16_fft(const float2* __restrict_
     constexpr int PADW = W + W / 16;
     double2* a = s_buf;
     double2* b = s_buf + PADW;
-    const int tid = threadIdx.x;
+    const int tid = stft_lane<W>();
     {
         float2 sm[16];
         double g[16];
@@ -361,46 +283,55 @@ __device__ __forceinline__ const double2* stft_r16_fft(const float2* __restrict_
         __syncthreads();
         double2* t = a; a = b; b = t;
     }
-    if ((LOG2W & 3) == 2) {   // one radix-4 pass left (sub-transforms of length W / 4)
-        constexpr int ns = W / 4;
-        double2 y[4][4];
+    constexpr int R = 1 << (LOG2W & 3);   // the closing pass: sub-transforms of length W / R left
+    if constexpr (R > 1) {
+        constexpr int ns = W / R;
+        double2 y[16 / R][R];   // 16 / R butterflies of radix R per thread
 #pragma unroll
-        for (int r = 0; r < 4; r++) {
-            const int j = tid + T * r;   // butterfly index < W / 4; k = j (ns = W / 4 > j)
-            double2 v0 = a[stft_pad(j)], v1 = a[stft_pad(j + ns)], v2 = a[stft_pad(j + 2 * ns)], v3 = a[stft_pad(j + 3 * ns)];
-            v1 = cmul(v1, tw[j]);
-            v2 = cmul(v2, tw[2 * j]);
-            v3 = cmul(v3, tw[3 * j]);
-            dft4(v0, v1, v2, v3);
-            y[r][0] = v0; y[r][1] = v1; y[r][2] = v2; y[r][3] = v3;
+        for (int r = 0; r < 16 / R; r++) {
+            const int j = tid + T * r;   // butterfly index < W / R; k = j (ns = W / R > j)
+#pragma unroll
+            for (int q = 0; q < R; q++) y[r][q] = a[stft_pad(j + ns * q)];
+#pragma unroll
+            for (int q = 1; q < R; q++) y[r][q] = cmul(y[r][q], tw[q * j]);
+            if constexpr (R == 2) dft2(y[r][0], y[r][1]);
+            else if constexpr (R == 4) dft4(y[r][0], y[r][1], y[r][2], y[r][3]);
+            else dft8(y[r]);
         }
 #pragma unroll
-        for (int r = 0; r < 4; r++)
+        for (int r = 0; r < 16 / R; r++)
 #pragma unroll
-            for (int q = 0; q < 4; q++) b[stft_pad(tid + T * r + ns * q)] = y[r][q];
+            for (int q = 0; q < R; q++) b[stft_pad(tid + T * r + ns * q)] = y[r][q];
         __syncthreads();
         double2* t = a; a = b; b = t;
     }
     return a;
 }
 
+// MODE 0: out = complex128 [F][W] = X / W;  MODE 1: out = float32 [F][W] dB map (fftshift + fliplr + complex64 cast + 10 log10f);
+// MODE 2: the image (img, see StftImage)
+// W = 2^LOG2W is compile-time: every loop below is fully unrolled (a thread's 16 loads are in flight together — the first version,
+// with run-time W, was bound by the latency of one load after the other — and the index arithmetic of the passes is shifts and masks).
 template <int LOG2W, int MODE>
-__global__ void __launch_bounds__((1 << LOG2W) / 16) k_stft_r16(const float2* __restrict__ x, int64_t n, int hop,
+__global__ void __launch_bounds__(stft_frames(1 << LOG2W) * (1 << LOG2W) / 16) k_stft_r16(const float2* __restrict__ x, int64_t n, int hop,
                                                                const double* __restrict__ window, const double2* __restrict__ tw,
                                                                int64_t nframes, void* __restrict__ out_, StftImage img) {
     constexpr int W = 1 << LOG2W;
     constexpr int T = W / 16;                 // threads per frame
     constexpr int PADW = W + W / 16;
-    extern __shared__ double2 s_buf[];        // two padded buffers (MODE 2: then the image staging)
+    constexpr int G = stft_frames(W);         // frames per block
+    extern __shared__ double2 s_buf[];        // two padded buffers per frame (MODE 2: then the image staging)
+    double2* buf = s_buf + stft_group<W>() * 2 * PADW;
     if (MODE == 2) {
-        stft_image_block<W, T, true>(
-            img, hop, [&](int64_t base, int64_t end) { return stft_r16_fft<LOG2W>(x, end, base, window, tw, s_buf); },
-            (unsigned char*)(s_buf + 2 * PADW), (uint32_t*)out_);
+        stft_image_block<W>(
+            img, hop, [&](int64_t base, int64_t end) { return stft_r16_fft<LOG2W>(x, end, base, window, tw, buf); },
+            (unsigned char*)(s_buf + 2 * G * PADW), (uint32_t*)out_);
         return;
     }
-    const int tid = threadIdx.x;
-    const int64_t f = blockIdx.x;
-    const double2* a = stft_r16_fft<LOG2W>(x, n, f * hop, window, tw, s_buf);
+    const int tid = stft_lane<W>();
+    const int64_t f = (int64_t)blockIdx.x * G + stft_group<W>();
+    const double2* a = stft_r16_fft<LOG2W>(x, n, f * hop, window, tw, buf);
+    if (G > 1 && f >= nframes) return;        // the last block's spare frames (their samples read as zeros)
     const double inv = 1.0 / (double)W;
     if (MODE == 0) {
         double2* out = (double2*)out_ + f * W;
@@ -424,58 +355,40 @@ __global__ void __launch_bounds__((1 << LOG2W) / 16) k_stft_r16(const float2* __
     }
 }
 
-template <int LOG2W, int MODE>
-static int stft_r16_launch(urh_ctx* ctx, const float* d_x, int64_t n, int hop, const double* d_window, const double2* tw,
-                           int64_t num_frames, void* d_out) {
-    constexpr int W = 1 << LOG2W;
-    const size_t smem = (size_t)2 * (W + W / 16) * sizeof(double2);
-    if (smem > 48 * 1024)
-        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_r16<LOG2W, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    URH_LAUNCH(ctx, (k_stft_r16<LOG2W, MODE>), (unsigned)num_frames, W / 16, smem, (const float2*)d_x, n, hop, d_window, tw, num_frames,
-               d_out, StftImage{});
+// the shared-memory kernel serves power-of-two windows of 128 .. 4096 points (W = 4096: 139 KB of FFT buffers), grids of fewer
+// than 2^31 blocks (frames, or image blocks: far beyond any capture that fits the device) and colormaps whose indices fit the
+// image mode's uint16 staging; everything else takes cuFFT
+static bool stft_smem_serves(int W, int64_t blocks, int entries) {
+    return (W & (W - 1)) == 0 && W >= 128 && W <= 4096 && blocks < ((int64_t)1 << 31) && entries <= 65536;
+}
+
+template <int LOG2W>
+static int stft_r16_launch(urh_ctx* ctx, int mode, const float* d_x, int64_t n, int hop, const double* d_window, const double2* tw,
+                           int64_t count, void* d_out, const StftImage& img) {
+    constexpr int W = 1 << LOG2W, G = stft_frames(W);
+    const auto kernel = mode == 0 ? k_stft_r16<LOG2W, 0> : mode == 1 ? k_stft_r16<LOG2W, 1> : k_stft_r16<LOG2W, 2>;
+    size_t smem = (size_t)2 * G * (W + W / 16) * sizeof(double2);
+    if (mode == 2) smem += (size_t)W * STFT_IMG_FPB * sizeof(uint16_t) + 1024 * sizeof(uint32_t);
+    if (smem > 48 * 1024) URH_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int64_t blocks = mode == 2 ? count : urh_div_up(count, G);
+    URH_LAUNCH(ctx, kernel, (unsigned)blocks, G * W / 16, smem, (const float2*)d_x, n, hop, d_window, tw, count, d_out, img);
     return URH_OK;
 }
 
-template <int LOG2W, int MODE>
-static int stft_fused_launch(urh_ctx* ctx, const float* d_x, int64_t n, int hop, const double* d_window, const double2* tw,
-                             int64_t num_frames, void* d_out) {
-    constexpr int W = 1 << LOG2W;
-    constexpr int THREADS = (W / 4 >= 256) ? 256 : (W / 4 >= 32 ? W / 4 : 32);
-    const size_t smem = (size_t)2 * W * sizeof(double2);
-    if (smem > 48 * 1024)
-        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_fused<LOG2W, THREADS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    URH_LAUNCH(ctx, (k_stft_fused<LOG2W, THREADS, MODE>), (unsigned)num_frames, THREADS, smem, (const float2*)d_x, n, hop, d_window, tw,
-               num_frames, d_out, StftImage{});
-    return URH_OK;
-}
-
-static int stft_fused(urh_ctx* ctx, const float* d_x, int64_t n, int W, int hop, const double* d_window, int64_t num_frames,
-                      void* d_out, int mode) {
+// one launch of k_stft_r16 for a window stft_smem_serves: `count` frames (modes 0, 1) or image blocks (mode 2)
+static int stft_r16(urh_ctx* ctx, int mode, int W, const float* d_x, int64_t n, int hop, const double* d_window, const double2* tw,
+                    int64_t count, void* d_out, const StftImage& img) {
     int log2w = 0;
     while ((1 << log2w) < W) log2w++;
-    urh_arena_reset(ctx);
-    double2* tw;
-    URH_CHECK(urh_arena(ctx, (size_t)W, &tw));
-    URH_LAUNCH(ctx, k_fft_twiddles, (unsigned)urh_div_up(W, 256), 256, 0, W, tw);
-    // grid.x is limited to 2^31 - 1 frames: far beyond any capture that fits the device
-#define STFT_CASE(L)                                                                                                          \
-    case L:                                                                                                                   \
-        return mode == 0 ? stft_fused_launch<L, 0>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out)         \
-                         : stft_fused_launch<L, 1>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out);
-    if (!getenv("URH_B200_STFT_RADIX4")) {   // 16 | W: three passes through shared memory instead of five
-        if (log2w == 10) return mode == 0 ? stft_r16_launch<10, 0>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out)
-                                          : stft_r16_launch<10, 1>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out);
-        if (log2w == 12) return mode == 0 ? stft_r16_launch<12, 0>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out)
-                                          : stft_r16_launch<12, 1>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out);
-        if (log2w == 8) return mode == 0 ? stft_r16_launch<8, 0>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out)
-                                         : stft_r16_launch<8, 1>(ctx, d_x, n, hop, d_window, (const double2*)tw, num_frames, d_out);
-    }
     switch (log2w) {
-        STFT_CASE(7) STFT_CASE(8) STFT_CASE(9) STFT_CASE(10) STFT_CASE(11) STFT_CASE(12)
-        default: break;
+        case 7: return stft_r16_launch<7>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        case 8: return stft_r16_launch<8>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        case 9: return stft_r16_launch<9>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        case 10: return stft_r16_launch<10>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        case 11: return stft_r16_launch<11>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        case 12: return stft_r16_launch<12>(ctx, mode, d_x, n, hop, d_window, tw, count, d_out, img);
+        default: URH_FAIL(ctx, URH_ERR_INVALID, "stft: unsupported window size %d", W);
     }
-#undef STFT_CASE
-    URH_FAIL(ctx, URH_ERR_INVALID, "stft_fused: unsupported window size");
 }
 
 static int ensure_plan(urh_ctx* ctx, int W, int64_t batch) {
@@ -499,10 +412,14 @@ static int ensure_plan(urh_ctx* ctx, int W, int64_t batch) {
 static int stft_run(urh_ctx* ctx, const float* d_x, int64_t n, int W, int hop, const double* d_window, int64_t num_frames,
                     void* d_out, int mode) {
     if (W <= 0 || hop <= 0 || num_frames <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "stft: bad window/hop/frames");
-    // power-of-two windows 128 .. 4096 (128 KB of shared memory): the fused kernel; anything else: cuFFT with two kernels around it
-    if ((W & (W - 1)) == 0 && W >= 128 && W <= 4096 && num_frames < ((int64_t)1 << 31) && !getenv("URH_B200_STFT_CUFFT"))
-        return stft_fused(ctx, d_x, n, W, hop, d_window, num_frames, d_out, mode);
     urh_arena_reset(ctx);
+    if (stft_smem_serves(W, num_frames, 0)) {
+        double2* tw;
+        URH_CHECK(urh_arena(ctx, (size_t)W, &tw));
+        URH_LAUNCH(ctx, k_fft_twiddles, (unsigned)urh_div_up(W, 256), 256, 0, W, tw);
+        return stft_r16(ctx, mode, W, d_x, n, hop, d_window, tw, num_frames, d_out, StftImage{});
+    }
+    // cuFFT with two kernels around it
     const int64_t max_batch = max((int64_t)1, ((int64_t)512 << 20) / ((int64_t)W * 16));
     const int64_t batch = min(num_frames, max_batch);
     double2* buf;
@@ -563,31 +480,6 @@ extern "C" int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, 
 }
 
 // ---- spectrogram images: STFT -> dB -> colormap in one launch (Spectrogram.create_spectrogram_image / create_image_segments) --------
-template <int LOG2W>
-static int stft_image_r16_launch(urh_ctx* ctx, const float* d_x, int hop, const double* d_window, const double2* tw, int64_t blocks,
-                                 const StftImage& img, uint32_t* d_out) {
-    constexpr int W = 1 << LOG2W;
-    const size_t smem = (size_t)2 * (W + W / 16) * sizeof(double2) + (size_t)W * STFT_IMG_FPB * sizeof(uint16_t) + 1024 * sizeof(uint32_t);
-    if (smem > 48 * 1024)
-        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_r16<LOG2W, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    URH_LAUNCH(ctx, (k_stft_r16<LOG2W, 2>), (unsigned)blocks, W / 16, smem, (const float2*)d_x, (int64_t)0, hop, d_window, tw, (int64_t)0,
-               (void*)d_out, img);
-    return URH_OK;
-}
-
-template <int LOG2W>
-static int stft_image_fused_launch(urh_ctx* ctx, const float* d_x, int hop, const double* d_window, const double2* tw, int64_t blocks,
-                                   const StftImage& img, uint32_t* d_out) {
-    constexpr int W = 1 << LOG2W;
-    constexpr int THREADS = (W / 4 >= 256) ? 256 : (W / 4 >= 32 ? W / 4 : 32);
-    const size_t smem = (size_t)2 * W * sizeof(double2) + (size_t)W * STFT_IMG_FPB * sizeof(uint16_t) + 1024 * sizeof(uint32_t);
-    if (smem > 48 * 1024)
-        URH_CUDA(ctx, cudaFuncSetAttribute(k_stft_fused<LOG2W, THREADS, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    URH_LAUNCH(ctx, (k_stft_fused<LOG2W, THREADS, 2>), (unsigned)blocks, THREADS, smem, (const float2*)d_x, (int64_t)0, hop, d_window, tw,
-               (int64_t)0, (void*)d_out, img);
-    return URH_OK;
-}
-
 // composed path: one chunk of dB rows (frames f0 .. f0 + nf - 1 of a segment with F frames) through the look-up into its place
 // transpose = 0: out[r][f0 + f] (row pitch F) = lut(db[f][r]);  transpose = 1: out[f0 + f][r] = lut(db[f][W - 1 - r])
 __global__ void k_bgra_place(const float* __restrict__ db, int64_t nf, int W, int64_t F, int64_t f0, const uint32_t* __restrict__ colormap,
@@ -635,11 +527,7 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
         max_frames = max(max_frames, F);
     }
     const float r32 = (float)((double)data_max - (double)data_min);   // as urh_bgra_lookup forms it
-    int log2w = 0;
-    while ((1 << log2w) < W) log2w++;
-    const bool fused = (W & (W - 1)) == 0 && W >= 128 && W <= 4096 && entries <= 65536 && blocks < ((int64_t)1 << 31) &&
-                       !getenv("URH_B200_STFT_CUFFT");
-    if (fused) {
+    if (stft_smem_serves(W, blocks, entries)) {
         if (!ctx->img_tw) URH_CUDA(ctx, cudaMalloc(&ctx->img_tw, (size_t)4096 * sizeof(double2)));
         if (ctx->img_tw_n != W) {
             URH_LAUNCH(ctx, k_fft_twiddles, (unsigned)urh_div_up(W, 256), 256, 0, W, (double2*)ctx->img_tw);
@@ -650,23 +538,7 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
         URH_CHECK(urh_arena(ctx, seg.size(), &d_seg));
         URH_CUDA(ctx, cudaMemcpyAsync(d_seg, seg.data(), seg.size() * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
         const StftImage img{d_seg, nseg, (const uint32_t*)d_colormap, entries, data_min, r32, transpose ? 1 : 0};
-        const double2* tw = (const double2*)ctx->img_tw;
-        uint32_t* out = (uint32_t*)d_out;
-        if (!getenv("URH_B200_STFT_RADIX4")) {
-            if (log2w == 8) return stft_image_r16_launch<8>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            if (log2w == 10) return stft_image_r16_launch<10>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            if (log2w == 12) return stft_image_r16_launch<12>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-        }
-        switch (log2w) {
-            case 7: return stft_image_fused_launch<7>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            case 8: return stft_image_fused_launch<8>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            case 9: return stft_image_fused_launch<9>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            case 10: return stft_image_fused_launch<10>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            case 11: return stft_image_fused_launch<11>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            case 12: return stft_image_fused_launch<12>(ctx, d_x, hop, d_window, tw, blocks, img, out);
-            default: break;
-        }
-        URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: unsupported window size");
+        return stft_r16(ctx, 2, W, d_x, n, hop, d_window, (const double2*)ctx->img_tw, blocks, d_out, img);
     }
     // composed: the dB map of up to 256 MiB of frames at a time (stft_run), then its pixels into place
     const int64_t chunk = min(max_frames, max((int64_t)1, ((int64_t)256 << 20) / ((int64_t)W * 4)));
