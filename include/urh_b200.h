@@ -187,9 +187,10 @@ int urh_stft(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop
 int urh_spectrogram_db(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop, const double* d_window,
                        int64_t num_frames, float* d_out);
 /* Spectrogram.apply_bgra_lookup (Spectrogram.py:192-206): d_out[cols][rows][4] = colormap[clip(int((entries - 1) * ((data.T - min) /
- * (max - min))))], colormap = entries x 4 bytes (blue, green, red, alpha); normalize = 0: the data are indices already. */
+ * (max - min))))], colormap = entries x 4 bytes (blue, green, red, alpha); normalize = 0: the data are indices already.  The bounds
+ * are the caller's Python floats: min is used as a float32, max - min is formed in double and rounded to float32 once, as numpy does. */
 int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, int64_t cols, const uint8_t* d_colormap, int entries,
-                    float data_min, float data_max, int normalize, uint8_t* d_out);
+                    double data_min, double data_max, int normalize, uint8_t* d_out);
 /* Spectrogram.create_spectrogram_image / create_image_segments (Spectrogram.py:164-190) in one launch: the BGRA image
  * apply_bgra_lookup(dB map) of every segment s = d_x[h_seg_start[s] : h_seg_start[s] + h_seg_len[s]] (complex64), each with its own
  * frame count max(1, (len - W) // hop + 1), zero-padded below W samples, written back to back into d_out: transpose = 0 gives
@@ -198,7 +199,7 @@ int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, int64_t col
  * 65536 entries take the fused kernel; anything else composes those two stages on the device. */
 int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop, const double* d_window,
                          const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* d_colormap, int entries,
-                         float data_min, float data_max, int transpose, uint8_t* d_out);
+                         double data_min, double data_max, int transpose, uint8_t* d_out);
 /* d_out[i] = d_x[start + i * step], i < count (complex64 samples; a Python slice of a capture of n samples, step may be negative) */
 int urh_gather_samples(urh_ctx* ctx, const float* d_x, int64_t n, int64_t start, int64_t step, int64_t count, float* d_out);
 /* Spectrogram.export_to_fta (Spectrogram.py:118-154): rows [row0, row0 + nrows) of the record array [W][frames][reps], packed
@@ -386,7 +387,7 @@ int urh_spectrogram_db_stream(urh_ctx* ctx, const float* h_x, int64_t n, int win
                               int64_t num_frames, int64_t chunk_samples, int ring, float* h_out);
 int urh_spectrogram_bgra_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
                                 const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* h_colormap, int entries,
-                                float data_min, float data_max, int transpose, int64_t chunk_samples, int ring, uint8_t* h_out);
+                                double data_min, double data_max, int transpose, int64_t chunk_samples, int ring, uint8_t* h_out);
 int urh_stream_windows(int entry, int64_t n, int64_t out_len, int64_t p0, int64_t p1, int64_t chunk_samples, const int64_t* h_seg_start,
                        const int64_t* h_seg_len, int nseg, int64_t* h_win, int64_t cap, int64_t* count);
 int urh_stream_window_schedule(const int64_t* h_win, int64_t chunks, int ring, int flags, int64_t* h_ops, int64_t cap, int64_t* count);

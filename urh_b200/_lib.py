@@ -155,8 +155,8 @@ SIGNATURES = {
     "urh_costas_stitch_stats": (i32, [vp, vp]),
     "urh_selftest_packed_div": (i32, [vp, C.c_uint64, i64, C.POINTER(i64), C.POINTER(i64)]),
     "urh_selftest_scan": (i32, [vp, i32, i32, vp, i64, vp, vp, vp, i64, vp]),
-    "urh_bgra_lookup": (i32, [vp, vp, i64, i64, vp, i32, f32, f32, i32, vp]),
-    "urh_spectrogram_bgra": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, f32, f32, i32, vp]),
+    "urh_bgra_lookup": (i32, [vp, vp, i64, i64, vp, i32, C.c_double, C.c_double, i32, vp]),
+    "urh_spectrogram_bgra": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, C.c_double, C.c_double, i32, vp]),
     "urh_gather_samples": (i32, [vp, vp, i64, i64, i64, i64, vp]),
     "urh_fta_records": (i32, [vp, vp, i64, i32, i64, i64, vp, C.c_double, i32, vp, vp]),
     "urh_path_minmax": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, vp]),
@@ -184,7 +184,7 @@ SIGNATURES = {
     "urh_dc_correction_stream": (i32, [vp, vp, i32, i64, i32, i64, i32, vp]),
     "urh_stft_stream": (i32, [vp, vp, i64, i32, i32, vp, i64, i64, i32, vp]),
     "urh_spectrogram_db_stream": (i32, [vp, vp, i64, i32, i32, vp, i64, i64, i32, vp]),
-    "urh_spectrogram_bgra_stream": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, f32, f32, i32, i64, i32, vp]),
+    "urh_spectrogram_bgra_stream": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, C.c_double, C.c_double, i32, i64, i32, vp]),
     "urh_stream_windows": (i32, [i32, i64, i64, i64, i64, i64, vp, vp, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_window_schedule": (i32, [vp, i64, i32, i32, vp, i64, C.POINTER(i64)]),
     "urh_stream_filter_footprint": (i32, [i32, i64, i64, i32, i64, i64, i64, i64, i32, i32, C.POINTER(i64)]),

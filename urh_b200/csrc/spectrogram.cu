@@ -122,10 +122,10 @@ struct StftImage {
 };
 
 // Spectrogram.apply_bgra_lookup per value: float32 subtract, divide, multiply, truncate toward zero (astype(int)), np.take(mode="clip");
-// NaN and out-of-range values become INT64_MIN in numpy, which mode="clip" maps to entry 0
+// numpy's cast is exact for |v| < 2^63; NaN, infinities and everything else become INT64_MIN, which mode="clip" maps to entry 0
 __device__ __forceinline__ int bgra_index(float v, float data_min, float range, float scale, int L, int normalize) {
     if (normalize) v = __fmul_rn(scale, __fdiv_rn(__fsub_rn(v, data_min), range));
-    long long k = (v == v && fabsf(v) < 9.0e18f) ? (long long)v : LLONG_MIN;
+    long long k = (v == v && fabsf(v) < 0x1p63f) ? (long long)v : LLONG_MIN;
     k = k < 0 ? 0 : (k > L - 1 ? L - 1 : k);
     return (int)k;
 }
@@ -467,15 +467,17 @@ __global__ void k_bgra_lookup(const float* __restrict__ data, int64_t rows, int6
     }
 }
 
+// The reference's bounds are Python floats, which meet the float32 array as float32 (weak scalars): data_min on its own, and the
+// range data_max - data_min formed in double first and rounded once.  Rounding the bounds before subtracting would round it twice.
+static inline float bgra_range(double data_min, double data_max) { return (float)(data_max - data_min); }
+
 extern "C" int urh_bgra_lookup(urh_ctx* ctx, const float* d_data, int64_t rows, int64_t cols, const uint8_t* d_colormap, int entries,
-                               float data_min, float data_max, int normalize, uint8_t* d_out) {
+                               double data_min, double data_max, int normalize, uint8_t* d_out) {
     if (rows <= 0 || cols <= 0) return URH_OK;
     if (entries <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "bgra_lookup: empty colormap");
-    // the reference forms (data_max - data_min) in Python floats; as a weak scalar it meets the float32 array as a float32
-    const float r32 = (float)((double)data_max - (double)data_min);
     const unsigned grid = (unsigned)min(urh_div_up(rows * cols, 256), (int64_t)ctx->sm_count * 16);
-    URH_LAUNCH(ctx, k_bgra_lookup, grid, 256, 0, d_data, rows, cols, (const uint32_t*)d_colormap, entries, data_min, r32, normalize,
-               (uint32_t*)d_out);
+    URH_LAUNCH(ctx, k_bgra_lookup, grid, 256, 0, d_data, rows, cols, (const uint32_t*)d_colormap, entries, (float)data_min,
+               bgra_range(data_min, data_max), normalize, (uint32_t*)d_out);
     return URH_OK;
 }
 
@@ -509,7 +511,7 @@ __global__ void k_bgra_place(const float* __restrict__ db, int64_t nf, int W, in
 
 extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, int window_size, int hop, const double* d_window,
                                     const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* d_colormap, int entries,
-                                    float data_min, float data_max, int transpose, uint8_t* d_out) {
+                                    double data_min, double data_max, int transpose, uint8_t* d_out) {
     const int W = window_size;
     if (W <= 0 || hop <= 0 || nseg <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: bad window/hop/segments");
     if (entries <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "spectrogram_bgra: empty colormap");
@@ -526,7 +528,7 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
         pixels += F * W;
         max_frames = max(max_frames, F);
     }
-    const float r32 = (float)((double)data_max - (double)data_min);   // as urh_bgra_lookup forms it
+    const float lo32 = (float)data_min, r32 = bgra_range(data_min, data_max);
     if (stft_smem_serves(W, blocks, entries)) {
         if (!ctx->img_tw) URH_CUDA(ctx, cudaMalloc(&ctx->img_tw, (size_t)4096 * sizeof(double2)));
         if (ctx->img_tw_n != W) {
@@ -537,7 +539,7 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
         int64_t* d_seg;
         URH_CHECK(urh_arena(ctx, seg.size(), &d_seg));
         URH_CUDA(ctx, cudaMemcpyAsync(d_seg, seg.data(), seg.size() * sizeof(int64_t), cudaMemcpyHostToDevice, ctx->stream));
-        const StftImage img{d_seg, nseg, (const uint32_t*)d_colormap, entries, data_min, r32, transpose ? 1 : 0};
+        const StftImage img{d_seg, nseg, (const uint32_t*)d_colormap, entries, lo32, r32, transpose ? 1 : 0};
         return stft_r16(ctx, 2, W, d_x, n, hop, d_window, (const double2*)ctx->img_tw, blocks, d_out, img);
     }
     // composed: the dB map of up to 256 MiB of frames at a time (stft_run), then its pixels into place
@@ -552,7 +554,7 @@ extern "C" int urh_spectrogram_bgra(urh_ctx* ctx, const float* d_x, int64_t n, i
             rc = stft_run(ctx, d_x + 2 * base, g[1] - base, W, hop, d_window, nf, db, 1);
             if (rc != URH_OK) break;
             const unsigned grid = (unsigned)min(urh_div_up(nf * W, 256), (int64_t)ctx->sm_count * 16);
-            k_bgra_place<<<grid, 256, 0, ctx->stream>>>(db, nf, W, g[2], f0, (const uint32_t*)d_colormap, entries, data_min, r32,
+            k_bgra_place<<<grid, 256, 0, ctx->stream>>>(db, nf, W, g[2], f0, (const uint32_t*)d_colormap, entries, lo32, r32,
                                                         transpose ? 1 : 0, (uint32_t*)d_out + g[4]);
             ctx->launches++;
             const cudaError_t e = cudaGetLastError();
@@ -603,7 +605,7 @@ extern "C" int urh_spectrogram_db_stream(urh_ctx* ctx, const float* h_x, int64_t
 // one long segment, rendered as a segment of its own; with transpose = 0 such a piece is the column band [W][f0:f1][4] of its image.
 extern "C" int urh_spectrogram_bgra_stream(urh_ctx* ctx, const float* h_x, int64_t n, int window_size, int hop, const double* h_window,
                                            const int64_t* h_seg_start, const int64_t* h_seg_len, int nseg, const uint8_t* h_colormap,
-                                           int entries, float data_min, float data_max, int transpose, int64_t chunk_samples, int ring,
+                                           int entries, double data_min, double data_max, int transpose, int64_t chunk_samples, int ring,
                                            uint8_t* h_out) {
     const int W = window_size;
     if (!h_x || !h_window || !h_out || !h_colormap || W <= 0 || hop <= 0 || nseg <= 0)
