@@ -53,6 +53,31 @@ def test_ppseq_to_bits_port(cassette, ref):
         assert fingerprint(mine) == cassette.want(lambda: fingerprint(answers(rfun(rows, sps, bps, write_bit_sample_pos=wp, pause_threshold=pt)))), trial
 
 
+
+def pulse_edge_tables(oracle):
+    """(name, rows, sps, bps) for the tables of tests/pulse_edge_cases.py that ppseq_to_bits takes (bps >= 1, sps >= 1) and that stay
+    small: orders up to 256, negative lengths, tables of n rows"""
+    from pulse_edge_cases import cases
+
+    for c in cases():
+        if c.bps >= 1 and c.sps >= 1 and len(c.x) <= 8192:
+            yield c.name, oracle.grab_pulse_lens(c.x, *c.args()), c.sps, c.bps
+
+
+def test_ppseq_to_bits_on_pulse_edge_tables(cassette, ref, oracle):
+    """_ppseq_to_bits on the pulse tables of the digitizer's edge cases, at each table's own bits per symbol"""
+    rfun = cassette.make(lambda: ref.ProtocolAnalyzer(None)._ppseq_to_bits)
+    tables = 0
+    for name, rows, sps, bps in pulse_edge_tables(oracle):
+        for pt, wp in ((8, True), (0, False)):
+            def answers(r):
+                return [[list(x) for x in r[0]], list(r[1]), [list(x) for x in r[2]]]
+            mine = answers(_oracle_ppseq_to_bits(rows, sps, bps, write_bit_sample_pos=wp, pause_threshold=pt))
+            assert fingerprint(mine) == cassette.want(lambda: fingerprint(answers(rfun(rows, sps, bps, write_bit_sample_pos=wp,
+                                                                                         pause_threshold=pt)))), (name, pt)
+        tables += 1
+    assert tables == 250
+
 def test_plateau_bookkeeping(cassette, ref):
     from urh_b200.ainterpretation import AutoInterpretation as AI
     rng = np.random.default_rng(9)

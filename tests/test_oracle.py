@@ -256,3 +256,41 @@ def test_oracle_center_edges_pinned_to_reference(oracle, request):
     assert got["posinf_in_window"] is None and got["posinf_trimmed"] is not None
     assert got["posinf_first_window_rank"] is None and got["posinf_last_trimmed_rank"] is not None
     assert got["kept_2"] is None and got["kept_3"] is not None
+
+
+def test_oracle_pulse_edges_pinned_to_reference(oracle, request):
+    """The oracle's grab_pulse_lens against the reference's compiled grab_pulse_lens on the named cases of tests/pulse_edge_cases.py:
+    orders 1 .. 256, coinciding / descending / NaN / infinite thresholds, samples on and next to each threshold, the sentinels of
+    every modulation string (-0.0 for QAM), NaN and +-inf samples, runs at tile edges, tolerances up to 65535 and >= n, the ASK
+    relabel at sps - 1 / sps / sps + 1 and the tail row dropped at n rows.  The reference's tables are recorded in
+    tests/golden/ref_pulse_edges.json (large ones as digests); with oracle/_ref built the pin also runs live."""
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette, same
+    from pulse_edge_cases import cases, thresholds
+
+    c = Cassette("pulse_edges", request.node.name)
+    sf = ref_loader.load_kernels()[0] if (RECORD or ref_loader.kernels_available()) else None
+    got = {}
+    for case in cases():
+        mine = oracle.grab_pulse_lens(case.x, *case.args())
+        want = c.want(lambda: [case.name, np.array(sf.grab_pulse_lens(case.x, *case.args()), dtype=np.int64)])
+        assert want[0] == case.name, (want[0], case.name)
+        assert same(mine, want[1]), case.name
+        if sf is not None:
+            assert np.array_equal(mine, np.array(sf.grab_pulse_lens(case.x, *case.args()))), case.name
+        got[case.name] = (case, mine)
+    c.close()
+    assert len(got) == 346
+    # the corners the cases must reach
+    for n in (2047, 2048, 2049, 4097, 2 ** 20 + 1):
+        for name in ("tail_drop_fsk_%d", "tail_drop_ask_%d"):
+            assert len(got[name % n][1]) == n, name % n                           # n firings: the tail row is dropped
+        assert len(got["tail_merge_one_ask_%d" % n][1]) == n - 1                  # merges leave room: the tail row stays
+    assert got["tol_ge_n_1_tol65535_FSK_data"][1].tolist() == [[0, 1 - 65535]]   # one row, negative length
+    assert got["tol_ge_n_5_tol5_FSK_data"][1].tolist() == [[0, 0]]
+    nan_thr = [k for k, (cs, _) in got.items() if cs.bps > 0 and np.isnan(thresholds(cs.center, cs.spacing, 1 << cs.bps)).any()]
+    assert len(nan_thr) == 64
+    assert sum(cs.bps == 8 for cs, _ in got.values()) == 42
+    qam = got["signed_zero_QAM"][0]
+    assert (np.signbit(qam.x) & (qam.x == 0)).any() and (~np.signbit(qam.x) & (qam.x == 0)).any()
+    assert not np.array_equal(got["signed_zero_QAM"][1], got["signed_zero_FSK"][1])
