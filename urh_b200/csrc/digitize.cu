@@ -262,21 +262,31 @@ static float max_magnitude_for(int dtype) {
 
 static bool iq_vec_aligned(const void* p, int dtype) { return ((uintptr_t)p % (2 * (size_t)urh_iq_bytes(dtype))) == 0; }
 
-// tile_lo / tile_hi: restrict the pass to tiles [tile_lo, tile_hi) (chunked ingest: a chunk is demodulated as soon as its
-// upload has landed); tile_hi < 0 = all tiles.
-// spec != NULL (float32 FSK, tile statistics, no DIG): the fast kernel's tiles are also digitized at the guess spec->tg into
-// tiles / staging (tol, stage_cap), with their margins; spec->lo / hi is set to that tile range (UrhSpec).
+// The optional parts of a dense pass over IQ (launch_dense_iq); the defaults leave each of them off.
+struct DensePass {
+    float* qad = nullptr;                 // the demodulated samples
+    const UrhDigitizer* dz = nullptr;     // digitize into dz's tables at the classes of cls (with spec: the fast tiles at the guess)
+    int has_halo = 0;                     // the sample preceding the first one is readable right before d_iq
+    UrhTileStats* tile_stats = nullptr;   // per-tile statistics of the kept samples
+    int64_t tile_lo = 0, tile_hi = -1;    // only tiles [tile_lo, tile_hi) (a chunk that has landed); tile_hi < 0: all tiles
+    UrhFine fine = {};                    // with tile_stats: the fine histogram of the kept samples
+    // float32 FSK with tile statistics and qad: the fast kernel's tiles are digitized at the guess spec->tg into dz's tables, with
+    // their margins; spec->lo / hi is set to that tile range
+    UrhSpec* spec = nullptr;
+};
+
 template <int DT, int MOD, bool DIG>
-static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const UrhDemodParams& dp, float* d_qad,
-                             const UrhClassify& cls, int tol, UrhTileSummary* tiles, uint32_t* staging,
-                             int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
-                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
-                             const UrhFine& fine = UrhFine{}, UrhSpec* spec = nullptr) {
+static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const UrhDemodParams& dp, const UrhClassify& cls,
+                             const DensePass& o) {
+    static const UrhDigitizer none = {};
+    const UrhDigitizer& dz = o.dz ? *o.dz : none;
+    int16_t* init_cls = DIG ? dz.d_init : nullptr;
+    const int cls_of_zero = DIG ? host_classify(0.0f, cls) : 0;
     const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const size_t fine_smem = fine.gh ? (size_t)URH_FINE_NB * sizeof(unsigned int) : 0;
-    if (tile_hi < 0 || tile_hi > ntiles) tile_hi = ntiles;
+    const size_t fine_smem = o.fine.gh ? (size_t)URH_FINE_NB * sizeof(unsigned int) : 0;
+    const int64_t tile_lo = o.tile_lo, tile_hi = (o.tile_hi < 0 || o.tile_hi > ntiles) ? ntiles : o.tile_hi;
     const int vec_in = iq_vec_aligned(d_iq, DT) ? 1 : 0;
-    const int vec_out = (d_qad && ((uintptr_t)d_qad % 8) == 0) ? 1 : 0;
+    const int vec_out = (o.qad && ((uintptr_t)o.qad % 8) == 0) ? 1 : 0;
     const int threads = URH_WARPS_PER_BLOCK * 32;
     auto generic = [&](int64_t begin, int64_t end) -> int {   // tiles [begin, end) clipped to the requested range
         begin = begin < tile_lo ? tile_lo : begin;
@@ -284,13 +294,13 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
         const int64_t count = end - begin;
         if (count <= 0) return URH_OK;
         URH_LAUNCH(ctx, (k_dense_iq<DT, MOD, DIG>), (unsigned)urh_div_up(count, URH_WARPS_PER_BLOCK), threads, fine_smem, d_iq, n, dp,
-                   d_qad, vec_in, vec_out, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, begin, count, has_halo,
-                   tile_stats, fine);
+                   o.qad, vec_in, vec_out, cls, dz.tol, dz.tiles, dz.staging, dz.cap, init_cls, cls_of_zero, begin, count, o.has_halo,
+                   o.tile_stats, o.fine);
         return URH_OK;
     };
     // FSK on aligned buffers with a binary digitizer: tiles 1 .. nfull-1 take the paired fast kernel
     const int64_t nfull = n / URH_TILE;
-    const bool fast = MOD == URH_MOD_FSK && vec_in && (!d_qad || vec_out) && (!DIG || cls.order == 2) && nfull > 1;
+    const bool fast = MOD == URH_MOD_FSK && vec_in && (!o.qad || vec_out) && (!DIG || cls.order == 2) && nfull > 1;
     URH_PROF_BEGIN(ctx);
     if (fast) {
         const int64_t fb = tile_lo > 1 ? tile_lo : 1, fe = tile_hi < nfull ? tile_hi : nfull;
@@ -298,24 +308,24 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
             const unsigned grid = (unsigned)urh_div_up(fe - fb, URH_WARPS_PER_BLOCK);
             bool speculated = false;
             if constexpr (DT == URH_DT_F32 && MOD == URH_MOD_FSK && !DIG) {
-                if (spec && tile_stats && d_qad) {
-                    URH_LAUNCH(ctx, (k_fsk_fifo<DT, true, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, 0.0f, dp.noise_value,
-                               tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine, (const float*)spec->tg, spec->margin);
-                    spec->lo = fb;
-                    spec->hi = fe;
+                if (o.spec && o.tile_stats && o.qad) {
+                    URH_LAUNCH(ctx, (k_fsk_fifo<DT, true, true, true>), grid, threads, fine_smem, d_iq, n, dp, o.qad, 0.0f, dp.noise_value,
+                               dz.tol, dz.tiles, dz.staging, dz.cap, fb, fe - fb, o.tile_stats, o.fine, (const float*)o.spec->tg, o.spec->margin);
+                    o.spec->lo = fb;
+                    o.spec->hi = fe;
                     speculated = true;
                 }
             }
             if (speculated) {
-            } else if (tile_stats && d_qad && !DIG) {
-                URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value,
-                           tol, tiles, staging, stage_cap, fb, fe - fb, tile_stats, fine);
-            } else if (d_qad) {
-                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                           tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
+            } else if (o.tile_stats && o.qad && !DIG) {
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, false, true, true>), grid, threads, fine_smem, d_iq, n, dp, o.qad, cls.thr[0], cls.noise_value,
+                           dz.tol, dz.tiles, dz.staging, dz.cap, fb, fe - fb, o.tile_stats, o.fine);
+            } else if (o.qad) {
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, true, false>), grid, threads, 0, d_iq, n, dp, o.qad, cls.thr[0], cls.noise_value, dz.tol,
+                           dz.tiles, dz.staging, dz.cap, fb, fe - fb, nullptr, UrhFine{});
             } else {
-                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, d_qad, cls.thr[0], cls.noise_value, tol,
-                           tiles, staging, stage_cap, fb, fe - fb, nullptr, UrhFine{});
+                URH_LAUNCH(ctx, (k_fsk_fifo<DT, DIG, false, false>), grid, threads, 0, d_iq, n, dp, o.qad, cls.thr[0], cls.noise_value, dz.tol,
+                           dz.tiles, dz.staging, dz.cap, fb, fe - fb, nullptr, UrhFine{});
             }
         }
         URH_CHECK(generic(0, 1));
@@ -327,18 +337,24 @@ static int launch_dense_iq_t(urh_ctx* ctx, const void* d_iq, int64_t n, const Ur
     return URH_OK;
 }
 
-template <int MOD, bool DIG>
-static int launch_dense_iq_m(urh_ctx* ctx, int dtype, const void* d_iq, int64_t n, const UrhDemodParams& dp,
-                             float* d_qad, const UrhClassify& cls, int tol, UrhTileSummary* tiles,
-                             uint32_t* staging, int stage_cap, int16_t* init_cls, int cls_of_zero, int has_halo = 0,
-                             UrhTileStats* tile_stats = nullptr, int64_t tile_lo = 0, int64_t tile_hi = -1,
-                             const UrhFine& fine = UrhFine{}, UrhSpec* spec = nullptr) {
+template <int DT>
+static int launch_dense_iq_dt(urh_ctx* ctx, int mod_type, const void* d_iq, int64_t n, const UrhDemodParams& dp, const UrhClassify& cls,
+                              const DensePass& o) {
+    const bool dig = o.dz && !o.spec;
+    if (mod_type == URH_MOD_ASK)
+        return dig ? launch_dense_iq_t<DT, URH_MOD_ASK, true>(ctx, d_iq, n, dp, cls, o) : launch_dense_iq_t<DT, URH_MOD_ASK, false>(ctx, d_iq, n, dp, cls, o);
+    return dig ? launch_dense_iq_t<DT, URH_MOD_FSK, true>(ctx, d_iq, n, dp, cls, o) : launch_dense_iq_t<DT, URH_MOD_FSK, false>(ctx, d_iq, n, dp, cls, o);
+}
+
+// The dense pass over the ASK / FSK capture d_iq[0, n) of dtype.
+static int launch_dense_iq(urh_ctx* ctx, int dtype, int mod_type, const void* d_iq, int64_t n, const UrhDemodParams& dp,
+                           const UrhClassify& cls, const DensePass& o) {
     switch (dtype) {
-        case URH_DT_I8: return launch_dense_iq_t<URH_DT_I8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
-        case URH_DT_U8: return launch_dense_iq_t<URH_DT_U8, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
-        case URH_DT_I16: return launch_dense_iq_t<URH_DT_I16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
-        case URH_DT_U16: return launch_dense_iq_t<URH_DT_U16, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine);
-        case URH_DT_F32: return launch_dense_iq_t<URH_DT_F32, MOD, DIG>(ctx, d_iq, n, dp, d_qad, cls, tol, tiles, staging, stage_cap, init_cls, cls_of_zero, has_halo, tile_stats, tile_lo, tile_hi, fine, spec);
+        case URH_DT_I8: return launch_dense_iq_dt<URH_DT_I8>(ctx, mod_type, d_iq, n, dp, cls, o);
+        case URH_DT_U8: return launch_dense_iq_dt<URH_DT_U8>(ctx, mod_type, d_iq, n, dp, cls, o);
+        case URH_DT_I16: return launch_dense_iq_dt<URH_DT_I16>(ctx, mod_type, d_iq, n, dp, cls, o);
+        case URH_DT_U16: return launch_dense_iq_dt<URH_DT_U16>(ctx, mod_type, d_iq, n, dp, cls, o);
+        case URH_DT_F32: return launch_dense_iq_dt<URH_DT_F32>(ctx, mod_type, d_iq, n, dp, cls, o);
         default: URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     }
 }
@@ -377,9 +393,7 @@ extern "C" int urh_afp_demod(urh_ctx* ctx, const void* d_iq, int dtype, int64_t 
     if (mod_type == URH_MOD_PSK) return urh_costas_demod(ctx, d_iq, dtype, n, dp.noise_sqrd, mod_order, costas_loop_bandwidth, d_out);
     UrhClassify cls;
     memset(&cls, 0, sizeof(cls));
-    if (mod_type == URH_MOD_ASK)
-        return launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_out, cls, 0, nullptr, nullptr, 0, nullptr, 0);
-    return launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_out, cls, 0, nullptr, nullptr, 0, nullptr, 0);
+    return launch_dense_iq(ctx, dtype, mod_type, d_iq, n, dp, cls, DensePass{d_out});
 }
 
 int urh_center_tiles_begin(urh_ctx* ctx, const float* d_x, const UrhTileStats* ts, int64_t n, int64_t* h_total);  // center.cu
@@ -401,75 +415,59 @@ extern "C" int urh_afp_demod_tiles(urh_ctx* ctx, const void* d_iq, int dtype, in
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     UrhTileStats* ts;
     URH_CHECK(urh_arena(ctx, (size_t)ntiles, &ts));
-    if (mod_type == URH_MOD_ASK)
-        URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, halo, ts)));
-    else
-        URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, halo, ts)));
+    URH_CHECK(launch_dense_iq(ctx, dtype, mod_type, d_iq, n, dp, cls, DensePass{d_qad_out, nullptr, halo, ts}));
     return urh_center_tiles_begin(ctx, d_qad_out, ts, n, h_kept);
 }
 
-// Shared tail of the two digitizer entry points: tile table + staging -> merged (state, length) rows.
-int urh_finish_local(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, int64_t* k);   // finish.cu
-int urh_finish_shard(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, int64_t global_offset, int64_t n_total, int64_t* k);   // finish.cu
-
-static int stage_cap_for(int tol) { return URH_TILE / (tol + 1) + 2; }
-
-// The digitizer's tables for ntiles tiles in the arena: tile summaries, cap staged candidates per tile, the initial state.
-static int digitizer_tables(urh_ctx* ctx, int64_t ntiles, int cap, UrhTileSummary** tiles, uint32_t** staging, int16_t** d_init) {
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, staging));
-    return urh_arena(ctx, 8, d_init);
+// Opening of every entry that builds a pulse table: no rows unless it succeeds.  args_ok: the entry's other required pointers are set.
+static int pulses_begin(urh_ctx* ctx, int64_t* k, bool args_ok = true) {
+    if (!k || !args_ok) return URH_ERR_INVALID;
+    *k = 0;
+    ctx->pulses_k = 0;
+    return URH_OK;
 }
 
-// The digitizer's dense pass over qad x[0, n), one warp per tile; binary symbols take the paired loads.  init: where the first tile
-// stores the digitizer's initial state (NULL: nowhere).  d_thr0: the threshold in device memory (then c0 is derived on the device);
-// ts: the demodulator's tile statistics, whose all-NOISE tiles are not read.
-static int launch_dense_qad(urh_ctx* ctx, const float* x, int64_t n, const UrhClassify& cls, int tol, UrhTileSummary* tiles,
-                            uint32_t* staging, int cap, int16_t* init, int c0, const float* d_thr0 = nullptr,
-                            const UrhTileStats* ts = nullptr) {
+// The digitizer's dense pass over the qad samples [s0, s1) at x, one warp per tile of dz's tables; binary symbols take the paired
+// loads.  Only the capture's first chunk (s0 == 0) stores the initial state.  d_thr0: the threshold in device memory (then c0 is
+// derived on the device); ts: the demodulator's tile statistics of the capture, whose all-NOISE tiles are not read.
+static int launch_dense_qad(urh_ctx* ctx, const UrhDigitizer& dz, const float* x, int64_t s0, int64_t s1, const UrhClassify& cls,
+                            const float* d_thr0 = nullptr, const UrhTileStats* ts = nullptr) {
+    const int64_t n = s1 - s0;
     const unsigned grid = (unsigned)urh_div_up(urh_div_up(n, URH_TILE), URH_WARPS_PER_BLOCK);
     const int vec_in = (((uintptr_t)x % 8) == 0) ? 1 : 0;
+    int16_t* init = s0 == 0 ? dz.d_init : nullptr;
+    const int c0 = d_thr0 ? 0 : host_classify(0.0f, cls);
+    if (ts) ts += s0 / URH_TILE;
     if (cls.order == 2)
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, tol, tiles, staging, cap, init,
-                   c0, d_thr0, ts);
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, dz.tol, dz.tiles, dz.staging,
+                   dz.cap, init, c0, d_thr0, ts);
     else
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, tol, tiles, staging, cap, init,
-                   c0, d_thr0, ts);
+        URH_LAUNCH(ctx, (k_dense_f32<SrcQad, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, x, n, vec_in, cls, dz.tol, dz.tiles, dz.staging,
+                   dz.cap, init, c0, d_thr0, ts);
     return URH_OK;
 }
 
 extern "C" int urh_grab_pulse_lens(urh_ctx* ctx, const float* d_qad, int64_t n, float center, uint16_t tolerance,
                                    int mod_type, uint32_t samples_per_symbol, uint8_t bits_per_symbol,
                                    float center_spacing, int64_t* k) {
-    if (!k) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k));
     if (n < 0) URH_FAIL(ctx, URH_ERR_INVALID, "negative length");
     if (n == 0) return URH_OK;  // pyx:416-417 -> empty (0,2) table
     urh_arena_reset(ctx);
     UrhClassify cls;
     URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
-    const int tol = tolerance;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
+    UrhDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol, urh_div_up(n, URH_TILE), false));
     URH_PROF_BEGIN(ctx);
-    URH_CHECK(launch_dense_qad(ctx, d_qad, n, cls, tol, tiles, staging, cap, d_init, host_classify(0.0f, cls)));
+    URH_CHECK(launch_dense_qad(ctx, dz, d_qad, 0, n, cls));
     URH_PROF_END(ctx);
-    return urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
+    return finish_tiles(ctx, dz, FinishShard::local(dz), k);
 }
 
 extern "C" int urh_demod_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, float noise_mag,
                                   int mod_type, float center, uint16_t tolerance, uint32_t samples_per_symbol,
                                   uint8_t bits_per_symbol, float center_spacing, float* d_qad_out, int64_t* k) {
-    if (!k) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k));
     if (n < 0) URH_FAIL(ctx, URH_ERR_INVALID, "negative length");
     if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     if (n == 0) return URH_OK;
@@ -491,29 +489,16 @@ extern "C" int urh_demod_digitize(urh_ctx* ctx, const void* d_iq, int dtype, int
     UrhClassify cls;
     URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
     const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
-    const int tol = tolerance;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
-    const int c0 = host_classify(0.0f, cls);
-    if (mod_type == URH_MOD_ASK)
-        URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0)));
-    else
-        URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0)));
-    return urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, k);
+    UrhDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol, urh_div_up(n, URH_TILE), false));
+    URH_CHECK(launch_dense_iq(ctx, dtype, mod_type, d_iq, n, dp, cls, DensePass{d_qad_out, &dz}));
+    return finish_tiles(ctx, dz, FinishShard::local(dz), k);
 }
 
 // ---- streaming through a ring of device slots (DESIGN.md §4.11) -----------------------------------------------------------------
 // A chunk is a whole number of tiles (the last one excepted; URH_FILTER_TILES), so every tile has the bounds and the arithmetic it
 // has in the resident call.  IQ kernels see the slot through a pointer shifted back by the chunk's first sample: they index the capture
 // globally, their tile range is the chunk's, and the halo sample (uploaded with the chunk) sits where the resident buffer holds it.
-int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
-                     int64_t rows_cap, int64_t* k);   // finish.cu
-
 // rows one digitizer pass over n samples can produce: firings are >= tol + 1 samples apart, plus the head and the tail row
 static int64_t rows_bound(int64_t n, int tol) { return n / (tol + 1) + 3; }
 
@@ -661,30 +646,23 @@ extern "C" int urh_stream_stats(urh_ctx* ctx, int64_t* h_out3) {
     return URH_OK;
 }
 
-// Per-chunk digitizer state of a streamed call: tile table and staging of one chunk, the carries between chunks, the row count.
+// The digitizer of a streamed call: tables for one chunk, reused chunk after chunk, the carries between chunks, the row count.
 struct StreamDigitizer {
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
+    UrhDigitizer dz;
     UrhChain* chain;
-    int cap, tol;
-    bool is_ask;
-    uint32_t sps;
-    int64_t n, rows, rows_all;
+    int64_t rows, rows_all;
     UrhArenaMark mark;
-    int init(urh_ctx* ctx, int64_t n_total, int64_t cs, int tolerance, bool ask, uint32_t samples_per_symbol) {
-        n = n_total; tol = tolerance; is_ask = ask; sps = samples_per_symbol; rows = 0;
-        cap = stage_cap_for(tol);
+    int init(urh_ctx* ctx, int64_t n, int64_t cs, int tol, bool ask, uint32_t sps) {
+        rows = 0;
         rows_all = rows_bound(n, tol);
-        URH_CHECK(digitizer_tables(ctx, cs / URH_TILE, cap, &tiles, &staging, &d_init));
+        URH_CHECK(dz.init(ctx, n, tol, ask, sps, cs / URH_TILE, true));
         URH_CHECK(urh_arena(ctx, 1, &chain));
-        URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
         mark = urh_arena_mark(ctx);
         return URH_OK;
     }
-    // the chunk [s0, s1) whose dense pass has filled tiles / staging
+    // the chunk [s0, s1) whose dense pass has filled the tables
     int finish(urh_ctx* ctx, int64_t s0, int64_t s1) {
-        const int64_t rc = rows_bound(s1 - s0, tol);
+        const int64_t rc = rows_bound(s1 - s0, dz.tol);
         const int64_t need = rows + rc;
         if (need > (int64_t)ctx->pulses_cap_rows) {
             int64_t grow = 2 * (int64_t)ctx->pulses_cap_rows;
@@ -693,7 +671,7 @@ struct StreamDigitizer {
         }
         urh_arena_release(ctx, mark);
         int64_t kc = 0;
-        URH_CHECK(urh_finish_chunk(ctx, s1 - s0, tol, is_ask, sps, tiles, staging, cap, d_init, chain, s0, n, rows, rc, &kc));
+        URH_CHECK(finish_tiles(ctx, dz, FinishShard::chunk(chain, s0, s1, dz.n, rows, rc), &kc));
         urh_stream_sample_free(ctx);
         rows += kc;
         return URH_OK;
@@ -718,29 +696,21 @@ static int stream_check(urh_ctx* ctx, int64_t n, int ring, int mod_type, int dty
     return URH_OK;
 }
 
-// IQ chunk computation on slot `s`: the dense kernels over tiles [s0 / TILE, ceil(s1 / TILE)) of the whole capture.
-template <bool DIG>
-static int stream_dense_iq(urh_ctx* ctx, int dtype, int mod_type, const char* d_src, int64_t src_slot, int64_t n, const UrhDemodParams& dp,
-                           float* qad_global, const UrhClassify& cls, int tol, StreamDigitizer* dz, int64_t s0, int64_t s1, int s,
-                           UrhTileStats* ts = nullptr, const UrhFine& fine = UrhFine{}) {
-    const int b = urh_iq_bytes(dtype);
-    const void* iq = d_src + s * src_slot + URH_STREAM_PAD - s0 * b;   // sample i of the capture at iq + i * b for i in [s0 - 1, s1)
-    const int64_t t0 = s0 / URH_TILE, t1 = urh_div_up(s1, URH_TILE);
-    UrhTileSummary* tiles = dz ? dz->tiles - t0 : nullptr;
-    uint32_t* staging = dz ? dz->staging - t0 * dz->cap : nullptr;
-    const int cap = dz ? dz->cap : 0;
-    int16_t* init = dz ? dz->d_init : nullptr;
-    const int c0 = DIG ? host_classify(0.0f, cls) : 0;
-    if (mod_type == URH_MOD_ASK)
-        return launch_dense_iq_m<URH_MOD_ASK, DIG>(ctx, dtype, iq, n, dp, qad_global, cls, tol, tiles, staging, cap, init, c0, 0, ts, t0, t1, fine);
-    return launch_dense_iq_m<URH_MOD_FSK, DIG>(ctx, dtype, iq, n, dp, qad_global, cls, tol, tiles, staging, cap, init, c0, 0, ts, t0, t1, fine);
-}
-
-// Digitizer dense pass over qad [s0, s1) at x (local view: chunk-relative tiles; only chunk 0 sets the initial state).
-static int stream_dense_qad(urh_ctx* ctx, const float* x, int64_t s0, int64_t s1, const UrhClassify& cls, StreamDigitizer& dz,
-                            const float* d_thr0 = nullptr, const UrhTileStats* ts = nullptr) {
-    return launch_dense_qad(ctx, x, s1 - s0, cls, dz.tol, dz.tiles, dz.staging, dz.cap, s0 == 0 ? dz.d_init : nullptr,
-                            d_thr0 ? 0 : host_classify(0.0f, cls), d_thr0, ts ? ts + s0 / URH_TILE : nullptr);
+// Dense pass over the IQ chunk w in the ring slot at `slot`: tiles [k0 / TILE, ceil(k1 / TILE)) of the whole capture; o.qad and
+// o.tile_stats are indexed globally, o.dz's tables hold the chunk's tiles.
+static int stream_dense_iq(urh_ctx* ctx, int dtype, int mod_type, const char* slot, int64_t n, const UrhDemodParams& dp,
+                           const UrhClassify& cls, const UrhWindow& w, DensePass o) {
+    const void* iq = slot + URH_STREAM_PAD - w.k0 * urh_iq_bytes(dtype);   // sample i of the capture at iq + i * b for i in [k0 - 1, k1)
+    o.tile_lo = w.k0 / URH_TILE;
+    o.tile_hi = urh_div_up(w.k1, URH_TILE);
+    UrhDigitizer view;
+    if (o.dz) {
+        view = *o.dz;
+        view.tiles -= o.tile_lo;
+        view.staging -= o.tile_lo * view.cap;
+        o.dz = &view;
+    }
+    return launch_dense_iq(ctx, dtype, mod_type, iq, n, dp, cls, o);
 }
 
 // ---- one-call paths: every stage enqueued on the context stream, ONE synchronisation at the end -----------------------------
@@ -758,9 +728,7 @@ extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, con
                                   float noise_mag, int mod_type, float center, uint16_t tolerance, uint32_t samples_per_symbol,
                                   uint8_t bits_per_symbol, float center_spacing, float* d_qad_out, int64_t global_offset,
                                   int64_t n_total, int64_t* k) {
-    if (!k) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k));
     if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "empty shard");
     if (mod_type != URH_MOD_ASK && mod_type != URH_MOD_FSK) URH_FAIL(ctx, URH_ERR_INVALID, "sharded path: ASK / FSK only");
     if (!d_qad_in && urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
@@ -768,36 +736,32 @@ extern "C" int urh_shard_digitize(urh_ctx* ctx, const void* d_iq, int dtype, con
     urh_arena_reset(ctx);
     UrhClassify cls;
     URH_CHECK(fill_classify(ctx, &cls, mod_type, center, bits_per_symbol, center_spacing));
-    const int tol = tolerance;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    int16_t* d_init;
-    URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
-    URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
-    const int c0 = host_classify(0.0f, cls);
+    UrhDigitizer dz;
+    URH_CHECK(dz.init(ctx, n, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol, urh_div_up(n, URH_TILE), true));
     if (d_qad_in) {
         URH_PROF_BEGIN(ctx);
-        URH_CHECK(launch_dense_qad(ctx, d_qad_in, n, cls, tol, tiles, staging, cap, d_init, c0));
+        URH_CHECK(launch_dense_qad(ctx, dz, d_qad_in, 0, n, cls));
         URH_PROF_END(ctx);
     } else {
         const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
-        if (mod_type == URH_MOD_ASK)
-            URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0, has_halo)));
-        else
-            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, true>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, d_init, c0, has_halo)));
+        URH_CHECK(launch_dense_iq(ctx, dtype, mod_type, d_iq, n, dp, cls, DensePass{d_qad_out, &dz, has_halo}));
     }
-    return urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, k);
+    return finish_tiles(ctx, dz, FinishShard::shard(ctx, dz, global_offset, n_total), k);
 }
 
-// demod (ASK / FSK) + capture-wide detect_center + digitize (binary symbols) in one call (BASELINE configs[1]).
-// sharded != 0: this rank's shard of a capture spread over the context's NCCL communicator (has_halo as urh_shard_digitize).
-// *center_state: 0 = detect_center finds no center (None; *k = 0), 1 = *center is valid, 2 = the device could not decide
-// (a tie between histogram peaks whose order numpy's argsort defines, or more than 6000 bins): d_qad_out is valid, the
-// caller finishes through the stepwise entry points (urh_center_window_stats / urh_center_histogram_tiles / urh_grab_pulse_lens).
-// sc != NULL: the IQ is streamed from sc->h_iq through a ring (d_iq unused), qad stays resident in d_qad_out (mirrored to sc->h_qad),
-// and the digitizer runs chunk by chunk over it with chained finishes, so no table grows with n but the tile statistics.
+// ---- the detect-center step: demod (ASK / FSK) + capture-wide detect_center + digitize (binary symbols) in one call ---------------
+// The step's results in the context's pinned mailbox, from its word 40 on (its first words are urh_read_i64's), typed as the
+// copies that land in them.
+struct CenterMail {
+    double center;
+    int state, pad;
+    int64_t cert[3];       // urh_center_plan_certify_stats: {certified, -, straddle mass}
+    int64_t kept;          // kept samples (streamed step)
+    unsigned int redone;   // speculated tiles the qad digitizer re-read
+};
+static_assert(40 * sizeof(int64_t) + sizeof(CenterMail) <= 64 * sizeof(int64_t), "CenterMail outgrows the mailbox");
+
+// sc: the IQ is streamed from sc->h_iq through a ring of sc->ring slots, qad mirrored to sc->h_qad, sc->kept = kept samples
 struct StreamCenter {
     int ring;
     int64_t chunk_samples;
@@ -805,174 +769,220 @@ struct StreamCenter {
     float* h_qad;
     int64_t* kept;
 };
+
+// What the phases of one step share.
+struct CenterStep {
+    const void* d_iq;   // the resident capture, or the scratch the host capture is uploaded into (streamed: unused)
+    int dtype, mod_type, has_halo;
+    int64_t n, ntiles;
+    float* d_qad;
+    UrhDemodParams dp;
+    UrhClassify cls;    // binary digitizer, threshold from device memory (the demodulation reads none of it)
+    UrhTileStats* ts;
+    UrhFine fine;       // fine.gh == nullptr: not collected
+    bool speculate;
+    UrhSpec spec;
+    UrhDigitizer dz;    // the tables over the whole capture (not streamed: the chunked digitizer has its own)
+};
+
+// Set-up: tile statistics; the fine histogram of the kept samples per slab of tiles, which lets detect_center certify its peaks
+// without a histogram pass over qad (center.cu, k_center_certify); the digitizer's tables; speculative digitizing (UrhSpec,
+// DESIGN.md §4.4.1): the demodulation pass digitizes its fast tiles at a guessed threshold, the qad digitizer re-reads only the
+// tiles whose margin does not prove the classes at the detected center.
+static int center_setup(urh_ctx* ctx, CenterStep& S, bool certify, bool tables, const char* forced_guess, int tol, uint32_t sps) {
+    URH_CHECK(urh_arena(ctx, (size_t)S.ntiles, &S.ts));
+    if (certify) {
+        S.fine.slab_tiles = urh_div_up(S.ntiles, URH_FINE_SLABS);
+        if (S.fine.slab_tiles < URH_WARPS_PER_BLOCK) S.fine.slab_tiles = URH_WARPS_PER_BLOCK;   // a block straddles at most one slab edge
+        const int64_t nslabs = urh_div_up(S.ntiles, S.fine.slab_tiles);
+        URH_CHECK(urh_arena(ctx, (size_t)(nslabs * URH_FINE_NB), &S.fine.gh));
+        URH_CUDA(ctx, cudaMemsetAsync(S.fine.gh, 0, (size_t)(nslabs * URH_FINE_NB) * sizeof(unsigned int), ctx->stream));
+        S.fine.scale = (S.mod_type == URH_MOD_FSK) ? 512.0f : 4096.0f;
+        S.fine.off = (S.mod_type == URH_MOD_FSK) ? 2048.0f : 0.0f;
+    }
+    S.cls.noise_value = urh_noise_value(S.mod_type);
+    S.cls.order = 2;
+    if (tables) URH_CHECK(S.dz.init(ctx, S.n, tol, S.mod_type == URH_MOD_ASK, sps, S.ntiles, false));
+    if (S.speculate) {
+        float* tg;
+        URH_CHECK(urh_arena(ctx, 1, &tg));
+        URH_CHECK(urh_arena(ctx, 1, &S.spec.redone));
+        URH_CHECK(urh_arena(ctx, (size_t)S.ntiles, &S.spec.margin));
+        S.spec.tg = tg;
+        URH_LAUNCH(ctx, k_speculate_guess, 1, URH_GUESS_THREADS, 0, (const float2*)S.d_iq, S.n, S.dp.noise_sqrd, forced_guess ? 1 : 0,
+                   forced_guess ? strtof(forced_guess, nullptr) : 0.0f, tg, S.spec.redone);
+    }
+    return URH_OK;
+}
+
+// Demodulation of tiles [t0, t1) of the capture at S.d_iq (speculating: the fast tiles are also digitized at the guess).
+static int center_demod(urh_ctx* ctx, CenterStep& S, int64_t t0, int64_t t1) {
+    DensePass o{S.d_qad, nullptr, S.has_halo, S.ts, t0, t1, S.fine};
+    if (S.speculate) {
+        o.dz = &S.dz;
+        o.spec = &S.spec;
+    }
+    return launch_dense_iq(ctx, S.dtype, S.mod_type, S.d_iq, S.n, S.dp, S.cls, o);
+}
+
+// Demodulation of a capture in (pinned) host memory: it is uploaded into S.d_iq in chunks on the copy stream and every chunk is
+// demodulated as soon as it has landed, so the demodulation pass hides behind the PCIe transfer.
+static int center_demod_host(urh_ctx* ctx, CenterStep& S, const void* h_iq, int64_t chunk_samples) {
+    const int64_t chunk_tiles = chunk_samples >= URH_TILE ? chunk_samples / URH_TILE : 1;
+    const size_t sample_bytes = (size_t)urh_iq_bytes(S.dtype);
+    int chunk_no = 0;
+    for (int64_t t0 = 0; t0 < S.ntiles; t0 += chunk_tiles, chunk_no++) {
+        const int64_t t1 = (t0 + chunk_tiles < S.ntiles) ? t0 + chunk_tiles : S.ntiles;
+        const int64_t s0 = t0 * URH_TILE, s1 = (t1 * URH_TILE < S.n) ? t1 * URH_TILE : S.n;
+        cudaEvent_t ev = ctx->ev_copy[chunk_no & 1];
+        URH_CUDA(ctx, cudaMemcpyAsync((char*)S.d_iq + (size_t)s0 * sample_bytes, (const char*)h_iq + (size_t)s0 * sample_bytes,
+                                      (size_t)(s1 - s0) * sample_bytes, cudaMemcpyHostToDevice, ctx->copy_stream[0]));
+        URH_CUDA(ctx, cudaEventRecord(ev, ctx->copy_stream[0]));
+        URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev, 0));
+        URH_CHECK(center_demod(ctx, S, t0, t1));
+    }
+    return URH_OK;
+}
+
+// Demodulation of a capture streamed from host memory through the ring R: qad stays resident in S.d_qad (mirrored to sc.h_qad).
+// *cs = the chunk samples of the call.
+static int center_demod_ring(urh_ctx* ctx, CenterStep& S, const StreamCenter& sc, int tol, StreamRing& R, int64_t* cs) {
+    const StreamSizes z = stream_sizes(S.n, S.dtype, tol, sc.chunk_samples, sc.ring, URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE);
+    *cs = z.cs;
+    const int64_t slot = r256(z.src_slot);
+    URH_CHECK(R.init(ctx, sc.ring, sc.ring * slot));
+    std::vector<UrhWindow> win;
+    URH_CHECK(urh_filter_windows(URH_FILTER_TILES, S.n, S.n, 1, 0, sc.chunk_samples, nullptr, nullptr, 0, win));
+    return stream_run(ctx, win, R, (const char*)sc.h_iq, urh_iq_bytes(S.dtype), R.mem, slot, sc.h_qad != nullptr,
+                      [&](int64_t, const UrhWindow& w, int s) {
+                          return stream_dense_iq(ctx, S.dtype, S.mod_type, R.mem + s * slot, S.n, S.dp, S.cls, w,
+                                                 DensePass{S.d_qad, nullptr, 0, S.ts, 0, -1, S.fine});
+                      },
+                      [&](int64_t, const UrhWindow& w, int, cudaStream_t cp) {   // from the resident qad
+                          URH_CUDA(ctx, cudaMemcpyAsync(sc.h_qad + w.k0, S.d_qad + w.k0, (size_t)(w.k1 - w.k0) * sizeof(float),
+                                                        cudaMemcpyDeviceToHost, cp));
+                          return URH_OK;
+                      },
+                      place_after_pad, true);
+}
+
+// center, state and certificate of the plan -> the mailbox, on the stream
+static int center_copy_results(urh_ctx* ctx, const CenterPlan* plan, CenterMail* mail) {
+    const double* d_center;
+    const int* d_state;
+    urh_center_plan_result(ctx, plan, nullptr, &d_center, &d_state);
+    URH_CUDA(ctx, cudaMemcpyAsync(&mail->center, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync(&mail->state, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    return urh_center_plan_certify_stats(ctx, plan, mail->cert);
+}
+
+// Digitizer tail, resident tables: one pass over qad at the detected center (after speculation most tiles only need their margin
+// checked: one resident wave of warps loops over them), the results copied, then the finish, which synchronises.
+static int center_digitize_resident(urh_ctx* ctx, CenterStep& S, const CenterPlan* plan, const FinishShard& sh, CenterMail* mail,
+                                    int64_t* rows) {
+    const float* d_centerf;
+    urh_center_plan_result(ctx, plan, &d_centerf, nullptr, nullptr);
+    URH_CUDA(ctx, cudaMemsetAsync(S.dz.d_init, 0, 16, ctx->stream));
+    const int vec_in = (((uintptr_t)S.d_qad % 8) == 0) ? 1 : 0;
+    int64_t grid = urh_div_up(S.ntiles, URH_WARPS_PER_BLOCK);
+    if (S.speculate) {
+        int per_sm = 0;
+        URH_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dense_f32<SrcQad2, float>, URH_WARPS_PER_BLOCK * 32, 0));
+        const int64_t resident = (int64_t)ctx->sm_count * (per_sm > 0 ? per_sm : 1);
+        if (grid > resident) grid = resident;
+    }
+    URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)grid, URH_WARPS_PER_BLOCK * 32, 0, (const float*)S.d_qad, S.n, vec_in, S.cls,
+               S.dz.tol, S.dz.tiles, S.dz.staging, S.dz.cap, S.dz.d_init, 0, d_centerf, (const UrhTileStats*)S.ts, S.spec);
+    URH_CHECK(center_copy_results(ctx, plan, mail));
+    mail->redone = 0u;
+    if (S.speculate) URH_CUDA(ctx, cudaMemcpyAsync(&mail->redone, S.spec.redone, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+    return finish_tiles(ctx, S.dz, sh, rows);
+}
+
+// Digitizer tail, streamed: the chunked digitizer synchronises per chunk anyway, so learn the state first and digitize (chunks of
+// cs samples with chained finishes, so no table grows with n but the tile statistics) only when there is a center.
+static int center_digitize_chunked(urh_ctx* ctx, CenterStep& S, const CenterPlan* plan, int64_t cs, int tol, uint32_t sps,
+                                   CenterMail* mail, int64_t* rows) {
+    URH_CHECK(center_copy_results(ctx, plan, mail));
+    URH_CUDA(ctx, cudaMemcpyAsync(&mail->kept, (const int64_t*)ctx->center_prefix + S.ntiles, sizeof(int64_t), cudaMemcpyDeviceToHost,
+                                  ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (mail->state != 1) return URH_OK;
+    const float* d_centerf;
+    urh_center_plan_result(ctx, plan, &d_centerf, nullptr, nullptr);
+    StreamDigitizer sd;
+    URH_CHECK(sd.init(ctx, S.n, cs, tol, S.mod_type == URH_MOD_ASK, sps));
+    for (int64_t s0 = 0; s0 < S.n; s0 += cs) {
+        const int64_t s1 = s0 + cs < S.n ? s0 + cs : S.n;
+        URH_CHECK(launch_dense_qad(ctx, sd.dz, S.d_qad + s0, s0, s1, S.cls, d_centerf, S.ts));
+        URH_CHECK(sd.finish(ctx, s0, s1));
+    }
+    *rows = sd.rows;
+    return URH_OK;
+}
+
+// (BASELINE configs[1]) sharded: this rank's shard of a capture spread over the context's NCCL communicator (has_halo as urh_shard_digitize).
+// *center_state: 0 = detect_center finds no center (None; *k = 0), 1 = *center is valid, 2 = the device could not decide
+// (a tie between histogram peaks whose order numpy's argsort defines, or more than 6000 bins): d_qad_out is valid, the
+// caller finishes through the stepwise entry points (urh_center_window_stats / urh_center_histogram_tiles / urh_grab_pulse_lens).
+// The IQ comes from d_iq, from h_iq uploaded into d_iq in chunks of chunk_samples, or from sc (d_iq unused).
 static int demod_center_digitize_impl(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, int has_halo, float noise_mag, int mod_type,
                                       uint16_t tolerance, uint32_t samples_per_symbol, int64_t max_size, float* d_qad_out, bool sharded,
                                       int64_t global_offset, int64_t n_total, double* center, int* center_state, int64_t* k,
                                       const void* h_iq = nullptr, int64_t chunk_samples = 0, const StreamCenter* sc = nullptr) {
-    if (!k || !center || !center_state) return URH_ERR_INVALID;
-    *k = 0;
+    URH_CHECK(pulses_begin(ctx, k, center && center_state));
     *center = 0.0;
     *center_state = 0;
-    ctx->pulses_k = 0;
     if (n <= 2 || (mod_type != URH_MOD_ASK && mod_type != URH_MOD_FSK) || !d_qad_out)
         URH_FAIL(ctx, URH_ERR_INVALID, "demod_center_digitize: ASK/FSK, n > 2 and a qad buffer are required");
     if (urh_iq_bytes(dtype) == 0) URH_FAIL(ctx, URH_ERR_DTYPE, "Unsupported dtype");
     if (sharded && !ctx->nccl_comm) URH_FAIL(ctx, URH_ERR_INVALID, "NCCL communicator not initialised (urh_nccl_init)");
+    // the step's switches, read on every call (the tests compare the paths they select): $URH_B200_CENTER_NO_CERTIFY=1 forces the
+    // histogram pass over qad, $URH_B200_NO_SPECULATE=1 turns speculation off, $URH_B200_SPECULATE_GUESS=<float> replaces the guess
+    const bool no_certify = getenv("URH_B200_CENTER_NO_CERTIFY") != nullptr, no_speculate = getenv("URH_B200_NO_SPECULATE") != nullptr;
+    const char* forced_guess = getenv("URH_B200_SPECULATE_GUESS");
     urh_arena_reset(ctx);
     URH_TL_RESET(ctx);
     URH_TL_MARK(ctx, "step start");
-    const UrhDemodParams dp = make_demod_params(noise_mag, mod_type, dtype);
-    UrhClassify cls;
-    memset(&cls, 0, sizeof(cls));
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    UrhTileStats* ts;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &ts));
-    // fine histogram of the kept samples, per slab of tiles: lets detect_center certify its peaks without a histogram pass over qad
-    // (center.cu, k_center_certify).  Not collected for a sharded capture; $URH_B200_CENTER_NO_CERTIFY=1 forces the histogram pass.
-    const bool no_certify = getenv("URH_B200_CENTER_NO_CERTIFY") != nullptr;   // read per call: tests compare both paths
-    UrhFine fine = {};
-    if (!sharded && !no_certify) {
-        fine.slab_tiles = urh_div_up(ntiles, URH_FINE_SLABS);
-        if (fine.slab_tiles < URH_WARPS_PER_BLOCK) fine.slab_tiles = URH_WARPS_PER_BLOCK;   // a block straddles at most one slab edge
-        const int64_t nslabs = urh_div_up(ntiles, fine.slab_tiles);
-        URH_CHECK(urh_arena(ctx, (size_t)(nslabs * URH_FINE_NB), &fine.gh));
-        URH_CUDA(ctx, cudaMemsetAsync(fine.gh, 0, (size_t)(nslabs * URH_FINE_NB) * sizeof(unsigned int), ctx->stream));
-        fine.scale = (mod_type == URH_MOD_FSK) ? 512.0f : 4096.0f;
-        fine.off = (mod_type == URH_MOD_FSK) ? 2048.0f : 0.0f;
-    }
-    // h_iq != NULL: the capture is in (pinned) host memory.  It is uploaded in chunks on the copy stream and every chunk is
-    // demodulated as soon as it has landed, so the demodulation pass hides behind the PCIe transfer.
-    const int64_t chunk_tiles = (h_iq && chunk_samples > 0) ? (chunk_samples >= URH_TILE ? chunk_samples / URH_TILE : 1) : ntiles;
-    const size_t sample_bytes = (size_t)urh_iq_bytes(dtype);
-    StreamRing ring;
-    int64_t scs = 0;
-    if (sc) {
-        const StreamSizes z = stream_sizes(n, dtype, tolerance, sc->chunk_samples, sc->ring, URH_STREAM_ENTRY_DEMOD_CENTER_DIGITIZE);
-        scs = z.cs;
-        URH_CHECK(ring.init(ctx, sc->ring, sc->ring * r256(z.src_slot)));
-        const int64_t slot = r256(z.src_slot);
-        std::vector<UrhWindow> win;
-        URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, sc->chunk_samples, nullptr, nullptr, 0, win));
-        URH_CHECK(stream_run(ctx, win, ring, (const char*)sc->h_iq, urh_iq_bytes(dtype), ring.mem, slot, sc->h_qad != nullptr,
-                             [&](int64_t, const UrhWindow& w, int s) {
-                                 return stream_dense_iq<false>(ctx, dtype, mod_type, ring.mem, slot, n, dp, d_qad_out, cls, 0, nullptr, w.k0, w.k1,
-                                                               s, ts, fine);
-                             },
-                             [&](int64_t, const UrhWindow& w, int, cudaStream_t cp) {   // from the resident qad
-                                 URH_CUDA(ctx, cudaMemcpyAsync(sc->h_qad + w.k0, d_qad_out + w.k0, (size_t)(w.k1 - w.k0) * sizeof(float),
-                                                               cudaMemcpyDeviceToHost, cp));
-                                 return URH_OK;
-                             },
-                             place_after_pad, true));
-    }
-    // the digitizer's tables, filled by the qad digitizer after the center chain, and by the speculative pass before it
-    cls.noise_value = urh_noise_value(mod_type);
-    cls.order = 2;
-    const int tol = tolerance;
-    const int cap = stage_cap_for(tol);
-    UrhTileSummary* tiles = nullptr;
-    uint32_t* staging = nullptr;
-    int16_t* d_init = nullptr;
-    if (!sc) URH_CHECK(digitizer_tables(ctx, ntiles, cap, &tiles, &staging, &d_init));
-    // speculative digitizing (UrhSpec, DESIGN.md §4.4.1): the pass digitizes its fast tiles at a guessed threshold, the qad digitizer
-    // re-reads only the tiles whose margin does not prove the classes at the detected center.  The resident single-GPU float32 FSK
-    // step only; $URH_B200_NO_SPECULATE=1 turns it off, $URH_B200_SPECULATE_GUESS=<float> replaces the guess (read per call).
-    const bool speculate = !sharded && !h_iq && !sc && mod_type == URH_MOD_FSK && dtype == URH_DT_F32 &&
-                           getenv("URH_B200_NO_SPECULATE") == nullptr;
-    UrhSpec spec = {};
-    if (speculate) {
-        float* tg;
-        URH_CHECK(urh_arena(ctx, 1, &tg));
-        URH_CHECK(urh_arena(ctx, 1, &spec.redone));
-        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &spec.margin));
-        spec.tg = tg;
-        const char* forced = getenv("URH_B200_SPECULATE_GUESS");
-        URH_LAUNCH(ctx, k_speculate_guess, 1, URH_GUESS_THREADS, 0, (const float2*)d_iq, n, dp.noise_sqrd, forced ? 1 : 0,
-                   forced ? strtof(forced, nullptr) : 0.0f, tg, spec.redone);
-    }
-    int chunk_no = 0;
-    for (int64_t t0 = 0; t0 < (sc ? 0 : ntiles); t0 += chunk_tiles, chunk_no++) {
-        const int64_t t1 = (t0 + chunk_tiles < ntiles) ? t0 + chunk_tiles : ntiles;
-        if (h_iq) {
-            const int64_t s0 = t0 * URH_TILE, s1 = (t1 * URH_TILE < n) ? t1 * URH_TILE : n;
-            cudaEvent_t ev = ctx->ev_copy[chunk_no & 1];
-            URH_CUDA(ctx, cudaMemcpyAsync((char*)d_iq + (size_t)s0 * sample_bytes, (const char*)h_iq + (size_t)s0 * sample_bytes,
-                                          (size_t)(s1 - s0) * sample_bytes, cudaMemcpyHostToDevice, ctx->copy_stream[0]));
-            URH_CUDA(ctx, cudaEventRecord(ev, ctx->copy_stream[0]));
-            URH_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ev, 0));
-        }
-        if (mod_type == URH_MOD_ASK)
-            URH_CHECK((launch_dense_iq_m<URH_MOD_ASK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, 0, nullptr, nullptr, 0, nullptr, 0, has_halo, ts, t0, t1, fine)));
-        else
-            URH_CHECK((launch_dense_iq_m<URH_MOD_FSK, false>(ctx, dtype, d_iq, n, dp, d_qad_out, cls, tol, tiles, staging, cap, nullptr, 0, has_halo,
-                                                             ts, t0, t1, fine, speculate ? &spec : nullptr)));
-    }
+    CenterStep S = {};
+    S.d_iq = d_iq; S.dtype = dtype; S.mod_type = mod_type; S.has_halo = has_halo;
+    S.n = n; S.ntiles = urh_div_up(n, URH_TILE);
+    S.d_qad = d_qad_out;
+    S.dp = make_demod_params(noise_mag, mod_type, dtype);
+    // the fine histogram is not collected for a sharded capture; speculation: the resident single-GPU float32 FSK step only
+    S.speculate = !sharded && !h_iq && !sc && mod_type == URH_MOD_FSK && dtype == URH_DT_F32 && !no_speculate;
+    URH_CHECK(center_setup(ctx, S, !sharded && !no_certify, !sc, forced_guess, tolerance, samples_per_symbol));
+
+    StreamRing ring;   // (freed when the step returns)
+    int64_t cs = 0;
+    if (sc) URH_CHECK(center_demod_ring(ctx, S, *sc, tolerance, ring, &cs));
+    else if (h_iq) URH_CHECK(center_demod_host(ctx, S, h_iq, chunk_samples));
+    else URH_CHECK(center_demod(ctx, S, 0, S.ntiles));
+
     CenterPlan* plan = nullptr;
-    URH_CHECK(urh_center_chain(ctx, d_qad_out, n, ts, max_size, sharded ? ctx->nccl_rank : 0, sharded ? ctx->nccl_world : 1,
-                               fine.gh ? &fine : nullptr, &plan));
-    const float* d_centerf;
-    const double* d_center;
-    const int* d_state;
-    urh_center_plan_result(ctx, plan, &d_centerf, &d_center, &d_state);
-    // digitizer pass over qad, threshold read from device memory
+    URH_CHECK(urh_center_chain(ctx, d_qad_out, n, S.ts, max_size, sharded ? ctx->nccl_rank : 0, sharded ? ctx->nccl_world : 1,
+                               S.fine.gh ? &S.fine : nullptr, &plan));
+
+    CenterMail* mail = (CenterMail*)(ctx->h_mail + 40);
     int64_t rows = 0;
-    if (sc) {
-        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
-        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 45, (const int64_t*)ctx->center_prefix + ntiles, sizeof(int64_t), cudaMemcpyDeviceToHost,
-                                      ctx->stream));
-        // the chunked digitizer synchronises per chunk anyway: learn the state first and digitize only when there is a center
-        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        int st0 = 0;
-        memcpy(&st0, ctx->h_mail + 41, sizeof(int));
-        if (st0 == 1) {
-            StreamDigitizer dz;
-            URH_CHECK(dz.init(ctx, n, scs, tol, mod_type == URH_MOD_ASK, samples_per_symbol));
-            for (int64_t s0 = 0; s0 < n; s0 += scs) {
-                const int64_t s1 = s0 + scs < n ? s0 + scs : n;
-                URH_CHECK(stream_dense_qad(ctx, d_qad_out + s0, s0, s1, cls, dz, d_centerf, ts));
-                URH_CHECK(dz.finish(ctx, s0, s1));
-            }
-            rows = dz.rows;
-        }
-        *sc->kept = ctx->h_mail[45];
-    } else {
-        URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
-        const int vec_in = (((uintptr_t)d_qad_out % 8) == 0) ? 1 : 0;
-        // after speculation most tiles only need their margin checked: one resident wave of warps loops over them (k_dense_f32)
-        int64_t grid = urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
-        if (speculate) {
-            int per_sm = 0;
-            URH_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dense_f32<SrcQad2, float>, URH_WARPS_PER_BLOCK * 32, 0));
-            const int64_t resident = (int64_t)ctx->sm_count * (per_sm > 0 ? per_sm : 1);
-            if (grid > resident) grid = resident;
-        }
-        URH_LAUNCH(ctx, (k_dense_f32<SrcQad2, float>), (unsigned)grid, URH_WARPS_PER_BLOCK * 32, 0,
-                   (const float*)d_qad_out, n, vec_in, cls, tol, tiles, staging, cap, d_init, 0, d_centerf, (const UrhTileStats*)ts, spec);
-        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 40, d_center, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 41, d_state, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CHECK(urh_center_plan_certify_stats(ctx, plan, ctx->h_mail + 42));
-        ctx->h_mail[46] = 0;
-        if (speculate) URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail + 46, spec.redone, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
-        if (sharded)
-            URH_CHECK(urh_finish_shard(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, global_offset, n_total, &rows));
-        else
-            URH_CHECK(urh_finish_local(ctx, n, tol, mod_type == URH_MOD_ASK, samples_per_symbol, tiles, staging, cap, d_init, &rows));
-    }
-    // the finish synchronised the stream: the two scalars have landed
-    memcpy(center, ctx->h_mail + 40, sizeof(double));
-    int st = 0;
-    memcpy(&st, ctx->h_mail + 41, sizeof(int));
-    *center_state = st;
-    ctx->center_cert[0] = ctx->h_mail[42];
-    ctx->center_cert[1] = fine.gh ? URH_FINE_NB : 0;
-    ctx->center_cert[2] = ctx->h_mail[44];
-    const int64_t redone = (spec.hi > spec.lo) ? ctx->h_mail[46] : 0;
-    ctx->spec_stats[0] = spec.hi - spec.lo;
-    ctx->spec_stats[1] = spec.hi - spec.lo - redone;
+    if (sc)
+        URH_CHECK(center_digitize_chunked(ctx, S, plan, cs, tolerance, samples_per_symbol, mail, &rows));
+    else
+        URH_CHECK(center_digitize_resident(ctx, S, plan, sharded ? FinishShard::shard(ctx, S.dz, global_offset, n_total) : FinishShard::local(S.dz),
+                                           mail, &rows));
+
+    // the finish or the chunked tail synchronised the stream: the results have landed
+    *center = mail->center;
+    *center_state = mail->state;
+    if (sc) *sc->kept = mail->kept;
+    ctx->center_cert[0] = mail->cert[0];
+    ctx->center_cert[1] = S.fine.gh ? URH_FINE_NB : 0;
+    ctx->center_cert[2] = mail->cert[2];
+    const int64_t redone = (S.spec.hi > S.spec.lo) ? mail->redone : 0;
+    ctx->spec_stats[0] = S.spec.hi - S.spec.lo;
+    ctx->spec_stats[1] = S.spec.hi - S.spec.lo - redone;
     ctx->spec_stats[2] = redone;
-    if (st != 1) {
+    if (mail->state != 1) {
         ctx->pulses_k = 0;
         rows = 0;
     }
@@ -1045,8 +1055,8 @@ extern "C" int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, i
     URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, chunk_samples, nullptr, nullptr, 0, win));
     return stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, r256(z.src_slot), true,
                       [&](int64_t, const UrhWindow& w, int s) {
-                          return stream_dense_iq<false>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp, d_qad + s * z.cs - w.k0, cls, 0,
-                                                        nullptr, w.k0, w.k1, s);
+                          return stream_dense_iq(ctx, dtype, mod_type, d_src + s * r256(z.src_slot), n, dp, cls, w,
+                                                 DensePass{d_qad + s * z.cs - w.k0});
                       },
                       contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad, 4), place_after_pad);
 }
@@ -1054,9 +1064,7 @@ extern "C" int urh_afp_demod_stream(urh_ctx* ctx, const void* h_iq, int dtype, i
 extern "C" int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qad_on_device, int64_t n, float center, uint16_t tolerance,
                                           int mod_type, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
                                           int64_t chunk_samples, int ring, int64_t* k) {
-    if (!k || !qad) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k, qad != nullptr));
     URH_CHECK(stream_check(ctx, n, ring, mod_type, 0, false));
     urh_arena_reset(ctx);
     UrhClassify cls;
@@ -1065,28 +1073,26 @@ extern "C" int urh_grab_pulse_lens_stream(urh_ctx* ctx, const float* qad, int qa
                                        URH_STREAM_ENTRY_GRAB_PULSE_LENS | (qad_on_device ? URH_STREAM_QAD_ON_DEVICE : 0));
     StreamRing R;
     URH_CHECK(R.init(ctx, ring, z.ring_bytes));
-    StreamDigitizer dz;
-    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
+    StreamDigitizer sd;
+    URH_CHECK(sd.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
     char* d_src = R.mem;
     std::vector<UrhWindow> win;
     URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
     URH_CHECK(stream_run(ctx, win, R, qad_on_device ? nullptr : (const char*)qad, 4, d_src, r256(z.src_slot), false,
                          [&](int64_t, const UrhWindow& w, int s) {
                              const float* x = qad_on_device ? qad + w.k0 : (const float*)(d_src + s * r256(z.src_slot) + URH_STREAM_PAD);
-                             URH_CHECK(stream_dense_qad(ctx, x, w.k0, w.k1, cls, dz));
-                             return dz.finish(ctx, w.k0, w.k1);
+                             URH_CHECK(launch_dense_qad(ctx, sd.dz, x, w.k0, w.k1, cls));
+                             return sd.finish(ctx, w.k0, w.k1);
                          },
                          no_download, place_after_pad));
-    *k = dz.rows;
+    *k = sd.rows;
     return URH_OK;
 }
 
 extern "C" int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, int mod_type, float center,
                                          uint16_t tolerance, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
                                          int64_t chunk_samples, int ring, float* h_qad_out, int64_t* k) {
-    if (!k || !h_iq) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k, h_iq != nullptr));
     URH_CHECK(stream_check(ctx, n, ring, mod_type, dtype, true));
     urh_arena_reset(ctx);
     UrhClassify cls;
@@ -1096,20 +1102,20 @@ extern "C" int urh_demod_digitize_stream(urh_ctx* ctx, const void* h_iq, int dty
                                        URH_STREAM_ENTRY_DEMOD_DIGITIZE | (h_qad_out ? URH_STREAM_QAD_OUT : 0));
     StreamRing R;
     URH_CHECK(R.init(ctx, ring, z.ring_bytes));
-    StreamDigitizer dz;
-    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
+    StreamDigitizer sd;
+    URH_CHECK(sd.init(ctx, n, z.cs, tolerance, mod_type == URH_MOD_ASK, samples_per_symbol));
     char* d_src = R.mem;
     float* d_qad = h_qad_out ? (float*)(R.mem + ring * r256(z.src_slot)) : nullptr;
     std::vector<UrhWindow> win;
     URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 1, 0, chunk_samples, nullptr, nullptr, 0, win));
     URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, r256(z.src_slot), h_qad_out != nullptr,
                          [&](int64_t, const UrhWindow& w, int s) {
-                             URH_CHECK(stream_dense_iq<true>(ctx, dtype, mod_type, d_src, r256(z.src_slot), n, dp,
-                                                             d_qad ? d_qad + s * z.cs - w.k0 : nullptr, cls, tolerance, &dz, w.k0, w.k1, s));
-                             return dz.finish(ctx, w.k0, w.k1);
+                             URH_CHECK(stream_dense_iq(ctx, dtype, mod_type, d_src + s * r256(z.src_slot), n, dp, cls, w,
+                                                       DensePass{d_qad ? d_qad + s * z.cs - w.k0 : nullptr, &sd.dz}));
+                             return sd.finish(ctx, w.k0, w.k1);
                          },
                          contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad_out, 4), place_after_pad));
-    *k = dz.rows;
+    *k = sd.rows;
     return URH_OK;
 }
 
@@ -1156,9 +1162,7 @@ extern "C" int urh_afp_demod_psk_stream(urh_ctx* ctx, const void* h_iq, int dtyp
 extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_mag, float center,
                                              uint16_t tolerance, uint32_t samples_per_symbol, uint8_t bits_per_symbol, float center_spacing,
                                              int64_t chunk_samples, int ring, float* h_qad_out, int64_t* k) {
-    if (!k || !h_iq) return URH_ERR_INVALID;
-    *k = 0;
-    ctx->pulses_k = 0;
+    URH_CHECK(pulses_begin(ctx, k, h_iq != nullptr));
     URH_CHECK(psk_stream_check(ctx, n, ring, dtype));
     urh_arena_reset(ctx);
     UrhClassify cls;
@@ -1174,21 +1178,21 @@ extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int
     float* d_qad = (float*)(R.mem + ring * slot);
     UrhCostasStream cs;
     URH_CHECK(urh_costas_stream_begin(ctx, &cs));
-    StreamDigitizer dz;
-    URH_CHECK(dz.init(ctx, n, z.cs, tolerance, false, samples_per_symbol));
+    StreamDigitizer sd;
+    URH_CHECK(sd.init(ctx, n, z.cs, tolerance, false, samples_per_symbol));
     std::vector<UrhWindow> win;
     URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
     URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), d_src, slot, h_qad_out != nullptr,
                          [&](int64_t c, const UrhWindow& w, int s) {
-                             urh_arena_release(ctx, dz.mark);
+                             urh_arena_release(ctx, sd.mark);
                              float* q = d_qad + s * z.cs;
                              URH_CHECK(urh_costas_stream_chunk(ctx, &cs, c, d_src + s * slot + URH_STREAM_PAD, dtype, w.k1 - w.k0, dp.noise_sqrd,
                                                                mod_order, 0.1f, q));
-                             URH_CHECK(stream_dense_qad(ctx, q, w.k0, w.k1, cls, dz));
-                             return dz.finish(ctx, w.k0, w.k1);
+                             URH_CHECK(launch_dense_qad(ctx, sd.dz, q, w.k0, w.k1, cls));
+                             return sd.finish(ctx, w.k0, w.k1);
                          },
                          contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad_out, 4), place_after_pad));
-    *k = dz.rows;
+    *k = sd.rows;
     return urh_costas_stream_end(ctx, &cs);
 }
 

@@ -379,19 +379,10 @@ __global__ void k_chain_last_row(UrhChain* __restrict__ chain, const int64_t* __
 }
 
 // ---- driver --------------------------------------------------------------------------------------------------------------
-struct FinishShard {
-    int rank, world;            // world == 1: unsharded
-    int64_t global_offset;      // first sample of this shard in the capture
-    int64_t n_total;
-    int emit_tail;
-    // chained chunk of a capture streamed through this GPU: the carries come from *chain instead of the other ranks, and the rows
-    // are appended to the pulse table after its first row_base rows (the caller has made room for rows_cap more)
-    UrhChain* chain;
-    int64_t row_base, rows_cap;
-};
-
-static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                        int stage_cap, const int16_t* d_init, const FinishShard& sh, int64_t* k) {
+// A shard folds the three scan totals of the preceding ranks, exchanged on the stream; a chained chunk takes them from and folds
+// them into *chain (device memory).
+int finish_tiles(urh_ctx* ctx, const UrhDigitizer& dz, const FinishShard& sh, int64_t* k) {
+    const int64_t n = sh.n;
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     const bool sharded = sh.world > 1;
     UrhChain* chain = sh.chain;
@@ -421,27 +412,27 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     int64_t* d_all2 = d_all1 + 4 * (sharded ? sh.world : 0);
     int64_t* d_all3 = d_all2 + 2 * (sharded ? sh.world : 0);
 
-    if (chain && sh.global_offset == 0) URH_LAUNCH(ctx, k_chain_start, 1, 1, 0, d_init, chain);
+    if (chain && sh.global_offset == 0) URH_LAUNCH(ctx, k_chain_start, 1, 1, 0, dz.d_init, chain);
     RunCarry rc_ident;
     rc_ident.len = 0; rc_ident.cls = 0; rc_ident.flags = 2 | 1;
     ScanRunCarry fa;
-    fa.tiles = tiles; fa.n = n; fa.carry = carry;
+    fa.tiles = dz.tiles; fa.n = n; fa.carry = carry;
     URH_CHECK((urhts::scan<RunCarry, RunCarryOp, ScanRunCarry>(ctx, ntiles, rc_ident, RunCarryOp(), fa, d_tot_run)));
     if (sharded) {
-        URH_LAUNCH(ctx, k_pack_stage1, 1, 1, 0, d_init, (const RunCarry*)d_tot_run, d_msg1);
+        URH_LAUNCH(ctx, k_pack_stage1, 1, 1, 0, dz.d_init, (const RunCarry*)d_tot_run, d_msg1);
         URH_TL_MARK(ctx, "x4 run carry: enter");
         URH_CHECK(urh_nccl_allgather(ctx, d_msg1, d_all1, 4 * sizeof(int64_t)));
         URH_TL_MARK(ctx, "x4 run carry: done");
         URH_LAUNCH(ctx, k_fold_carry, 1, 1, 0, (const int64_t*)d_all1, sh.rank, d_xcarry);
     }
     ScanCandidates fb;
-    fb.tiles = tiles; fb.staging = staging; fb.stage_cap = stage_cap; fb.carry = carry;
+    fb.tiles = dz.tiles; fb.staging = dz.staging; fb.stage_cap = dz.cap; fb.carry = carry;
     fb.xcarry = sharded ? d_xcarry : (chain ? &chain->run : nullptr);
-    fb.tol = tol; fb.head_rel = head_rel; fb.prev_cls = prev_cls; fb.fire = fire;
+    fb.tol = dz.tol; fb.head_rel = head_rel; fb.prev_cls = prev_cls; fb.fire = fire;
     CandAgg ca_ident;
     ca_ident.cnt = 0; ca_ident.last_cls = CLS_NONE; ca_ident.pad = 0;
     URH_CHECK((urhts::scan<CandAgg, CandOp, ScanCandidates, 4>(ctx, ntiles, ca_ident, CandOp(), fb, d_tot_cand)));   // heavy load(): thin blocks
-    const int16_t* prev0 = chain ? &chain->prev_cls : d_init;
+    const int16_t* prev0 = chain ? &chain->prev_cls : dz.d_init;
     if (sharded) {
         URH_TL_MARK(ctx, "x5 candidates: enter");
         URH_CHECK(urh_nccl_allgather(ctx, d_tot_cand, d_all2, sizeof(CandAgg)));
@@ -474,19 +465,19 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     const int64_t row_base = chain ? sh.row_base : 0;
     int64_t* raw = ctx->pulses + 2 * row_base;
     int64_t raw_cap = chain ? sh.rows_cap : cap_rows;
-    if (is_ask) URH_CHECK(urh_arena(ctx, (size_t)raw_cap * 2, &raw));
+    if (dz.is_ask) URH_CHECK(urh_arena(ctx, (size_t)raw_cap * 2, &raw));
     int64_t got[2] = {0, 0};
     for (int attempt = 0; attempt < 2; attempt++) {
-        URH_LAUNCH(ctx, k_finish_rows, (unsigned)urh_div_up(ntiles, 8 * FIN_TILES), 256, 0, tiles, staging, stage_cap, (const int32_t*)head_rel,
+        URH_LAUNCH(ctx, k_finish_rows, (unsigned)urh_div_up(ntiles, 8 * FIN_TILES), 256, 0, dz.tiles, dz.staging, dz.cap, (const int32_t*)head_rel,
                    (const int32_t*)prev_cls, prev0, (const int64_t*)row_off, (const int64_t*)prev_fired, xprev, ntiles, sh.global_offset,
-                   sh.n_total, tol, is_ask ? 1 : 0, (int64_t)sps, sh.emit_tail, row_base, raw, raw_cap, d_small);
+                   sh.n_total, dz.tol, dz.is_ask ? 1 : 0, (int64_t)dz.sps, sh.emit_tail, row_base, raw, raw_cap, d_small);
         if (sharded && attempt == 0) URH_TL_MARK(ctx, "rows written");
         URH_CHECK(urh_read_i64(ctx, d_small, 2, got));
         if (got[0] <= raw_cap) break;
         // rows_cap bounds a chained chunk's rows (one per candidate plus the tail), so only the unchained table can overflow
         if (attempt == 1 || chain) URH_FAIL(ctx, URH_ERR_CUDA, "finish_tiles: row buffer overflow after regrowth");
         // more rows than guessed: grow and repeat stage D only
-        if (is_ask) {
+        if (dz.is_ask) {
             URH_CHECK(urh_arena(ctx, (size_t)got[0] * 2, &raw));
             raw_cap = got[0];
         } else {
@@ -497,7 +488,7 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     }
     if (chain) URH_LAUNCH(ctx, k_chain_advance, 1, 1, 0, chain, (const RunCarry*)d_tot_run, (const CandAgg*)d_tot_cand, (const FireAgg*)d_tot_fire);
     int64_t K = got[0];
-    if (is_ask && K > 0) {
+    if (dz.is_ask && K > 0) {
         if (!chain) URH_CHECK(urh_ensure_pulses(ctx, (size_t)K));
         int64_t* out = ctx->pulses + 2 * row_base;
         URH_CUDA(ctx, cudaMemsetAsync(out, 0, (size_t)K * 2 * sizeof(int64_t), ctx->stream));
@@ -513,37 +504,4 @@ static int finish_tiles(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t 
     ctx->pulses_k = row_base + K;
     *k = K;
     return URH_OK;
-}
-
-// One chunk of a capture streamed through this GPU (digitize.cu): the same stages as a shard, with the three carries taken from
-// and folded into *chain (device memory) instead of exchanged between ranks.  *k = rows this chunk added to the pulse table
-// (a first row that continues the table's last row is merged into it).
-int urh_finish_chunk(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, UrhChain* chain, int64_t global_offset, int64_t n_total, int64_t row_base,
-                     int64_t rows_cap, int64_t* k) {
-    FinishShard sh;
-    sh.rank = 0; sh.world = 1; sh.global_offset = global_offset; sh.n_total = n_total;
-    sh.emit_tail = (global_offset + n == n_total) ? 1 : 0;
-    sh.chain = chain; sh.row_base = row_base; sh.rows_cap = rows_cap;
-    return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
-}
-
-int urh_finish_local(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, int64_t* k) {
-    FinishShard sh;
-    sh.rank = 0; sh.world = 1; sh.global_offset = 0; sh.n_total = n; sh.emit_tail = 1;
-    sh.chain = nullptr; sh.row_base = 0; sh.rows_cap = 0;
-    return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
-}
-
-// One shard of a capture spread over the ranks of the context's NCCL communicator: same stages, the three scan totals
-// exchanged on the stream.  Every rank ends with the rows of its own shard (urh_fetch_pulses); equal states meeting at a
-// shard edge are joined by the consumer.
-int urh_finish_shard(urh_ctx* ctx, int64_t n, int tol, bool is_ask, uint32_t sps, const UrhTileSummary* tiles, const uint32_t* staging,
-                     int stage_cap, const int16_t* d_init, int64_t global_offset, int64_t n_total, int64_t* k) {
-    FinishShard sh;
-    sh.rank = ctx->nccl_rank; sh.world = ctx->nccl_world; sh.global_offset = global_offset; sh.n_total = n_total;
-    sh.emit_tail = (ctx->nccl_rank == ctx->nccl_world - 1) ? 1 : 0;
-    sh.chain = nullptr; sh.row_base = 0; sh.rows_cap = 0;
-    return finish_tiles(ctx, n, tol, is_ask, sps, tiles, staging, stage_cap, d_init, sh, k);
 }

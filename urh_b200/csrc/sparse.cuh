@@ -1,6 +1,7 @@
 // Run stitching across tiles (RunCarry), used by the digitizer's tile-level finish (finish.cu), and the gathered candidate table of
 // the message segmenter and the plateau RLE (stats.cu): tile summaries + per-tile staged candidates  ->  one ordered, compact table.
-// UrhChain: what a chunk's finish receives from the chunks before it (finish.cu).
+// UrhChain: what a chunk's finish receives from the chunks before it; UrhDigitizer and FinishShard: what a finish reads and where
+// its rows go (finish.cu).
 #pragma once
 #include "dense.cuh"
 
@@ -54,6 +55,57 @@ struct __align__(16) UrhChain {
     int16_t prev_cls;      // class of the last candidate of the preceding chunks (chunk 0: the digitizer's initial state)
     int16_t pad[7];
 };
+
+// staged candidates per tile of a digitizer at tolerance tol: firings are >= tol + 1 samples apart
+static inline int stage_cap_for(int tol) { return URH_TILE / (tol + 1) + 2; }
+
+// The digitizer of one pulse table: the dense pass fills the tile summaries, the staged candidates of each tile and the initial
+// state; finish_tiles turns them into (state, length) rows.
+struct UrhDigitizer {
+    int64_t n;                // samples the pulse table covers (a shard: its own)
+    int tol, cap;             // tolerance; staged candidates per tile
+    bool is_ask;
+    uint32_t sps;             // samples per symbol
+    UrhTileSummary* tiles;
+    uint32_t* staging;
+    int16_t* d_init;          // the initial state, stored by the pass over the capture's first tile
+    // The tables for ntiles tiles from the arena.  zero_init: d_init is zeroed now, on the stream.
+    int init(urh_ctx* ctx, int64_t n_, int tol_, bool ask, uint32_t sps_, int64_t ntiles, bool zero_init) {
+        n = n_; tol = tol_; cap = stage_cap_for(tol); is_ask = ask; sps = sps_;
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
+        URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
+        URH_CHECK(urh_arena(ctx, 8, &d_init));
+        if (zero_init) URH_CUDA(ctx, cudaMemsetAsync(d_init, 0, 16, ctx->stream));
+        return URH_OK;
+    }
+};
+
+// Which rows a finish writes and what precedes them: the whole capture, one shard of the context's NCCL communicator, or a chunk
+// of a capture streamed through this GPU.
+struct FinishShard {
+    int64_t n;                  // samples of this shard (chunk)
+    int rank, world;            // world == 1: unsharded
+    int64_t global_offset;      // first sample of this shard in the capture
+    int64_t n_total;
+    int emit_tail;
+    // chained chunk: the carries come from *chain instead of the other ranks, and the rows are appended to the pulse table after
+    // its first row_base rows (the caller has made room for rows_cap more)
+    UrhChain* chain;
+    int64_t row_base, rows_cap;
+
+    static FinishShard local(const UrhDigitizer& dz) { return FinishShard{dz.n, 0, 1, 0, dz.n, 1, nullptr, 0, 0}; }
+    // every rank ends with the rows of its own shard; equal states meeting at a shard edge are joined by the consumer
+    static FinishShard shard(const urh_ctx* ctx, const UrhDigitizer& dz, int64_t global_offset, int64_t n_total) {
+        return FinishShard{dz.n, ctx->nccl_rank, ctx->nccl_world, global_offset, n_total, ctx->nccl_rank == ctx->nccl_world - 1 ? 1 : 0,
+                           nullptr, 0, 0};
+    }
+    // the chunk [s0, s1) of a capture of n_total samples; a first row that continues the table's last row is merged into it
+    static FinishShard chunk(UrhChain* chain, int64_t s0, int64_t s1, int64_t n_total, int64_t row_base, int64_t rows_cap) {
+        return FinishShard{s1 - s0, 0, 1, s0, n_total, s1 == n_total ? 1 : 0, chain, row_base, rows_cap};
+    }
+};
+// The pulse table of the tiles dz's dense pass filled (finish.cu).  *k = the rows this finish added.
+int finish_tiles(urh_ctx* ctx, const UrhDigitizer& dz, const FinishShard& sh, int64_t* k);
 
 struct UrhCandidates {
     int64_t count;   // number of candidates (host copy)
