@@ -1,7 +1,7 @@
 """CPU model of detect_center's binning in center.cu, pinned to numpy.
 
-Restated here: the bin edges as np.arange forms them and as k_hist_edges / k_center_plan form them (one rounded product, one
-rounded sum; np.arange's length ceil((stop - start) / step)), the float thresholds ru(edge_k), rd(last edge) and
+Restated here: the bin edges as np.arange forms them and as cen_edge forms them for k_center_plan and for caller-given edges
+(one rounded product, one rounded sum; np.arange's length ceil((stop - start) / step)), the float thresholds ru(edge_k), rd(last edge) and
 f_min = max(ru(hmin), succ(-4)), and HistBins::bin_of in both variants.  The FAST guess's FFMA is evaluated exactly
 (fractions.Fraction) and rounded once to float32, so the model says what the device computes, not what float64 numpy would.
 Pinned to np.histogram / np.searchsorted over many (hmin, hstep, nbins), with |edge| / hstep from 1 to past 2^24: the FAST guess
@@ -50,12 +50,21 @@ def fmaf(a, b, c):
 
 
 def arange_edges(hmin, hstep, nbins):
-    """k_hist_edges: hmin + k * hstep, one rounded product and one rounded sum (np.arange's element formula)"""
+    """caller-given edges hmin + k * hstep, one rounded product and one rounded sum (np.arange's element formula)"""
     return hmin + np.arange(nbins + 1, dtype=np.float64) * hstep
 
 
+def cen_edges(hmin, edge1, delta, nedges):
+    """cen_edge: start, start + step, then start + k * delta"""
+    e = hmin + np.arange(nedges, dtype=np.float64) * delta
+    e[0] = hmin
+    if nedges > 1:
+        e[1] = edge1
+    return e
+
+
 class Bins:
-    """the thresholds k_hist_edges writes and HistBins::load / bin_of reads"""
+    """the thresholds cen_edge_table writes and HistBins::load / bin_of reads"""
 
     def __init__(self, hmin, hstep, nbins):
         self.edges = arange_edges(hmin, hstep, nbins)
@@ -215,11 +224,7 @@ def plan_edges(mn, mx, var):
     if length < 2:
         return None
     edge1 = mn + hstep
-    delta = edge1 - mn
-    k = np.arange(length, dtype=np.float64)
-    e = mn + k * delta
-    e[0], e[1] = mn, edge1
-    return e
+    return cen_edges(mn, edge1, edge1 - mn, length)
 
 
 def test_plan_edges_are_np_arange():
@@ -246,3 +251,4 @@ def test_plan_edges_are_np_arange():
         assert got is not None and np.array_equal(got.view(np.uint64), want.view(np.uint64)), (mn, mx, var)
         hit_exact += float(np.ceil((mx + np.float32(var) - mn) / np.float32(var))) == (mx + np.float32(var) - mn) / np.float32(var)
     assert hit_exact >= 10
+

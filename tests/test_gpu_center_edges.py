@@ -5,12 +5,14 @@
 * urh_center_histogram / urh_center_histogram_tiles with caller-chosen (hmin, hstep, nbins) forcing each variant of
   k_hist_interior (one-look-up FAST with |edge| / hstep just below 2^20, the shared-memory loop with the edge table, shared-memory
   counts with the table in global memory, global counts): counts equal np.histogram on the same edges, with every float32 of some
-  bins and samples on ru(edge), pred(ru(edge)), f_hi and succ(f_hi);
+  bins and samples on ru(edge), pred(ru(edge)), f_hi and succ(f_hi); over the same rank windows, among them windows that start or
+  end on a tile boundary next to a silent tile and one inside a tile, urh_center_window_stats (k_center_window) equals numpy;
 * the fused steps on ASK / FSK captures: demod_detect_center (bitwise off and on), demod_center_digitize one-call and stepwise,
   the certified pick on and off, levels on both sides of the fine histogram's 1.0 clamp, and a strong nearly constant ASK carrier
   whose variance cancels in the double tile sums;
 * the device chain's restatement of np.arange (length, edges, the 6000-bin handback) through the state and center it returns."""
 import ctypes as C
+import math
 import os
 import zlib
 
@@ -156,14 +158,35 @@ def test_histogram_entries_equal_numpy(AI, name):
         ctx.check(ctx.lib.urh_center_stats(ctx.handle, C.c_void_p(d.ptr), len(x), -1, st.ctypes.data_as(C.c_void_p)))
         kept = x[x > -4]
         assert int(st[0]) == len(kept)
-        for r0, r1 in ((0, len(kept)), (int(st[1]), int(st[2])), (TILE + 5, TILE + 6), (3 * TILE - 7, min(7 * TILE + 3, len(kept)))):
-            want, _ = np.histogram(kept[r0:r1], bins=edges)
+        windows = [(0, len(kept)), (int(st[1]), int(st[2])), (TILE + 5, TILE + 6), (3 * TILE - 7, min(7 * TILE + 3, len(kept)))]
+        # P[t] = kept samples before tile t; tile 2 is silent, so P[2] == P[3] (ranges below -4 keep almost nothing)
+        P = np.cumsum(np.concatenate([[0], (x[:8 * TILE] > -4).reshape(8, TILE).sum(axis=1)]))
+        assert P[2] == P[3]
+        if P[5] - P[4] > 6:
+            windows += [(P[3], P[5]),         # r0: the first rank after the silent tile, r1 - 1: the last rank of tile 4
+                        (P[1] + 5, P[2]),     # r1 - 1: the last rank before the silent tile
+                        (P[1], P[2]),         # exactly tile 1
+                        (P[4] + 3, P[5] - 3)]   # inside one tile
+        else:
+            assert edges[-1] <= -4.0, name   # only a range below detect_center's -4 keeps (almost) nothing
+        for r0, r1 in ((int(a), int(b)) for a, b in windows):
+            rect = kept[r0:r1]
+            want, _ = np.histogram(rect, bins=edges)
             for entry in (ctx.lib.urh_center_histogram_tiles, ctx.lib.urh_center_histogram):
                 y = np.zeros(nbins, dtype=np.int64)
                 ctx.check(entry(ctx.handle, C.c_void_p(d.ptr), len(x), r0, r1, C.c_double(hmin), C.c_double(hstep), nbins,
                                 y.ctypes.data_as(C.c_void_p)))
                 bad = np.nonzero(y != want)[0]
                 assert len(bad) == 0, (name, arr_name, r0, r1, bad[:5], y[bad[:5]], want[bad[:5]])
+            w = np.zeros(5)
+            ctx.check(ctx.lib.urh_center_window_stats(ctx.handle, C.c_void_p(d.ptr), len(x), r0, r1, w.ctypes.data_as(C.c_void_p)))
+            want_w = (len(rect), float(rect.min()), float(rect.max())) if len(rect) else (0, np.inf, -np.inf)
+            assert (w[0], w[1], w[2]) == want_w, (name, arr_name, r0, r1, w)
+            # double sums of float32 values (their squares are exact) in any order: within gamma_(n-1) * sum |term| of the exact sum
+            r64 = rect.astype(np.float64)
+            gamma = (len(rect) - 1) * 2.0 ** -53 / (1 - (len(rect) - 1) * 2.0 ** -53)
+            for got, terms in ((w[3], r64), (w[4], r64 * r64)):
+                assert abs(got - math.fsum(terms)) <= gamma * np.abs(terms).sum(), (name, arr_name, r0, r1, got, math.fsum(terms))
         del keep
 
 

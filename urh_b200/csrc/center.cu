@@ -9,8 +9,10 @@
 //      demodulated k_tile_stats_f32 reads it once.
 //   2. rank prefix over the tile counts -> the two tiles the rank window cuts; window statistics = table entries of the
 //      interior tiles + a rank-exact re-read of the (at most two) cut tiles.  No pass over the samples.
-//   3. histogram: ONE pass over qad.  Bin edges become float thresholds (exact, see k_hist_edges), every thread counts
+//   3. histogram: ONE pass over qad.  Bin edges become float thresholds (exact, see cen_edge_table), every thread counts
 //      its currently popular bins in registers and only misses touch the shared-memory histogram.
+// The window and histogram kernels read their parameters from a CenterPlan: the device-resident chain (second half) fills it on
+// the device, the stepwise entries from their arguments (k_center_set).
 #include "dense.cuh"
 #include "tilescan.cuh"
 
@@ -79,19 +81,6 @@ static int kept_prefix(urh_ctx* ctx, const UrhTileStats* ts, int64_t ntiles, int
     return urhts::scan<int64_t, CenAddI64, ScanKept>(ctx, ntiles, (int64_t)0, CenAddI64(), fk, prefix + ntiles);
 }
 
-// Tile t holds ranks [prefix[t], prefix[t+1]).  win[0] = tile of rank r0, win[1] = tile of rank r1-1 (r0 < r1 <= total);
-// win[2], win[3] = those tiles again if the window cuts them (covers them only partly), else -1.  Pre-set to -1.
-__global__ void k_find_window_tiles(const int64_t* __restrict__ prefix, int64_t ntiles, int64_t r0, int64_t r1, int64_t* __restrict__ win) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= ntiles) return;
-    const int64_t a = prefix[t], b = prefix[t + 1];
-    if (b <= a) return;
-    const bool covered = a >= r0 && b <= r1;
-    const bool has_r0 = a <= r0 && r0 < b, has_r1 = a <= r1 - 1 && r1 - 1 < b;
-    if (has_r0) { win[0] = t; win[2] = covered ? -1 : t; }
-    if (has_r1) { win[1] = t; win[3] = (covered || has_r0) ? -1 : t; }
-}
-
 // block-wide exclusive rank of each thread's first kept sample inside one tile (8 consecutive samples per thread)
 #define CEN_PER (URH_TILE / 256)
 __device__ __forceinline__ int64_t cen_tile_ranks(const float* __restrict__ x, int64_t n, int64_t t, int64_t tile_rank0, float (&v)[CEN_PER],
@@ -139,61 +128,6 @@ __device__ __forceinline__ void cen_block_fold(double sum, double sq, float mn, 
     }
 }
 
-// rank-exact partial statistics of the cut tiles win[2], win[3]; one block each
-__global__ void __launch_bounds__(256) k_cut_tile_stats(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
-                                                       const int64_t* __restrict__ win, int64_t r0, int64_t r1, CenStats* __restrict__ out) {
-    __shared__ int s_pre[256];
-    const int64_t t = win[2 + blockIdx.x];
-    double sum = 0.0, sq = 0.0;
-    float mn = INFINITY, mx = -INFINITY;
-    long long cnt = 0;
-    if (t >= 0) {
-        float v[CEN_PER];
-        int64_t rank = cen_tile_ranks(x, n, t, prefix[t], v, s_pre);
-#pragma unroll
-        for (int j = 0; j < CEN_PER; j++) {
-            if (v[j] > -4.0f) {
-                if (rank >= r0 && rank < r1) {
-                    sum += (double)v[j];
-                    sq += (double)v[j] * (double)v[j];
-                    mn = fminf(mn, v[j]);
-                    mx = fmaxf(mx, v[j]);
-                    cnt++;
-                }
-                rank++;
-            }
-        }
-    }
-    cen_block_fold(sum, sq, mn, mx, cnt, out + blockIdx.x);
-}
-
-// tiles entirely inside the rank window: fold the table; grid-stride, one partial per block
-__global__ void __launch_bounds__(256) k_interior_tile_stats(const UrhTileStats* __restrict__ ts, const int64_t* __restrict__ prefix,
-                                                            int64_t ntiles, int64_t r0, int64_t r1, CenStats* __restrict__ partial) {
-    double sum = 0.0, sq = 0.0;
-    float mn = INFINITY, mx = -INFINITY;
-    long long cnt = 0;
-    for (int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x; t < ntiles; t += (int64_t)gridDim.x * 256) {
-        const int64_t a = prefix[t], b = prefix[t + 1];
-        if (b > a && a >= r0 && b <= r1) {
-            const UrhTileStats v = ts[t];
-            sum += v.sum; sq += v.sumsq; mn = fminf(mn, v.mn); mx = fmaxf(mx, v.mx); cnt += v.cnt;
-        }
-    }
-    cen_block_fold(sum, sq, mn, mx, cnt, partial + blockIdx.x);
-}
-
-__global__ void __launch_bounds__(256) k_center_fold(const CenStats* __restrict__ partial, int64_t count, CenStats* __restrict__ out) {
-    double sum = 0.0, sq = 0.0;
-    float mn = INFINITY, mx = -INFINITY;
-    long long cnt = 0;
-    for (int64_t t = threadIdx.x; t < count; t += 256) {
-        const CenStats p = partial[t];
-        sum += p.sum; sq += p.sumsq; mn = fminf(mn, p.mn); mx = fmaxf(mx, p.mx); cnt += p.cnt;
-    }
-    cen_block_fold(sum, sq, mn, mx, cnt, out);
-}
-
 // Rank prefix over a tile table; leaves {x, ts, prefix, n} in ctx for the window / histogram calls.
 int urh_center_tiles_begin(urh_ctx* ctx, const float* d_x, const UrhTileStats* ts, int64_t n, int64_t* h_total) {
     const int64_t ntiles = urh_div_up(n, URH_TILE);
@@ -220,35 +154,6 @@ static int tiles_from_array(urh_ctx* ctx, const float* d_x, int64_t n, int64_t* 
 
 static bool tiles_match(const urh_ctx* ctx, const float* d_x, int64_t n) {
     return ctx->center_prefix && ctx->center_n == n && ctx->center_x == (const void*)d_x;
-}
-
-// {count, min, max, sum, sumsq} of the kept samples whose LOCAL rank is in [r0, r1): interior tiles from the table, the
-// cut tiles re-read from d_qad.  A shard passes the global window minus its rank offset (clamped to its own count).
-extern "C" int urh_center_window_stats(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out5) {
-    h_out5[0] = 0.0; h_out5[1] = INFINITY; h_out5[2] = -INFINITY; h_out5[3] = 0.0; h_out5[4] = 0.0;
-    if (!tiles_match(ctx, d_qad, n)) URH_FAIL(ctx, URH_ERR_INVALID, "urh_afp_demod_tiles (same qad, same n) must precede urh_center_window_stats");
-    if (r1 <= r0) return URH_OK;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int64_t* prefix = (const int64_t*)ctx->center_prefix;
-    const UrhTileStats* ts = (const UrhTileStats*)ctx->center_ts;
-    int64_t* d_win;
-    CenStats* partial;
-    CenStats* folded;
-    const int nb = ctx->sm_count * 2;
-    URH_CHECK(urh_arena(ctx, 4, &d_win));
-    URH_CHECK(urh_arena(ctx, (size_t)nb + 4, &partial));
-    URH_CHECK(urh_arena(ctx, 2, &folded));
-    URH_CUDA(ctx, cudaMemsetAsync(d_win, 0xff, 4 * sizeof(int64_t), ctx->stream));
-    URH_LAUNCH(ctx, k_find_window_tiles, (unsigned)urh_div_up(ntiles, 256), 256, 0, prefix, ntiles, r0, r1, d_win);
-    URH_LAUNCH(ctx, k_interior_tile_stats, nb, 256, 0, ts, prefix, ntiles, r0, r1, partial);
-    URH_LAUNCH(ctx, k_cut_tile_stats, 2, 256, 0, d_qad, n, prefix, d_win, r0, r1, partial + nb);
-    URH_LAUNCH(ctx, k_center_fold, 1, 256, 0, partial, (int64_t)nb + 2, folded);
-    CenStats st;
-    URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail, folded, sizeof(CenStats), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    memcpy(&st, ctx->h_mail, sizeof(st));
-    h_out5[0] = (double)st.cnt; h_out5[1] = (double)st.mn; h_out5[2] = (double)st.mx; h_out5[3] = st.sum; h_out5[4] = st.sumsq;
-    return URH_OK;
 }
 
 // np.mean / np.var of the window [r0, r1) exactly as numpy computes them for a float32 array (pairwise.cu); needs the tile
@@ -291,15 +196,32 @@ extern "C" int urh_center_stats(urh_ctx* ctx, const float* d_x, int64_t n, int64
 // ---- 3. histogram -------------------------------------------------------------------------------------------------------
 // Bin edges of np.histogram as FLOAT thresholds: a float sample f satisfies f >= edge_k (double) iff f >= ru(edge_k), the
 // smallest float not below the edge, so the binning needs no double arithmetic and stays exact.
-// fe[0..nbins] = ru(hmin + k*hstep); fe[nbins+1] = rd(last edge) (np.histogram closes the last bin);
+// fe[0..nbins] = ru(edge k); fe[nbins+1] = rd(last edge) (np.histogram closes the last bin);
 // fe[nbins+2] = the smallest float that both exceeds -4 (detect_center's filter) and reaches the first edge.
-__global__ void k_hist_edges(double hmin, double hstep, int64_t nbins, float* __restrict__ fe) {
-    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    // edges exactly as np.arange forms them: one rounded product, one rounded sum (no FMA)
-    if (k <= nbins) fe[k] = __double2float_ru(__dadd_rn(hmin, __dmul_rn((double)k, hstep)));
-    if (k == nbins) {
-        fe[nbins + 1] = __double2float_rd(__dadd_rn(hmin, __dmul_rn((double)nbins, hstep)));
-        fe[nbins + 2] = fmaxf(__double2float_ru(hmin), nextafterf(-4.0f, 0.0f));
+
+// Edge k exactly as np.arange forms it: start, start + step, then start + k * delta, one rounded product and one rounded sum (no
+// FMA).  Caller-given edges hmin + k * hstep are the case edge1 = hmin + hstep, delta = hstep.  The operands are references, so a
+// caller that keeps them in memory reads only the one it uses.
+template <typename K>
+__device__ __forceinline__ double cen_edge(K k, const double& hmin, const double& edge1, const double& delta) {
+    return (k == 0) ? hmin : (k == 1 ? edge1 : __dadd_rn(hmin, __dmul_rn((double)k, delta)));
+}
+
+// The thresholds of edges k0, k0 + stride, ... <= nbins, and the counters hist[k] (and xhist[k]) of those k below nbins zeroed.
+__device__ __forceinline__ void cen_edge_table(long long k0, long long stride, long long nbins, const double& hmin, const double& edge1,
+                                               const double& delta, float* __restrict__ fe, unsigned long long* __restrict__ hist,
+                                               unsigned long long* __restrict__ xhist) {
+    for (long long k = k0; k <= nbins; k += stride) {
+        const double e = cen_edge(k, hmin, edge1, delta);
+        fe[k] = __double2float_ru(e);
+        if (k == nbins) {
+            fe[nbins + 1] = __double2float_rd(e);
+            fe[nbins + 2] = fmaxf(__double2float_ru(hmin), nextafterf(-4.0f, 0.0f));
+        }
+        if (k < nbins) {
+            hist[k] = 0ull;
+            if (xhist) xhist[k] = 0ull;
+        }
     }
 }
 
@@ -470,15 +392,6 @@ __device__ __forceinline__ void hist_interior_body(const float* __restrict__ x, 
     }
 }
 
-template <bool SMEM, bool FAST>
-__global__ void __launch_bounds__(256, 4) k_hist_interior(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ win,
-                                                      const float* __restrict__ g_fe, float scale, int nbins,
-                                                      unsigned long long* __restrict__ hist, int edges_in_smem,
-                                                      const int64_t* __restrict__ prefix) {
-    const int64_t w0 = win[0];   // < 0: empty window
-    hist_interior_body<SMEM, FAST>(x, n, w0 + 1, w0 >= 0 ? win[1] : 0, blockIdx.x, gridDim.x, g_fe, scale, nbins, hist, edges_in_smem, prefix);
-}
-
 // the window's first and last tile (win[0], win[1]; one block each): rank-exact, straight to the global histogram
 __device__ __forceinline__ void hist_window_ends_body(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
                                                       const int64_t* __restrict__ win, int64_t r0, int64_t r1,
@@ -501,54 +414,6 @@ __device__ __forceinline__ void hist_window_ends_body(const float* __restrict__ 
         }
         rank += kept ? 1 : 0;
     }
-}
-
-__global__ void __launch_bounds__(256) k_hist_window_ends(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
-                                                         const int64_t* __restrict__ win, int64_t r0, int64_t r1,
-                                                         const float* __restrict__ g_fe, float scale, int nbins,
-                                                         unsigned long long* __restrict__ hist) {
-    hist_window_ends_body(x, n, prefix, win, r0, r1, g_fe, scale, nbins, hist);
-}
-
-// Counts for edges hmin + k*hstep, k = 0..nbins (np.arange) over the samples of LOCAL rank [r0, r1); needs the tile
-// table of the same array (urh_afp_demod_tiles / urh_center_stats) in the arena.
-extern "C" int urh_center_histogram_tiles(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double hmin,
-                                          double hstep, int64_t nbins, int64_t* h_hist) {
-    if (nbins <= 0) return URH_OK;
-    if (!tiles_match(ctx, d_qad, n)) URH_FAIL(ctx, URH_ERR_INVALID, "urh_afp_demod_tiles (same qad, same n) must precede urh_center_histogram_tiles");
-    if (nbins > (int64_t)1 << 30) URH_FAIL(ctx, URH_ERR_INVALID, "too many histogram bins");
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int64_t* prefix = (const int64_t*)ctx->center_prefix;
-    unsigned long long* hist;
-    float* fe;
-    int64_t* d_win;
-    URH_CHECK(urh_arena(ctx, (size_t)nbins, &hist));
-    URH_CHECK(urh_arena(ctx, (size_t)nbins + 3, &fe));
-    URH_CHECK(urh_arena(ctx, 4, &d_win));
-    URH_CUDA(ctx, cudaMemsetAsync(hist, 0, (size_t)nbins * sizeof(unsigned long long), ctx->stream));
-    URH_CUDA(ctx, cudaMemsetAsync(d_win, 0xff, 4 * sizeof(int64_t), ctx->stream));
-    if (r1 > r0) {
-        URH_LAUNCH(ctx, k_hist_edges, (unsigned)urh_div_up(nbins + 1, 256), 256, 0, hmin, hstep, nbins, fe);
-        URH_LAUNCH(ctx, k_find_window_tiles, (unsigned)urh_div_up(ntiles, 256), 256, 0, prefix, ntiles, r0, r1, d_win);
-        // shared memory (48 KB without opt-in): histogram first, then the edge table if it still fits
-        const bool in_smem = nbins <= 12000;
-        const int edges_smem = (in_smem && nbins <= 6000) ? 1 : 0;
-        const size_t dyn = (in_smem ? (size_t)nbins * 4 : 0) + (edges_smem ? (size_t)(nbins + 3) * 4 : 0);
-        const float scale = (float)(1.0 / hstep);
-        // one-look-up binning needs the float guess to be good to half a bin
-        const double edge_abs = fmax(fabs(hmin), fabs(hmin + (double)nbins * hstep));
-        const bool fast = edges_smem && hstep > 0.0 && edge_abs / hstep < 1048576.0;
-        const unsigned gs = (unsigned)min(urh_div_up(ntiles, 8), (int64_t)ctx->sm_count * 8);
-        const int64_t* cw = d_win;
-        const float* cfe = fe;
-        if (in_smem && fast) URH_LAUNCH(ctx, (k_hist_interior<true, true>), gs, 256, dyn, d_qad, n, cw, cfe, scale, (int)nbins, hist, edges_smem, prefix);
-        else if (in_smem) URH_LAUNCH(ctx, (k_hist_interior<true, false>), gs, 256, dyn, d_qad, n, cw, cfe, scale, (int)nbins, hist, edges_smem, prefix);
-        else URH_LAUNCH(ctx, (k_hist_interior<false, false>), gs, 256, dyn, d_qad, n, cw, cfe, scale, (int)nbins, hist, edges_smem, prefix);
-        URH_LAUNCH(ctx, k_hist_window_ends, 2, 256, 0, d_qad, n, prefix, (const int64_t*)d_win, r0, r1, (const float*)fe, scale, (int)nbins, hist);
-    }
-    URH_CUDA(ctx, cudaMemcpyAsync(h_hist, hist, (size_t)nbins * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return URH_OK;
 }
 
 // Stage 2 of the stand-alone detect_center.  Reuses the tile table urh_center_stats left for this array; builds it if
@@ -574,6 +439,8 @@ extern "C" int urh_center_histogram(urh_ctx* ctx, const float* d_x, int64_t n, i
 //     mean of their left edges.  np.argsort's order among EQUAL counts is implementation-defined, so a tie that would decide
 //     which peak is taken hands the decision back to the host path (state 2), as do more than CEN_MAX_BINS bins.
 // Sharded captures: the kept counts, the window partials and the histogram are exchanged with NCCL on the context stream.
+// The stepwise entries (urh_center_window_stats, urh_center_histogram_tiles) run the same window and histogram kernels on a plan
+// that k_center_set fills from their arguments.
 // =============================================================================================================================
 #define CEN_MAX_BINS 6000
 #define CEN_VAR_MIN_RATIO 0x1p-14   // the double tile-sum variance stands in for numpy's only down to var = mean^2 * 2^-14
@@ -582,7 +449,7 @@ struct __align__(16) CenterPlan {
     long long total, offset;   // kept samples of the capture / of the preceding shards
     long long r0, r1;          // global rank window
     long long lr0, lr1;        // this shard's part of it (local ranks)
-    long long win[4];          // window tiles (k_find_window_tiles layout)
+    long long win[4];          // window tiles (cen_window_tiles)
     CenStats local;            // this shard's window partial
     double hmin, edge1, delta;
     long long nbins;
@@ -628,6 +495,22 @@ __device__ __forceinline__ int64_t cen_tile_of_rank(const int64_t* __restrict__ 
     return lo;
 }
 
+// Tiles of the local rank window [r0, r1): w[0] holds rank r0, w[1] rank r1 - 1 (tiles without a kept sample hold no rank);
+// w[2], w[3] = those tiles again where the window cuts them (covers them only partly), else -1.  All -1 for an empty window.
+__device__ __forceinline__ void cen_window_tiles(const int64_t* __restrict__ prefix, int64_t ntiles, long long r0, long long r1,
+                                                 long long (&w)[4]) {
+    long long w0 = -1, w1 = -1, w2 = -1, w3 = -1;
+    if (r1 > r0) {
+        w0 = cen_tile_of_rank(prefix, ntiles, r0);
+        w1 = cen_tile_of_rank(prefix, ntiles, r1 - 1);
+        const bool cov0 = prefix[w0] >= r0 && prefix[w0 + 1] <= r1;
+        const bool cov1 = prefix[w1] >= r0 && prefix[w1 + 1] <= r1;
+        w2 = cov0 ? -1 : w0;
+        w3 = (cov1 || w1 == w0) ? -1 : w1;
+    }
+    w[0] = w0; w[1] = w1; w[2] = w2; w[3] = w3;
+}
+
 // window tiles + {count, min, max, sum, sumsq} of this shard's window: interior tiles from the table (grid-stride), the two
 // cut tiles rank-exactly (blocks 0 and 1), folded by the last block to finish.  partial: gridDim.x + 2 entries.
 __global__ void __launch_bounds__(256) k_center_window(const float* __restrict__ x, int64_t n, const UrhTileStats* __restrict__ ts,
@@ -638,17 +521,10 @@ __global__ void __launch_bounds__(256) k_center_window(const float* __restrict__
     __shared__ bool s_last;
     const long long r0 = plan->lr0, r1 = plan->lr1;
     if (threadIdx.x == 0) {
-        long long w0 = -1, w1 = -1, w2 = -1, w3 = -1;
-        if (r1 > r0) {
-            w0 = cen_tile_of_rank(prefix, ntiles, r0);
-            w1 = cen_tile_of_rank(prefix, ntiles, r1 - 1);
-            const bool cov0 = prefix[w0] >= r0 && prefix[w0 + 1] <= r1;
-            const bool cov1 = prefix[w1] >= r0 && prefix[w1 + 1] <= r1;
-            w2 = cov0 ? -1 : w0;
-            w3 = (cov1 || w1 == w0) ? -1 : w1;
-        }
-        s_win[0] = w0; s_win[1] = w1; s_win[2] = w2; s_win[3] = w3;
-        if (blockIdx.x == 0) { plan->win[0] = w0; plan->win[1] = w1; plan->win[2] = w2; plan->win[3] = w3; }
+        long long w[4];
+        cen_window_tiles(prefix, ntiles, r0, r1, w);
+        s_win[0] = w[0]; s_win[1] = w[1]; s_win[2] = w[2]; s_win[3] = w[3];
+        if (blockIdx.x == 0) { plan->win[0] = w[0]; plan->win[1] = w[1]; plan->win[2] = w[2]; plan->win[3] = w[3]; }
     }
     __syncthreads();
     double sum = 0.0, sq = 0.0;
@@ -766,28 +642,19 @@ __global__ void __launch_bounds__(256) k_center_plan(const CenStats* __restrict_
     }
     __syncthreads();
     if (s_state != 1) return;
-    const long long nbins = s_nbins;
-    for (long long k = threadIdx.x; k <= nbins; k += 256) {
-        const double e = (k == 0) ? s_hmin : (k == 1 ? s_edge1 : __dadd_rn(s_hmin, __dmul_rn((double)k, s_delta)));
-        fe[k] = __double2float_ru(e);
-        if (k == nbins) {
-            fe[nbins + 1] = __double2float_rd(e);
-            fe[nbins + 2] = fmaxf(__double2float_ru(s_hmin), nextafterf(-4.0f, 0.0f));
-        }
-        if (k < nbins) {
-            hist[k] = 0ull;
-            if (xhist) xhist[k] = 0ull;
-        }
-    }
+    cen_edge_table(threadIdx.x, 256, s_nbins, s_hmin, s_edge1, s_delta, fe, hist, xhist);
 }
 
-template <bool FAST>
-__global__ void __launch_bounds__(256, 3) k_hist_interior_dev(const float* __restrict__ x, int64_t n, const CenterPlan* __restrict__ plan,
-                                                          const float* __restrict__ g_fe, unsigned long long* __restrict__ hist,
-                                                          const int64_t* __restrict__ prefix) {
+// The histogram of the window's interior tiles (plan->win[0] + 1 .. plan->win[1]).  A caller that enqueues both FAST variants gets
+// only the one matching plan->fast run.  SMEM: counts in shared memory; edges_in_smem: the edge table too (FAST needs it).
+// MIN_BLOCKS per SM: 3 with the table in shared memory (every register kept, no spills), 4 with it in global memory (measured faster).
+template <bool SMEM, bool FAST, int MIN_BLOCKS>
+__global__ void __launch_bounds__(256, MIN_BLOCKS) k_hist_interior(const float* __restrict__ x, int64_t n, const CenterPlan* __restrict__ plan,
+                                                                  const float* __restrict__ g_fe, unsigned long long* __restrict__ hist,
+                                                                  const int64_t* __restrict__ prefix, int edges_in_smem) {
     if (plan->state != 1 || plan->certified || (plan->fast != 0) != FAST) return;
-    hist_interior_body<true, FAST>(x, n, plan->win[0] + 1, plan->win[1], blockIdx.x, gridDim.x, g_fe, plan->scale, (int)plan->nbins, hist, 1,
-                                   prefix);
+    hist_interior_body<SMEM, FAST>(x, n, plan->win[0] + 1, plan->win[1], blockIdx.x, gridDim.x, g_fe, plan->scale, (int)plan->nbins, hist,
+                                   edges_in_smem, prefix);
 }
 
 // Slabs [*sf, *se) lie wholly among the window's interior tiles (win0, win1): their fine-histogram rows count in full.
@@ -798,10 +665,10 @@ __device__ __forceinline__ void cen_full_slabs(int64_t win0, int64_t win1, int64
 
 // Blocks 0 and 1: the window's first and last tile, rank-exactly, into hist (and xhist).  With a fine histogram (xhist != NULL)
 // blocks 2.. bin the interior tiles of the slabs the window covers only partly into xhist: the exact part of the certificate.
-__global__ void __launch_bounds__(256) k_hist_window_ends_dev(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
-                                                             const CenterPlan* __restrict__ plan, const float* __restrict__ g_fe,
-                                                             unsigned long long* __restrict__ hist, unsigned long long* __restrict__ xhist,
-                                                             int64_t slab_tiles) {
+__global__ void __launch_bounds__(256) k_hist_window_ends(const float* __restrict__ x, int64_t n, const int64_t* __restrict__ prefix,
+                                                         const CenterPlan* __restrict__ plan, const float* __restrict__ g_fe,
+                                                         unsigned long long* __restrict__ hist, unsigned long long* __restrict__ xhist,
+                                                         int64_t slab_tiles) {
     if (plan->state != 1) return;
     if (blockIdx.x < 2) {
         hist_window_ends_body(x, n, prefix, (const int64_t*)plan->win, plan->lr0, plan->lr1, g_fe, plan->scale, (int)plan->nbins, hist, xhist);
@@ -823,9 +690,9 @@ __global__ void __launch_bounds__(256) k_hist_window_ends_dev(const float* __res
     }
 }
 
-// left edge of bin k exactly as np.arange forms it (k_center_pick, k_center_certify)
+// left edge of bin k (k_center_pick, k_center_certify)
 __device__ __forceinline__ double cen_left_edge(const CenterPlan* plan, int k) {
-    return (k == 0) ? plan->hmin : (k == 1 ? plan->edge1 : __dadd_rn(plan->hmin, __dmul_rn((double)k, plan->delta)));
+    return cen_edge(k, plan->hmin, plan->edge1, plan->delta);
 }
 
 // ---- the certified peak pick (DESIGN.md §4.4.1) --------------------------------------------------------------------------
@@ -1026,6 +893,99 @@ __global__ void __launch_bounds__(256) k_center_pick(const unsigned long long* _
     (void)top_val;
 }
 
+// ---- the stepwise entries on the chain's kernels ------------------------------------------------------------------------------
+// The plan of a stepwise call: the caller's local window [r0, r1) and, with nbins > 0, its tiles and the caller's edges
+// hmin + k * hstep (edge1 = hmin + hstep, delta = hstep) with their threshold table and zeroed counters.  The window statistics need
+// no tiles here: k_center_window finds them itself.  nbins + 1 threads or more.
+__global__ void __launch_bounds__(256) k_center_set(const int64_t* __restrict__ prefix, int64_t ntiles, long long r0, long long r1, double hmin,
+                                                   double hstep, long long nbins, float scale, int fast, CenterPlan* __restrict__ plan,
+                                                   float* __restrict__ fe, unsigned long long* __restrict__ hist) {
+    const double edge1 = __dadd_rn(hmin, hstep);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        plan->lr0 = r0; plan->lr1 = r1;
+        plan->ticket = 0u;
+        plan->state = 1;
+        plan->certified = 0;
+        if (nbins > 0) {
+            long long w[4];
+            cen_window_tiles(prefix, ntiles, r0, r1, w);
+            for (int i = 0; i < 4; i++) plan->win[i] = w[i];
+            plan->hmin = hmin; plan->edge1 = edge1; plan->delta = hstep; plan->nbins = nbins;
+            plan->scale = scale;
+            plan->fast = fast;
+        }
+    }
+    if (nbins > 0)
+        cen_edge_table((long long)blockIdx.x * blockDim.x + threadIdx.x, (long long)gridDim.x * blockDim.x, nbins, hmin, edge1, hstep, fe, hist,
+                       nullptr);
+}
+
+// {count, min, max, sum, sumsq} of the kept samples whose LOCAL rank is in [r0, r1), summed in the chain's order (k_center_window):
+// interior tiles from the table, the cut tiles re-read from d_qad.  A shard passes the global window minus its rank offset
+// (clamped to its own count).
+extern "C" int urh_center_window_stats(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out5) {
+    h_out5[0] = 0.0; h_out5[1] = INFINITY; h_out5[2] = -INFINITY; h_out5[3] = 0.0; h_out5[4] = 0.0;
+    if (!tiles_match(ctx, d_qad, n)) URH_FAIL(ctx, URH_ERR_INVALID, "urh_afp_demod_tiles (same qad, same n) must precede urh_center_window_stats");
+    if (r1 <= r0) return URH_OK;
+    const int64_t ntiles = urh_div_up(n, URH_TILE);
+    const int64_t* prefix = (const int64_t*)ctx->center_prefix;
+    CenterPlan* plan;
+    CenStats* partial;
+    const int nb = ctx->sm_count * 2;
+    URH_CHECK(urh_arena(ctx, 1, &plan));
+    URH_CHECK(urh_arena(ctx, (size_t)nb + 2, &partial));
+    URH_LAUNCH(ctx, k_center_set, 1, 1, 0, prefix, ntiles, (long long)r0, (long long)r1, 0.0, 0.0, 0LL, 0.0f, 0, plan, nullptr, nullptr);
+    URH_LAUNCH(ctx, k_center_window, nb, 256, 0, d_qad, n, (const UrhTileStats*)ctx->center_ts, prefix, ntiles, plan, partial);
+    CenStats st;
+    URH_CUDA(ctx, cudaMemcpyAsync(ctx->h_mail, &plan->local, sizeof(CenStats), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    memcpy(&st, ctx->h_mail, sizeof(st));
+    h_out5[0] = (double)st.cnt; h_out5[1] = (double)st.mn; h_out5[2] = (double)st.mx; h_out5[3] = st.sum; h_out5[4] = st.sumsq;
+    return URH_OK;
+}
+
+// Counts for edges hmin + k*hstep, k = 0..nbins (np.arange) over the samples of LOCAL rank [r0, r1); needs the tile
+// table of the same array (urh_afp_demod_tiles / urh_center_stats) in the arena.
+extern "C" int urh_center_histogram_tiles(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double hmin,
+                                          double hstep, int64_t nbins, int64_t* h_hist) {
+    if (nbins <= 0) return URH_OK;
+    if (!tiles_match(ctx, d_qad, n)) URH_FAIL(ctx, URH_ERR_INVALID, "urh_afp_demod_tiles (same qad, same n) must precede urh_center_histogram_tiles");
+    if (nbins > (int64_t)1 << 30) URH_FAIL(ctx, URH_ERR_INVALID, "too many histogram bins");
+    if (r1 <= r0) {
+        memset(h_hist, 0, (size_t)nbins * sizeof(int64_t));
+        return URH_OK;
+    }
+    const int64_t ntiles = urh_div_up(n, URH_TILE);
+    const int64_t* prefix = (const int64_t*)ctx->center_prefix;
+    CenterPlan* plan;
+    float* fe;
+    unsigned long long* hist;
+    URH_CHECK(urh_arena(ctx, 1, &plan));
+    URH_CHECK(urh_arena(ctx, (size_t)nbins + 3, &fe));
+    URH_CHECK(urh_arena(ctx, (size_t)nbins, &hist));
+    // shared memory (48 KB without opt-in): histogram first, then the edge table if it still fits
+    const bool in_smem = nbins <= 12000;
+    const int edges_smem = (in_smem && nbins <= 6000) ? 1 : 0;
+    const size_t dyn = (in_smem ? (size_t)nbins * 4 : 0) + (edges_smem ? (size_t)(nbins + 3) * 4 : 0);
+    const float scale = (float)(1.0 / hstep);
+    // one-look-up binning needs the float guess to be good to half a bin
+    const double edge_abs = fmax(fabs(hmin), fabs(hmin + (double)nbins * hstep));
+    const int fast = (edges_smem && hstep > 0.0 && edge_abs / hstep < 1048576.0) ? 1 : 0;
+    const unsigned gs = (unsigned)min(urh_div_up(ntiles, 8), (int64_t)ctx->sm_count * 8);
+    URH_LAUNCH(ctx, k_center_set, (unsigned)urh_div_up(nbins + 1, 256), 256, 0, prefix, ntiles, (long long)r0, (long long)r1, hmin, hstep,
+               (long long)nbins, scale, fast, plan, fe, hist);
+    const CenterPlan* cplan = plan;
+    const float* cfe = fe;
+    if (fast) URH_LAUNCH(ctx, (k_hist_interior<true, true, 3>), gs, 256, dyn, d_qad, n, cplan, cfe, hist, prefix, edges_smem);
+    else if (edges_smem) URH_LAUNCH(ctx, (k_hist_interior<true, false, 3>), gs, 256, dyn, d_qad, n, cplan, cfe, hist, prefix, edges_smem);
+    else if (in_smem) URH_LAUNCH(ctx, (k_hist_interior<true, false, 4>), gs, 256, dyn, d_qad, n, cplan, cfe, hist, prefix, edges_smem);
+    else URH_LAUNCH(ctx, (k_hist_interior<false, false, 4>), gs, 256, dyn, d_qad, n, cplan, cfe, hist, prefix, edges_smem);
+    URH_LAUNCH(ctx, k_hist_window_ends, 2, 256, 0, d_qad, n, prefix, cplan, cfe, hist, (unsigned long long*)nullptr, (int64_t)1);
+    URH_CUDA(ctx, cudaMemcpyAsync(h_hist, hist, (size_t)nbins * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+
 // The chain.  ts = the demodulator's tile table of d_qad (arena); *d_plan_out stays valid until the next arena reset.
 // Enqueues everything on the context stream; no synchronisation.  world > 1: the context's NCCL communicator.
 // fine != NULL (world == 1 only): the demodulator's fine histogram of d_qad; k_center_certify may then decide the center without
@@ -1075,11 +1035,11 @@ int urh_center_chain(urh_ctx* ctx, const float* d_qad, int64_t n, const UrhTileS
     const size_t dyn = (size_t)CEN_MAX_BINS * 4 + (size_t)(CEN_MAX_BINS + 3) * 4;   // histogram + edge table, 48 KB
     const unsigned gs = (unsigned)min(urh_div_up(ntiles, 8), (int64_t)ctx->sm_count * 8);
     // the window's cut tiles (and, with a fine histogram, the interior tiles of its cut slabs), then the certificate
-    URH_LAUNCH(ctx, k_hist_window_ends_dev, fine ? 2 + ctx->sm_count * 4 : 2, 256, fine ? dyn : 0, d_qad, n, (const int64_t*)prefix,
+    URH_LAUNCH(ctx, k_hist_window_ends, fine ? 2 + ctx->sm_count * 4 : 2, 256, fine ? dyn : 0, d_qad, n, (const int64_t*)prefix,
                (const CenterPlan*)plan, (const float*)fe, hist, xhist, fine ? fine->slab_tiles : (int64_t)1);
     if (fine) URH_LAUNCH(ctx, k_center_certify, 1, CERT_THREADS, 0, *fine, plan, (const float*)fe, (const unsigned long long*)xhist, cert_lo, cert_hi);
-    URH_LAUNCH(ctx, (k_hist_interior_dev<true>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
-    URH_LAUNCH(ctx, (k_hist_interior_dev<false>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix);
+    URH_LAUNCH(ctx, (k_hist_interior<true, true, 3>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix, 1);
+    URH_LAUNCH(ctx, (k_hist_interior<true, false, 3>), gs, 256, dyn, d_qad, n, (const CenterPlan*)plan, (const float*)fe, hist, (const int64_t*)prefix, 1);
     if (world > 1) {
         URH_TL_MARK(ctx, "x3 histogram sum: enter");
         URH_CHECK(urh_nccl_allreduce_i64(ctx, (int64_t*)hist, CEN_MAX_BINS, 0));
