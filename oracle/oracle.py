@@ -107,9 +107,11 @@ def segment_messages_from_magnitudes(mags, noise_threshold):
 def fir_filter(x, taps):
     x = np.ascontiguousarray(x, dtype=np.complex64)
     taps = np.ascontiguousarray(taps, dtype=np.complex64)
+    # the reference's shape, np.zeros(N + M - 1)[:N]: N - 1 outputs without taps, ValueError (negative dimensions) for N = M = 0
+    shape = np.zeros(len(x) + len(taps) - 1, dtype=np.complex64)[: len(x)].shape
     out = np.zeros(len(x), dtype=np.complex64)
     lib().oracle_fir_filter(_p(x), C.c_int64(len(x)), _p(taps), C.c_int64(len(taps)), _p(out))
-    return out
+    return out[: shape[0]]
 
 
 def arr2decibel(arr):

@@ -67,8 +67,10 @@ def test_fir_filter_shard_with_history_equals_whole_capture(ctx, m):
     assert bits_equal(out.get(), ref)
 
 
-def test_fir_exact_sass_unchanged():
-    """the history mode is a template parameter: the instantiation urh_fir_filter launches keeps its machine code"""
+def test_fir_exact_sass_pinned():
+    """the machine code of the instantiation urh_fir_filter launches is pinned: the history mode is a template parameter, so the
+    shard entry cannot change it, and any change to the tap loop or the after-loop NaN recheck (k_fir_exact) shows here and has to
+    be re-recorded on purpose"""
     golden = json.load(open(os.path.join(ROOT, "tests", "golden", "fir_exact_sass.json")))
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -294,3 +294,68 @@ def test_oracle_pulse_edges_pinned_to_reference(oracle, request):
     qam = got["signed_zero_QAM"][0]
     assert (np.signbit(qam.x) & (qam.x == 0)).any() and (~np.signbit(qam.x) & (qam.x == 0)).any()
     assert not np.array_equal(got["signed_zero_QAM"][1], got["signed_zero_FSK"][1])
+
+
+def test_oracle_fir_edges_pinned_to_reference(oracle, request):
+    """The oracle's fir_filter against the reference's compiled fir_filter on the named cases of tests/fir_edge_cases.py: tap and sample
+    counts around the 1024-output block, non-finite samples at block, halo and head positions, non-finite taps at q = 0, m // 2 and
+    m - 1, the three branches of __mulsc3's Annex G recovery, sums that overflow and meet -inf, subnormals, signed zeros, tap counts
+    past the shared-memory tile and empty inputs.  Words are compared with NaN folded and -0 apart from +0.  The reference's outputs
+    are recorded in tests/golden/ref_fir_edges.json (large ones as digests); with oracle/_ref built the pin also runs live."""
+    import warnings
+
+    from fir_edge_cases import cases, fast_loop, folded
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette, same
+
+    def answer(fir, case):
+        try:
+            return folded(np.asarray(fir(case.x, case.taps)))
+        except ValueError:
+            return "ValueError"
+
+    c = Cassette("fir_edges", request.node.name)
+    sf = ref_loader.load_kernels()[0] if (RECORD or ref_loader.kernels_available()) else None
+    got = {}
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)
+        for case in cases():
+            mine = answer(oracle.fir_filter, case)
+            want = c.want(lambda: [case.name, answer(sf.fir_filter, case)])
+            assert want[0] == case.name, (want[0], case.name)
+            assert (mine == want[1]) if isinstance(mine, str) or isinstance(want[1], str) else same(mine, want[1]), case.name
+            if sf is not None:
+                live = answer(sf.fir_filter, case)
+                assert (mine == live) if isinstance(mine, str) or isinstance(live, str) else np.array_equal(mine, live), case.name
+            got[case.name] = (case, mine)
+    c.close()
+    assert len(got) == 685
+    # the corners the cases must reach: outputs where the naive product or a padded product gives what the reference does not
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)
+        differs = {name for name, (cs, y) in got.items()
+                   if cs.group not in ("large_m", "empty") and not np.array_equal(folded(fast_loop(cs.x, cs.taps)), y)}
+    assert {name for name, (cs, _) in got.items() if cs.group == "annexg"} <= differs
+    assert sum(got[k][0].group == "nonfinite_samples" for k in differs) >= 80
+    assert sum(got[k][0].group == "nonfinite_taps" for k in differs) >= 100
+    assert not differs & {name for name, (cs, _) in got.items() if cs.group in ("shapes", "subnormal", "signed_zero")}
+    # a non-finite tap at q = m - 1 only meets the zero initial state in the first m - 1 outputs
+    y = got["annexg_padded_inf_tap3_example"][1].view(np.float32)
+    assert np.array_equal(y[:4], np.array([0.5, 0.5, 1.25, 0.25], np.float32)) and np.isinf(y[4])
+    # recovered products: infinite, not NaN
+    assert np.isinf(got["annexg_inf_sample_example"][1].view(np.float32)[2:]).all()
+    y = got["annexg_overflow_nan_example"][1].view(np.float32)
+    assert y[0] == -np.inf and y[1] == np.inf
+    # an overflowed sum meets -inf: NaN in the real part without a NaN product
+    assert np.isnan(got["overflow_then_neginf_real"][1].view(np.float32)[0::2]).any()
+    # subnormal words survive (no flush to zero), and the outputs of all -0 terms are +0
+    tiny = np.float32(np.finfo(np.float32).tiny)
+    for name in ("subnormal_products", "subnormal_samples", "subnormal_taps", "subnormal_near_flt_min", "subnormal_tiny_sums"):
+        v = got[name][1].view(np.float32)
+        assert ((v != 0) & (np.abs(v) < tiny)).sum() > 10, name
+    assert (got["neg_zero_samples"][1] == 0).all() and (got["neg_zero_all_terms"][1] == 0).all()
+    assert (np.signbit(got["neg_zero_all_terms"][0].x.view(np.float32))).any()
+    # the reference's shapes for empty inputs
+    assert got["empty_taps_n0"][1] == "ValueError"
+    assert len(got["empty_taps_n1"][1]) == 0 and len(got["empty_taps_n3"][1]) == 4 and len(got["empty_samples_m2"][1]) == 0
+    assert {len(cs.taps) for cs, _ in got.values() if cs.group == "large_m"} == {12287, 12288, 20000}

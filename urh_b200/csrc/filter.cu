@@ -2,7 +2,8 @@
 // Filter.work / apply_fir_filter / apply_bandpass_filter Filter.py:31-46, 84-101).
 //
 // fir_filter is reproduced in the reference's exact accumulation order: y[k] = sum over i ascending of
-// x[i]*taps[k-i], every complex64 product and every add individually rounded (no FMA) — bit-identical output.
+// x[i]*taps[k-i], every complex64 product and every add individually rounded (no FMA) — bit-identical output, non-finite
+// samples and taps included (see urh_fir_filter).
 // A block stages its input tile (outputs + M-1 halo samples) in shared memory with cp.async.bulk (TMA 1-D bulk
 // copy, mbarrier completion); each thread then produces 4 consecutive outputs so that every tap fetched from
 // shared memory is used four times.  This kernel is FP32-ALU-bound (8*M unfused flops per sample), not
@@ -44,6 +45,21 @@ __device__ __forceinline__ void fir_mbar_wait(uint64_t* bar, uint32_t phase) {
         "DONE:\n"
         "}\n" ::"r"((uint32_t)__cvta_generic_to_shared(bar)),
         "r"(phase));
+}
+
+// One output as the reference computes it: +0, then x[k - q] * taps[q] for q = qmax .. 0 (ascending input index), each product
+// std::complex<float>'s (urh_cmulf, with the Annex G recovery) and each add rounded.  xk points at x[k]; qmax leaves out the zero
+// initial state.  The kernels below call it only for an output whose fast sum has both parts NaN (see urh_fir_filter).
+__device__ __noinline__ float2 fir_exact_output(const float2* xk, const float2* taps, int qmax) {
+    float2 acc = make_float2(0.f, 0.f);
+    for (int q = qmax; q >= 0; q--) {
+        const float2 v = xk[-q], h = taps[q];
+        float pr, pi;
+        urh_cmulf(v.x, v.y, h.x, h.y, pr, pi);
+        acc.x = __fadd_rn(acc.x, pr);
+        acc.y = __fadd_rn(acc.y, pi);
+    }
+    return acc;
 }
 
 // Exact-order complex64 FIR.  smem: [taps M float2][tile FIR_TILE + M - 1 float2]
@@ -103,6 +119,50 @@ __global__ void __launch_bounds__(FIR_THREADS) k_fir_exact(const float2* __restr
 #pragma unroll
     for (int r = 0; r < FIR_PER_THREAD; r++)
         if (k0 + r < n) y[k0 + r] = acc[r];
+    // both parts NaN: a product may have needed the Annex G recovery or been a padded 0 * non-finite tap (urh_fir_filter).  Such
+    // outputs are redone from global memory after the stores, so that nothing but a 4-bit mask lives past the tap loop.
+    unsigned redo = 0;
+#pragma unroll
+    for (int r = 0; r < FIR_PER_THREAD; r++)
+        if (k0 + r < n && isnan(acc[r].x) && isnan(acc[r].y)) redo |= 1u << r;
+    for (int r = 0; redo; r++, redo >>= 1)
+        if (redo & 1) y[k0 + r] = fir_exact_output(x + k0 + r, taps, HISTORY ? m - 1 : (int)min((int64_t)m - 1, k0 + r));
+}
+
+// The same sums for tap counts whose tile does not fit in shared memory: one output per thread, taps and samples read from global
+// memory, the real terms only (no zero initial state), the same descending q and the same recheck.
+template <bool HISTORY>
+__global__ void __launch_bounds__(FIR_THREADS) k_fir_exact_global(const float2* __restrict__ x, int64_t n, const float2* __restrict__ taps,
+                                                                   int m, float2* __restrict__ y) {
+    const int64_t k = (int64_t)blockIdx.x * FIR_THREADS + threadIdx.x;
+    if (k >= n) return;
+    const int qmax = HISTORY ? m - 1 : (int)min((int64_t)m - 1, k);
+    float2 acc = make_float2(0.f, 0.f);
+    for (int q = qmax; q >= 0; q--) {
+        const float2 v = x[k - q], h = taps[q];
+        const float pr = __fsub_rn(__fmul_rn(v.x, h.x), __fmul_rn(v.y, h.y));
+        const float pi = __fadd_rn(__fmul_rn(v.x, h.y), __fmul_rn(v.y, h.x));
+        acc.x = __fadd_rn(acc.x, pr);
+        acc.y = __fadd_rn(acc.y, pi);
+    }
+    if (isnan(acc.x) && isnan(acc.y)) acc = fir_exact_output(x + k, taps, qmax);
+    y[k] = acc;
+}
+
+#define FIR_SMEM_MAX (200 * 1024)
+
+template <bool HISTORY>
+static int fir_launch(urh_ctx* ctx, const float* d_x, int64_t n, const float* d_taps, int m, float* d_y) {
+    const size_t smem = (size_t)(((m + 1) & ~1) + FIR_TILE + m - 1 + 2) * sizeof(float2);
+    if (smem > FIR_SMEM_MAX) {   // m >= 12288
+        URH_LAUNCH(ctx, k_fir_exact_global<HISTORY>, (unsigned)urh_div_up(n, FIR_THREADS), FIR_THREADS, 0, (const float2*)d_x, n,
+                   (const float2*)d_taps, m, (float2*)d_y);
+        return URH_OK;
+    }
+    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact<HISTORY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    URH_LAUNCH(ctx, k_fir_exact<HISTORY>, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
+               (float2*)d_y);
+    return URH_OK;
 }
 
 // replaces signal_functions.fir_filter: x, y complex64[n] (device), taps complex64[m] (device)
@@ -112,16 +172,18 @@ extern "C" int urh_fir_filter(urh_ctx* ctx, const float* d_x, int64_t n, const f
         URH_CUDA(ctx, cudaMemsetAsync(d_y, 0, (size_t)n * 8, ctx->stream));
         return URH_OK;
     }
-    const size_t smem = (size_t)(((m + 1) & ~1) + FIR_TILE + m - 1 + 2) * sizeof(float2);
-    if (smem > 200 * 1024) URH_FAIL(ctx, URH_ERR_INVALID, "fir_filter: %d taps exceed the shared-memory tile (max ~11000)", m);
-    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // NOTE on the reference's zero products: for the first m-1 outputs the reference simply has fewer terms; adding
-    // the products of zero-padded samples (0*h = +-0) to a non-zero accumulator changes nothing, and the very first
-    // term of every output is x[0]*h (k < m) or a real sample, so the sums are bit-identical except for the sign of
-    // an all-zero result, which the reference (np.zeros start) also produces as +0 -> handled by starting at +0.
-    URH_LAUNCH(ctx, k_fir_exact<false>, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
-               (float2*)d_y);
-    return URH_OK;
+    // Why k_fir_exact's fast loop plus its recheck gives the reference's words.  The reference adds x[i] * taps[k - i] for its real
+    // samples only, to an output that starts at +0 (np.zeros), each product a std::complex<float> product (__mulsc3).  The fast loop
+    // multiplies naively and, for the first m-1 outputs, first adds the products of the zero initial state x[-1], x[-2], ...
+    // * A naive product differs from __mulsc3's only when both of its parts are NaN (only then does the recovery run).
+    // * A padded product 0 * taps[q] is +-0 in both parts when taps[q] is finite: added to +0 it leaves +0, so the real terms then
+    //   meet the accumulator the reference starts from.  When taps[q] is infinite or NaN, it is NaN in both parts.
+    // * Either exception makes both parts of the sum NaN, and NaN absorbs every later add.  So a sum that is not NaN in both parts
+    //   saw neither: it is the reference's sum.  A sum that is NaN in both parts is recomputed over its real terms with urh_cmulf
+    //   (fir_exact_output), in the same order.  Such outputs need a non-finite sample, tap or overflow, so the fast loop is untouched.
+    // HISTORY (a shard after the first) has no padding, so only the recovery applies.  Beyond the shared-memory tile
+    // (m >= 12288) k_fir_exact_global computes the same sums from global memory.
+    return fir_launch<false>(ctx, d_x, n, d_taps, m, d_y);
 }
 
 // One shard of a capture cut by contiguous sample range: has_history != 0 means d_x[-(m-1) .. -1] hold the previous shard's last
@@ -130,12 +192,7 @@ extern "C" int urh_fir_filter(urh_ctx* ctx, const float* d_x, int64_t n, const f
 extern "C" int urh_fir_filter_shard(urh_ctx* ctx, const float* d_x, int64_t n, int has_history, const float* d_taps, int m, float* d_y) {
     if (!has_history || m <= 1) return urh_fir_filter(ctx, d_x, n, d_taps, m, d_y);
     if (n <= 0) return URH_OK;
-    const size_t smem = (size_t)(((m + 1) & ~1) + FIR_TILE + m - 1 + 2) * sizeof(float2);
-    if (smem > 200 * 1024) URH_FAIL(ctx, URH_ERR_INVALID, "fir_filter_shard: %d taps exceed the shared-memory tile (max ~11000)", m);
-    URH_CUDA(ctx, cudaFuncSetAttribute(k_fir_exact<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    URH_LAUNCH(ctx, k_fir_exact<true>, (unsigned)urh_div_up(n, FIR_TILE), FIR_THREADS, smem, (const float2*)d_x, n, (const float2*)d_taps, m,
-               (float2*)d_y);
-    return URH_OK;
+    return fir_launch<true>(ctx, d_x, n, d_taps, m, d_y);
 }
 
 // Direct convolution sample c[t + offset], c = full convolution of x (complex64) with h (complex128 taps),

@@ -470,6 +470,14 @@ def fir_filter(input_samples, filter_taps):
         input_samples = np.ascontiguousarray(input_samples)
     taps = np.ascontiguousarray(np.asarray(filter_taps, dtype=np.complex64))
     n = len(input_samples)
+    if len(taps) == 0:
+        # the reference returns np.zeros(N + M - 1)[:N]: N - 1 zeros without taps, and np.zeros(-1) raises for N = 0
+        if n == 0:
+            raise ValueError("negative dimensions are not allowed")
+        if not on_device:
+            return np.zeros(n - 1, dtype=np.complex64)
+        out = DeviceArray(ctx, (n - 1,), np.complex64)
+        return out.zero() if n > 1 else out
     if not on_device and n and filter_use_stream(_lib.FILTER_FIR, n, n, np.float32, len(taps), 0, device_budget(ctx)):
         host = np.empty(n, dtype=np.complex64)
         ctx.check(ctx.lib.urh_fir_filter_stream(ctx.handle, _host_ptr(input_samples), n, _host_ptr(taps) if len(taps) else None, len(taps),
