@@ -164,6 +164,11 @@ int urh_fir_filter(urh_ctx* ctx, const float* d_x, int64_t n, const float* d_tap
 int urh_convolve_c128(urh_ctx* ctx, const float* d_x, int64_t n, const double* d_taps, int m, int64_t offset,
                       int64_t out_len, float* d_y);
 int urh_dc_correction(urh_ctx* ctx, const float* d_iq, int64_t n, float* d_out, int exact_order);
+/* the FFT branch of the band-pass and Filter.fft_convolve_1d (Filter.py:69-82): one non-finite sample makes every output NaN + NaN j.
+ * urh_nonfinite_flag: *d_flag = 1 if any of the n complex64 values has a NaN or infinite part (never cleared);
+ * urh_nan_fill_if: d_y[0 .. n) = NaN + NaN j if *d_flag != 0.  Both asynchronous on the context stream. */
+int urh_nonfinite_flag(urh_ctx* ctx, const float* d_x, int64_t n, int* d_flag);
+int urh_nan_fill_if(urh_ctx* ctx, float* d_y, int64_t n, const int* d_flag);
 /* the same for an integer capture: numpy promotes to float64 (exact integer column sums), d_out = double[n][2] */
 int urh_dc_correction_int(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, double* d_out);
 /* The filters of one shard of a capture cut by contiguous sample range (urh_b200/dist.py).

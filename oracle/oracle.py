@@ -329,12 +329,21 @@ def design_windowed_sinc_bandpass(f_low, f_high, bw):
 
 
 def fft_convolve_1d(x, h):
-    """Filter.py:69-82"""
+    """Filter.py:69-82: complex transforms when x or h is complex, else rfft / irfft (a real result)"""
     n = len(x) + len(h) - 1
     n_opt = 1 << (n - 1).bit_length()
-    result = np.fft.ifft(np.fft.fft(x, n_opt) * np.fft.fft(h, n_opt), n_opt)[0:n]
+    if np.iscomplexobj(x) or np.iscomplexobj(h):
+        fft, ifft = np.fft.fft, np.fft.ifft
+    else:
+        fft, ifft = np.fft.rfft, np.fft.irfft
+    result = ifft(fft(x, n_opt) * fft(h, n_opt), n_opt)[0:n]
     too_much = (len(result) - len(x)) // 2
     return result[too_much:-too_much]
+
+
+def dc_correction(x):
+    """Filter.py:31-33 (Filter.work with FilterType.dc_correction)"""
+    return x - np.mean(x, axis=0)
 
 
 def apply_bandpass_filter(data, f_low, f_high, filter_bw=0.08):

@@ -359,3 +359,131 @@ def test_oracle_fir_edges_pinned_to_reference(oracle, request):
     assert got["empty_taps_n0"][1] == "ValueError"
     assert len(got["empty_taps_n1"][1]) == 0 and len(got["empty_taps_n3"][1]) == 4 and len(got["empty_samples_m2"][1]) == 0
     assert {len(cs.taps) for cs, _ in got.values() if cs.group == "large_m"} == {12287, 12288, 20000}
+
+
+def test_oracle_spectral_edges_pinned_to_reference(oracle, request, tmp_path):
+    """The oracle's STFT, dB map, FTA amplitudes, band-pass, fft_convolve_1d and DC correction against the reference's own Filter and
+    Spectrogram (Spectrogram.stft, its __calculate_spectrogram, export_to_fta, Filter.apply_bandpass_filter, Filter.fft_convolve_1d and
+    Filter.work with FilterType.dc_correction) on the named cases of tests/spectral_edge_cases.py.  Per result: dtype, shape, the words
+    with NaN folded and -0 apart from +0, and the per-component classes (finite, NaN, +inf, -inf), recorded as digests in
+    tests/golden/ref_spectral_edges.json and replayed where the reference is absent; with the reference present the pin also runs live."""
+    import warnings
+
+    from oracle import ref_loader
+    from oracle.cassette import RECORD, Cassette, digest
+    from spectral_edge_cases import answers, bad_frames, cases, classes, folded, frames_of, hop_of
+
+    def pack(results):
+        return [[k, np.asarray(a).dtype.str, list(np.shape(a)), digest(folded(a)), digest(classes(a))] for k, a in results]
+
+    def o_fta(x, W, ov):
+        return np.flipud(oracle.spectrogram_db(x, W, ov).T)
+
+    def functions(ns):
+        if ns is None:
+            return dict(stft=oracle.stft, spectrogram_db=lambda x, W, ov: oracle.spectrogram_db(x, W, ov), fta=o_fta,
+                        apply_bandpass_filter=oracle.apply_bandpass_filter, fft_convolve_1d=oracle.fft_convolve_1d,
+                        dc_correction=oracle.dc_correction)
+
+        def r_fta(x, W, ov):
+            path = str(tmp_path / "spectrogram.fta")
+            ns.Spectrogram(x, W, ov).export_to_fta(1e6, path, include_amplitude=True)
+            rec = np.fromfile(path, dtype=[("f", np.float64), ("t", np.uint32), ("a", np.float32)])
+            return rec["a"].reshape(W, -1, 3)[:, :, 0]
+        return dict(stft=lambda x, W, ov: ns.Spectrogram(x, W, ov).stft(x),
+                    spectrogram_db=lambda x, W, ov: ns.Spectrogram(x, W, ov)._Spectrogram__calculate_spectrogram(x), fta=r_fta,
+                    apply_bandpass_filter=ns.Filter.apply_bandpass_filter, fft_convolve_1d=ns.Filter.fft_convolve_1d,
+                    dc_correction=lambda x: ns.Filter([], ns.FilterType.dc_correction).work(x))
+
+    c = Cassette("spectral_edges", request.node.name)
+    ns = ref_loader.load_python_layer() if (RECORD or ref_loader.python_layer_available()) else None
+    mine_f, ref_f = functions(None), (functions(ns) if ns is not None else None)
+    got = {}
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore", RuntimeWarning)
+        for case in cases():
+            mine = answers(case, **mine_f)
+            live = answers(case, **ref_f) if ref_f is not None else None
+            want = c.want(lambda: [case.name, pack(live)])
+            assert want[0] == case.name, (want[0], case.name)
+            assert pack(mine) == want[1], case.name
+            got[case.name] = (case, dict(mine))
+        # the hop-0 overlap: the reference divides by zero, and so does the oracle
+        kinds = []
+        for f in (mine_f, ref_f):
+            try:
+                f["stft"](np.ones(100, np.complex64), 64, 1.0)
+                kinds.append("returned")
+            except Exception as e:   # noqa: BLE001 - the exception's type is what is compared
+                kinds.append(type(e).__name__)
+        assert kinds[0] == c.want(lambda: kinds[1]) == "ZeroDivisionError"
+    c.close()
+    assert len(got) == 464, len(got)
+
+    # the corners the cases must reach
+    with warnings.catch_warnings(), np.errstate(all="ignore"):
+        warnings.simplefilter("ignore", RuntimeWarning)
+        # band-pass, FFT branch: one non-finite sample makes every output NaN in both parts; a direct convolution would not
+        all_nan = []
+        for name, (cs, r) in got.items():
+            if cs.group != "bandpass":
+                continue
+            y = r["out"]
+            m = len(oracle.design_windowed_sinc_bandpass(0.0, 0.1, cs.bw))
+            fft_branch = not m < 8 * np.log(np.sqrt(len(cs.x)))
+            bad = not np.isfinite(cs.x.view(np.float32)).all()
+            if fft_branch and bad:
+                assert np.isnan(y.real).all() and np.isnan(y.imag).all(), name
+                h = oracle.design_windowed_sinc_bandpass(*sorted((cs.f_low, cs.f_high)), cs.bw)
+                direct = np.convolve(cs.x.astype(np.complex128), h, "full")[(m - 1) // 2: (m - 1) // 2 + len(cs.x)]
+                if np.isfinite(direct).sum() > len(cs.x) // 2:
+                    all_nan.append(name)
+            elif not bad and not (fft_branch and ("fft_overflow" in name or "huge_3e38" in name)):
+                assert np.isfinite(y).all(), name
+        assert len(all_nan) >= 6 and "bandpass_m51_fft_n5000_inf" in all_nan, all_nan
+        # ... and the single-precision transform of a complex64 capture overflows on samples near FLT_MAX: all NaN, where the float64
+        # result of the same operation is finite (the device's double convolution gives the latter, DESIGN.md §4.5)
+        for name in ("bandpass_m41_fft_fft_overflow", "bandpass_m51_fft_fft_overflow", "bandpass_m41_fft_huge_3e38", "bandpass_m51_fft_huge_3e38"):
+            cs, r = got[name]
+            assert np.isnan(r["out"]).all(), name
+            assert np.isfinite(oracle.apply_bandpass_filter(cs.x.astype(np.complex128), cs.f_low, cs.f_high, cs.bw)).all(), name
+        assert np.isfinite(got["bandpass_m51_direct_fft_overflow"][1]["out"]).all()
+        # fft_convolve_1d of real x and real h: the rfft branch's real result
+        assert got["convolve_real_real"][1]["out"].dtype == np.float64 and got["convolve_real_f32"][1]["out"].dtype == np.float32
+        assert np.isnan(got["convolve_inf_tap"][1]["out"]).all() and np.isnan(got["convolve_real_nonfinite"][1]["out"]).all()
+        # STFT: every bin of a frame that reads a non-finite sample is NaN + NaN j (numpy's complex product forms (inf, NaN) or NaN, and
+        # the transform spreads it), so its dB value is NaN; a real-window product would leave whole frames with finite or infinite parts
+        whole_nan = []
+        for name, (cs, r) in got.items():
+            if cs.group not in ("stft", "segments"):
+                continue
+            hop = hop_of(cs.W, cs.ov)
+            bad = bad_frames(cs.x, cs.W, hop)
+            X, db = r["stft"], r["db"]
+            assert X.shape == db.shape == (frames_of(len(cs.x), cs.W, hop), cs.W)
+            assert (np.isnan(X.real) & np.isnan(X.imag))[bad].all() and np.isnan(db[bad]).all(), name
+            assert np.isfinite(X[~bad]).all(), name
+            if cs.group == "stft" and bad.any():
+                x = np.concatenate([cs.x, np.zeros(max(0, cs.W - len(cs.x)), np.complex64)])
+                w = np.hanning(cs.W)
+                for f in np.nonzero(bad)[0]:
+                    fr = x[f * hop: f * hop + cs.W]
+                    prod = np.empty(cs.W, np.complex128)
+                    prod.real, prod.imag = fr.real * w, fr.imag * w
+                    real_win = np.fft.fft(prod)
+                    if np.isnan(X[f]).all() and not (np.isnan(real_win.real) & np.isnan(real_win.imag)).all():
+                        whole_nan.append(name)
+                        break
+        assert len(whole_nan) >= 100, len(whole_nan)
+        # huge and squared-overflow captures: a +inf dB value from float32 |X|^2, with finite STFT bins
+        assert np.isposinf(got["stft_W1024_ov0.5_sq_overflow"][1]["db"]).any()
+        assert np.isposinf(got["stft_W128_ov0.5_huge_1e30"][1]["db"]).all()
+        # DC: float32 column sums that overflow give non-finite columns up to 2^22 rows; a NaN or +-inf column is NaN
+        for n in (2, 1025, 1 << 22):
+            y = got["dc_n%d_overflow_col0" % n][1]["out"]
+            assert not np.isfinite(y[:, 0]).any() and np.isfinite(y[:, 1]).all(), n
+            assert np.isnan(got["dc_n%d_nan_col0" % n][1]["out"][:, 0]).all()
+            assert np.isnan(got["dc_n%d_pm_inf_col1" % n][1]["out"][:, 1]).all()
+        y = got["dc_n1025_subnormal_negzero"][1]["out"]
+        assert (y[:, 1] == 0).all() and np.signbit(y[:, 1]).all()   # the column sum starts from +0: -0 - (+0) = -0
+        assert got["dc_int16_n1025_extremes"][1]["out"].dtype == np.float64

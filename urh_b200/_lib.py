@@ -104,6 +104,8 @@ SIGNATURES = {
     "urh_fir_filter": (i32, [vp, vp, i64, vp, i32, vp]),
     "urh_convolve_c128": (i32, [vp, vp, i64, vp, i32, i64, i64, vp]),
     "urh_dc_correction": (i32, [vp, vp, i64, vp, i32]),
+    "urh_nonfinite_flag": (i32, [vp, vp, i64, vp]),
+    "urh_nan_fill_if": (i32, [vp, vp, i64, vp]),
     "urh_dc_correction_int": (i32, [vp, vp, i32, i64, vp]),
     "urh_fir_filter_shard": (i32, [vp, vp, i64, i32, vp, i32, vp]),
     "urh_dc_column_sums": (i32, [vp, vp, i64, i32, vp, vp]),

@@ -284,6 +284,38 @@ extern "C" int urh_convolve_c128(urh_ctx* ctx, const float* d_x, int64_t n, cons
     return URH_OK;
 }
 
+// ---- the FFT branch of the band-pass and fft_convolve_1d (Filter.py:69-82): the reference transforms the whole capture, so one
+// non-finite sample makes every output NaN + NaN j.  The direct convolution above leaves that to the outputs that read the sample.
+// Every sample feeds at least one output of the centred crop, and with finite taps an output that reads a non-finite sample is not
+// finite, so the caller flags the OUTPUTS and fills them all when one is not finite (DESIGN.md §4.5).
+// *flag = 1 if any of the count floats is NaN or infinite (never cleared here, so that a flag can be carried over several calls)
+__global__ void k_nonfinite_flag(const float* __restrict__ x, int64_t count, int* __restrict__ flag) {
+    bool bad = false;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) bad |= !isfinite(x[i]);
+    if (__syncthreads_or(bad) && threadIdx.x == 0) *flag = 1;
+}
+
+__global__ void k_nan_fill_if(float* __restrict__ y, int64_t count, const int* __restrict__ flag) {
+    if (!*flag) return;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) y[i] = __int_as_float(0x7fc00000);
+}
+
+extern "C" int urh_nonfinite_flag(urh_ctx* ctx, const float* d_x, int64_t n, int* d_flag) {
+    if (n <= 0) return URH_OK;
+    const unsigned grid = (unsigned)min(urh_div_up(2 * n, 256), (int64_t)ctx->sm_count * 16);
+    URH_LAUNCH(ctx, k_nonfinite_flag, grid, 256, 0, d_x, 2 * n, d_flag);
+    return URH_OK;
+}
+
+extern "C" int urh_nan_fill_if(urh_ctx* ctx, float* d_y, int64_t n, const int* d_flag) {
+    if (n <= 0) return URH_OK;
+    const unsigned grid = (unsigned)min(urh_div_up(2 * n, 256), (int64_t)ctx->sm_count * 16);
+    URH_LAUNCH(ctx, k_nan_fill_if, grid, 256, 0, d_y, 2 * n, d_flag);
+    return URH_OK;
+}
+
 // ---- DC correction: x - mean(x, axis=0) (Filter.py:32-33) --------------------------------------------------------------
 // numpy's np.mean over axis 0 of a C-contiguous float32 (n,2) array accumulates each column naively in float32 in
 // row order (SURVEY H9).  exact != 0 reproduces that serial chain (one lane per column, the warp streams the data

@@ -24,6 +24,15 @@
         }                                                                                       \
     } while (0)
 
+// sample * window value as the STFT's input.  A non-finite sample gives NaN + NaN j, so every bin of each frame that reads it is
+// NaN + NaN j whatever the order of the butterflies, as in the reference: numpy promotes the window to complex, so (inf, 0) * g is
+// (inf, NaN) and inf * 0 is NaN, and its transform of the frames spreads that to both parts of every bin (DESIGN.md §4.6).  A real
+// product would leave finite and infinite bins: +inf dB where the reference has NaN.
+__device__ __forceinline__ double2 stft_windowed(float2 s, double g) {
+    if (!(isfinite(s.x) && isfinite(s.y))) return make_double2(__longlong_as_double(0x7ff8000000000000ll), __longlong_as_double(0x7ff8000000000000ll));
+    return make_double2((double)s.x * g, (double)s.y * g);
+}
+
 // frames[f][w] = x[(f0+f)*hop + w] * window[w]  (complex128; samples beyond n are zero: Spectrogram.py:102-103)
 __global__ void k_stft_window(const float2* __restrict__ x, int64_t n, int W, int hop, const double* __restrict__ window,
                               int64_t f0, int64_t nframes, double2* __restrict__ frames) {
@@ -34,11 +43,7 @@ __global__ void k_stft_window(const float2* __restrict__ x, int64_t n, int W, in
         const int w = (int)(idx - f * W);
         const int64_t i = (f0 + f) * hop + w;
         double2 v = make_double2(0.0, 0.0);
-        if (i < n) {
-            const float2 s = x[i];
-            const double g = window[w];
-            v = make_double2((double)s.x * g, (double)s.y * g);
-        }
+        if (i < n) v = stft_windowed(x[i], window[w]);
         frames[idx] = v;
     }
 }
@@ -258,7 +263,7 @@ __device__ __forceinline__ const double2* stft_r16_fft(const float2* __restrict_
             g[m] = window[w];
         }
 #pragma unroll
-        for (int m = 0; m < 16; m++) a[stft_pad(tid + T * m)] = make_double2((double)sm[m].x * g[m], (double)sm[m].y * g[m]);
+        for (int m = 0; m < 16; m++) a[stft_pad(tid + T * m)] = stft_windowed(sm[m], g[m]);
     }
     __syncthreads();
     constexpr int NPASS16 = LOG2W / 4;

@@ -729,6 +729,13 @@ def apply_bandpass_filter_sharded(ctx, hx, sb: ShardBuffer, bounds, f_low, f_hig
     out = ShardBuffer(ctx, sb.n, np.float32, halo=out_h)
     ctx.check(ctx.lib.urh_convolve_c128(ctx.handle, C.c_void_p(win.ptr), len(win), C.c_void_p(d_t.ptr), len(h), int(offset), sb.n,
                                         C.c_void_p(out.shard.ptr)))
+    if not len(h) < 8 * math.log(math.sqrt(bounds[-1][1])):
+        # the FFT branch: one non-finite sample anywhere in the capture makes every output NaN + NaN j (Filter._convolve_full_slice)
+        flag = to_device(np.zeros(1, np.int32), ctx)
+        ctx.check(ctx.lib.urh_nonfinite_flag(ctx.handle, C.c_void_p(out.shard.ptr), sb.n, C.c_void_p(flag.ptr)))
+        if any(int(f) for f in hx.allgather(int(flag.get()[0]))):
+            flag = to_device(np.ones(1, np.int32), ctx)
+            ctx.check(ctx.lib.urh_nan_fill_if(ctx.handle, C.c_void_p(out.shard.ptr), sb.n, C.c_void_p(flag.ptr)))
     exchange_halos(ctx, hx, out, out_halos)
     ctx.sync()
     return out

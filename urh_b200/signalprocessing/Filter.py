@@ -104,12 +104,16 @@ class Filter(object):
         return N + 1 if N % 2 == 0 else N  # odd length
 
     @staticmethod
-    def _convolve_full_slice(data: np.ndarray, h: np.ndarray, offset: int, out_len: int) -> np.ndarray:
+    def _convolve_full_slice(data: np.ndarray, h: np.ndarray, offset: int, out_len: int, fft_branch=False) -> np.ndarray:
         """full_convolution(data, h)[offset : offset + out_len] on the GPU (complex128 taps, double accumulation); a host capture whose
-        resident call does not fit the device budget streams through the windowed ring"""
+        resident call does not fit the device budget streams through the windowed ring.  fft_branch: the reference transforms the whole
+        capture (Filter.py:69-82), so one non-finite sample or tap makes every output NaN + NaN j.  Every sample feeds an output of the
+        centred crop and the taps are finite past the first check, so a non-finite output is what flags it (DESIGN.md §4.5)."""
         ctx = _lib.default_context()
         x = np.ascontiguousarray(data, dtype=np.complex64)
         taps = np.ascontiguousarray(h, dtype=np.complex128)
+        if fft_branch and not np.isfinite(taps).all():
+            return np.full(max(out_len, 0), complex(np.nan, np.nan), dtype=np.complex64)
         if (len(x) and len(taps) and out_len > 0
                 and signal_functions.filter_use_stream(_lib.FILTER_CONVOLVE, len(x), out_len, np.float32, len(taps), offset,
                                                        signal_functions.device_budget(ctx))):
@@ -117,12 +121,21 @@ class Filter(object):
             ctx.check(ctx.lib.urh_convolve_c128_stream(ctx.handle, x.ctypes.data_as(C.c_void_p), len(x), taps.ctypes.data_as(C.c_void_p),
                                                        len(taps), int(offset), int(out_len), signal_functions.FILTER_STREAM_CHUNK,
                                                        signal_functions.STREAM_RING, out.ctypes.data_as(C.c_void_p)))
+            if fft_branch:
+                words = out.view(np.float32)
+                step = 1 << 22
+                if not all(np.isfinite(words[i: i + step]).all() for i in range(0, len(words), step)):
+                    out.fill(complex(np.nan, np.nan))
             return out
         d_x = to_device(x.view(np.float32), ctx)
         d_t = to_device(taps.view(np.float64), ctx)
         out = DeviceArray(ctx, (out_len,), np.complex64)
         ctx.check(ctx.lib.urh_convolve_c128(ctx.handle, C.c_void_p(d_x.ptr), len(x), C.c_void_p(d_t.ptr), len(taps), int(offset),
                                             int(out_len), C.c_void_p(out.ptr)))
+        if fft_branch:
+            flag = to_device(np.zeros(1, np.int32), ctx)
+            ctx.check(ctx.lib.urh_nonfinite_flag(ctx.handle, C.c_void_p(out.ptr), int(out_len), C.c_void_p(flag.ptr)))
+            ctx.check(ctx.lib.urh_nan_fill_if(ctx.handle, C.c_void_p(out.ptr), int(out_len), C.c_void_p(flag.ptr)))
         return out.get()
 
     @staticmethod
@@ -130,13 +143,18 @@ class Filter(object):
         """Filter.py:69-82 — centred crop of the full convolution (the reference computes it with a power-of-two FFT in
         complex128; here it is a direct convolution on the GPU with complex128 taps and double accumulation, returned as
         complex64 — what every reference caller casts the result to (IQArray) — i.e. the values agree to 1e-5 of the signal
-        scale, DESIGN.md 4.5, not to float64 precision).  len(h) <= 2 gives too_much == 0 and the reference's
-        ``result[0:-0]`` is EMPTY: reproduced."""
+        scale, DESIGN.md 4.5, not to float64 precision).  Real x and real h take the reference's rfft / irfft branch: the real
+        part, as float64 (float32 when both are float32).  One non-finite sample or tap makes every output NaN, as the transform
+        does.  len(h) <= 2 gives too_much == 0 and the reference's ``result[0:-0]`` is EMPTY: reproduced."""
+        x, h = np.asarray(x), np.asarray(h)
+        real = not (np.iscomplexobj(x) or np.iscomplexobj(h))
+        dtype = (np.float32 if x.dtype == h.dtype == np.float32 else np.float64) if real else np.complex64
         n = len(x) + len(h) - 1
         too_much = (n - len(x)) // 2
         if too_much == 0:
-            return np.zeros(0, dtype=np.complex64)
-        return Filter._convolve_full_slice(x, h, too_much, n - 2 * too_much)
+            return np.zeros(0, dtype=dtype)
+        y = Filter._convolve_full_slice(x, h, too_much, n - 2 * too_much, fft_branch=True)
+        return y.real.astype(dtype) if real else y
 
     @staticmethod
     def bandpass_taps(f_low, f_high, filter_bw=0.08):
