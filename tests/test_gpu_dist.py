@@ -1,4 +1,9 @@
-"""GPU (>= 2 devices): sharded capture over NCCL == single-GPU result.  Skipped on a 1-GPU box."""
+"""GPU (>= 2 devices): sharded capture over NCCL == single-GPU result.  Skipped on a 1-GPU box.
+
+tests/test_gpu_dist_one_gpu.py runs the noise level, segmentation, center protocol, sharded Costas loop, estimate() and halo paths
+rank by rank on one GPU with host stand-ins for the NCCL calls dist.py makes from Python.  What only this test covers is NCCL itself and the
+exchanges the library makes from C: the sharded digitizer (urh_shard_digitize), the fused demod + center + digitize step
+(urh_shard_demod_center_digitize) and the center chain's rank/world mode."""
 import os
 import subprocess
 import sys

@@ -1,5 +1,9 @@
 """GPU (>= 2 devices): the sharded band-pass, FIR, DC correction, dB map and spectrogram images (urh_b200.dist, NCCL halos) equal the
-single-GPU public functions bit for bit.  Skipped on a 1-GPU box."""
+single-GPU public functions bit for bit.  Skipped on a 1-GPU box.
+
+The same entries, with their plans, halo exchanges and validation, run rank by rank on one GPU in tests/test_gpu_dist_one_gpu.py
+(host stand-ins for the NCCL calls); this test adds real NCCL send/recv and all-gathers between devices, and the band-passed
+demod + center + digitize chain, whose center and digitizer exchange from inside the library."""
 import os
 import subprocess
 import sys

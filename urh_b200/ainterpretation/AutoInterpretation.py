@@ -385,7 +385,8 @@ def center_stats_from_window(kept, r0, r1, w):
         st[2] = st[1]  # empty window: no center
         return st
     mean = w[3] / cnt
-    ss = max(0.0, w[4] - cnt * mean * mean)
+    # a window of one value has no spread: Σx² − n·mean² can leave a rounding residue, numpy's variance of it is far below its ulp
+    ss = 0.0 if w[1] == w[2] else max(0.0, w[4] - cnt * mean * mean)
     st[3], st[4], st[5], st[6] = w[1], w[2], mean, ss / cnt
     return st
 

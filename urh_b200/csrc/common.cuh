@@ -64,6 +64,7 @@ struct urh_ctx {
     int64_t costas_stats[3];
     int64_t costas_redone;  // super-chunks the stitch pass had to chain itself
     int64_t costas_stitch[4];  // {super-chunks adopted from family A, from family B, chained by the stitch warp, segs}
+    void* costas_shard;   // the sharded PSK run between urh_costas_shard_speculate and its adopt / resolve (costas_spec.cu)
     // cuFFT plans of detect_modulation / cwt_haar: [0] C2C, [1] Z2Z, batch 2, length mod_plan_n
     int mod_plan[2];
     int mod_plan_valid[2];
@@ -173,6 +174,7 @@ struct UrhCostasStream {
     int segs;
 };
 int urh_costas_stream_begin(urh_ctx* ctx, UrhCostasStream* S);
+void urh_costas_shard_release(urh_ctx* ctx);
 int urh_costas_stream_chunk(urh_ctx* ctx, UrhCostasStream* S, int64_t c, const void* d_iq, int dtype, int64_t n, float noise_sqrd,
                             int loop_order, float bandwidth, float* d_out);
 int urh_costas_stream_end(urh_ctx* ctx, const UrhCostasStream* S);

@@ -31,6 +31,7 @@ extern "C" int urh_ctx_create(int device, urh_ctx** out) {
     ctx->shard_tiles = nullptr;
     ctx->shard_staging = nullptr;
     ctx->shard_state = nullptr;
+    ctx->costas_shard = nullptr;
     ctx->bits_valid = 0;
     ctx->mod_plan_valid[0] = ctx->mod_plan_valid[1] = 0;
     ctx->center_prefix = nullptr;
@@ -91,6 +92,7 @@ extern "C" void urh_ctx_destroy(urh_ctx* ctx) {
     for (auto& b : ctx->arena) cudaFree(b.ptr);
     if (ctx->pulses) cudaFree(ctx->pulses);
     if (ctx->shard_state) free(ctx->shard_state);
+    urh_costas_shard_release(ctx);
     if (ctx->h_mail) cudaFreeHost(ctx->h_mail);
     if (ctx->ts_mem) cudaFree(ctx->ts_mem);
     if (ctx->step_dev) cudaFree(ctx->step_dev);

@@ -750,7 +750,16 @@ int urh_costas_stream_end(urh_ctx* ctx, const UrhCostasStream* S) {
 // d_iq points at the shard's first own sample; later shards have URH_COSTAS_HALO samples of the preceding shard stored in
 // front of it.  urh_costas_shard_speculate is asynchronous; urh_costas_shard_resolve needs the preceding shard's final
 // loop state (state_in = {freq, phase}; ignored on the first shard) and returns this shard's.
-static CsRun g_shard_run;  // one sharded PSK demodulation in flight per process (one process per GPU)
+// The run lives on the context, so every context of a process can hold its own sharded run between these calls.
+static CsRun& shard_run(urh_ctx* ctx) {
+    if (!ctx->costas_shard) ctx->costas_shard = new CsRun();
+    return *(CsRun*)ctx->costas_shard;
+}
+
+void urh_costas_shard_release(urh_ctx* ctx) {
+    delete (CsRun*)ctx->costas_shard;
+    ctx->costas_shard = nullptr;
+}
 
 extern "C" int urh_costas_halo_samples(void) { return CS_WARM; }
 
@@ -760,7 +769,7 @@ extern "C" int urh_costas_shard_speculate(urh_ctx* ctx, const void* d_iq, int dt
     if (order != 2 && order != 4) URH_FAIL(ctx, URH_ERR_INVALID, "sharded PSK: loop order 2 or 4");
     volatile float nm = noise_mag;
     volatile float sq = nm * nm;
-    CsRun& R = g_shard_run;
+    CsRun& R = shard_run(ctx);
     URH_CHECK(cs_params(ctx, &R.P, dtype, sq, order, bandwidth));
     R.iq = d_iq; R.dtype = dtype; R.n = n; R.start = first_shard ? (CS_EXACT | CS_CAP) : 0; R.out = d_out;
     R.st0 = nullptr;
@@ -773,14 +782,14 @@ extern "C" int urh_costas_shard_resolve(urh_ctx* ctx, const float* h_state_in, f
     CsState in;
     in.freq = h_state_in ? h_state_in[0] : 0.f;
     in.phase = h_state_in ? h_state_in[1] : 1.5f;
-    return cs_resolve(ctx, g_shard_run, in, h_state_out);
+    return cs_resolve(ctx, shard_run(ctx), in, h_state_out);
 }
 
 // Later shards: hop over the shard under each of the `order` hypotheses "the shard starts in candidate h's start state",
 // all at once (one warp each), independent of the preceding shard.  h_out[h] = {start.freq, start.phase, end.freq, end.phase}.
 // The first shard has one true run: h_out[0] = {initial state, end state}.  Returns the number of hypotheses in *count.
 extern "C" int urh_costas_shard_hypotheses(urh_ctx* ctx, float* h_out, int* count) {
-    CsRun& R = g_shard_run;
+    CsRun& R = shard_run(ctx);
     const bool first_shard = R.start & CS_EXACT;
     const int nh = first_shard ? 1 : R.nbr;
     CsState none;
@@ -802,7 +811,7 @@ extern "C" int urh_costas_shard_hypotheses(urh_ctx* ctx, float* h_out, int* coun
 
 // Adopt hypothesis h (its start state equalled, bit for bit, the preceding shard's end state): assemble + fix.
 extern "C" int urh_costas_shard_adopt(urh_ctx* ctx, int h, float* h_state_out) {
-    CsRun& R = g_shard_run;
+    CsRun& R = shard_run(ctx);
     if (h < 0 || h >= ((R.start & CS_EXACT) ? 1 : R.nbr)) URH_FAIL(ctx, URH_ERR_INVALID, "costas_shard_adopt: no such hypothesis");
     R.adopted = h;
     return cs_finish(ctx, R, h_state_out);

@@ -116,10 +116,16 @@ class ShardBuffer(object):
 
 
 def exchange_halo(ctx, hx, sb: ShardBuffer):
-    """rank r receives the last `halo_len` samples of rank r-1's shard (NCCL all-gather of the tails)"""
+    """rank r receives the last `halo_len` samples of rank r-1's shard (NCCL all-gather of the tails).  Every rank checks every
+    shard that supplies a halo against it before the NCCL collective, so a short shard raises ValueError on every rank alike."""
     h = sb.halo_len
-    assert sb.n >= h, "shard shorter than the halo"
-    tail = sb.shard[sb.n - h: sb.n]
+    shapes = hx.allgather((sb.n, h))
+    if any(hq != h for _, hq in shapes):
+        raise ValueError("exchange_halo: the ranks hold halos of %s samples; they must be equal" % sorted(set(hq for _, hq in shapes)))
+    for q, (nq, _) in enumerate(shapes[:-1]):
+        if nq < h:
+            raise ValueError("exchange_halo: shard %d (%d samples) is shorter than the %d-sample halo shard %d needs" % (q, nq, h, q + 1))
+    tail = sb.buf[sb.pad + sb.n - h: sb.pad + sb.n]   # the last rank's tail is sent but not used: it may reach into its halo
     allv = DeviceArray(ctx, (hx.world * h, 2), sb.dtype)
     ctx.check(ctx.lib.urh_nccl_allgather(ctx.handle, C.c_void_p(tail.ptr), C.c_void_p(allv.ptr), tail.nbytes))
     if hx.rank > 0:
@@ -149,14 +155,17 @@ def resolve_psk_chain(hyps):
 
 
 def afp_demod_psk_sharded(ctx, rank, world, sb: ShardBuffer, noise_mag, mod_order, costas_loop_bandwidth, d_out):
-    """PSK demodulation (Costas loop) of a capture sharded over the ranks, bit-identical to the serial loop.  Every rank
+    """PSK demodulation (Costas loop) of a capture sharded over the ranks, bit-identical to the serial loop (the run between the
+    library calls lives on ``ctx``).  Every rank
     speculates over its shard concurrently (the expensive pass) AND hops over it under each hypothesis "my shard starts in
     candidate h's start state" — what a locked loop of the preceding shard ends in, bit for bit.  One all-gather of
     (start, end) state pairs lets every rank pick its hypothesis (``resolve_psk_chain``); nothing waits for a neighbour.
     Only a shard whose predecessor ends in no hypothesis' start state (it begins inside a gap that carries a frozen or creeping
     loop state) falls back to the rank-to-rank hand-over from that shard on.  sb needs a halo of costas_halo() samples."""
     lib = ctx.lib
-    assert rank == 0 or sb.halo_len >= costas_halo(ctx)
+    if world > 1 and sb.halo_len < costas_halo(ctx):   # checked on rank 0 too, so every rank raises alike
+        raise ValueError("afp_demod_psk_sharded: the shard buffer's halo (%d samples) is shorter than the Costas warm-up (%d)"
+                         % (sb.halo_len, costas_halo(ctx)))
     ctx.check(lib.urh_costas_shard_speculate(ctx.handle, C.c_void_p(sb.shard.ptr), _lib.dtype_code(sb.dtype), sb.n, int(rank == 0),
                                              float(noise_mag), int(mod_order), float(costas_loop_bandwidth), C.c_void_p(d_out.ptr)))
     mine = np.zeros((4, 4), dtype=np.float32)
@@ -250,7 +259,8 @@ def center_protocol(rank, world, kept, window_stats, histogram, allgather_i64, a
 def detect_center_distributed(ctx, rank, world, sb: ShardBuffer, noise_mag, mod_type, d_qad, max_size=None):
     """afp_demod of the shard into ``d_qad`` + the capture-wide detect_center, every rank ending with the same center.
     Exchange (NCCL, a few hundred bytes + one histogram): kept-sample counts -> global rank window; per-rank window
-    partials {count, min, max, sum, sumsq} folded in rank order (deterministic) -> bin edges; histogram all-reduce."""
+    partials {count, min, max, sum, sumsq} folded in rank order (deterministic) -> bin edges; histogram all-reduce.
+    The bin width comes from Σ/Σ², not numpy's float32 variance: the reference's None-ness, center within one bin width (DESIGN §6)."""
     from .device import DeviceArray
     lib = ctx.lib
     code = _lib.demod_mod_code(mod_type)
@@ -340,28 +350,35 @@ def merge_shard_rows(parts):
 
 
 def detect_noise_level_sharded(ctx, hx, sb: ShardBuffer, global_offset, n_total):
-    """AutoInterpretation.detect_noise_level over the whole capture: per-rank partial (sum, max) of the 100 global,
-    end-aligned chunks, ONE NCCL all-reduce (sum half / max half share a buffer: max via sum of ... two calls), then
-    the reference's host logic."""
+    """AutoInterpretation.detect_noise_level over the whole capture from the 100 global, end-aligned chunks: every chunk is reduced
+    whole by the rank that holds its first sample, with the single-GPU slice partition, so every chunk sum is the single-GPU word at
+    any world size.  A chunk that a shard edge cuts is completed from the following shards first (``fetch_range``).  Two NCCL
+    all-reduces (sum, max) then add one owner's value to zeros; the reference's host logic decides."""
     from .ainterpretation import AutoInterpretation as AI
 
     if n_total <= 3:
         return 0
     chunksize, nchunks = AI._chunking(n_total)
-    # global chunk j covers [n_total-(j+1)*cs, n_total-j*cs); intersect with this shard
+    lo, hi = int(global_offset), int(global_offset) + sb.n
+    bounds = [(int(a), int(b)) for a, b in hx.allgather((lo, hi))]
+
+    def holder(i):
+        return next(q for q, (a, b) in enumerate(bounds) if a <= i < b)
+
     sums = np.zeros(nchunks, dtype=np.float64)
     maxs = np.full(nchunks, -1.0, dtype=np.float64)
-    lo, hi = int(global_offset), int(global_offset) + sb.n
     for j in range(nchunks):
+        # global chunk j covers [n_total-(j+1)*cs, n_total-j*cs)
         c0, c1 = n_total - (j + 1) * chunksize, n_total - j * chunksize
-        a, b = max(c0, lo), min(c1, hi)
-        if a >= b:
-            if c1 <= lo:
-                break
+        owner = holder(c0)
+        if c1 <= bounds[owner][1]:
+            part = sb.shard[c0 - lo: c1 - lo] if hx.rank == owner else None
+        else:
+            part = fetch_range(ctx, hx.rank, bounds, sb.shard, c0, c1, owner)   # collective: every rank takes this branch
+        if hx.rank != owner:
             continue
-        part = sb.shard[a - lo: b - lo]
         s1, m1 = np.zeros(1), np.zeros(1)
-        ctx.check(ctx.lib.urh_noise_chunk_stats_iq(ctx.handle, C.c_void_p(part.ptr), _lib.dtype_code(sb.dtype), b - a, b - a, 1,
+        ctx.check(ctx.lib.urh_noise_chunk_stats_iq(ctx.handle, C.c_void_p(part.ptr), _lib.dtype_code(sb.dtype), chunksize, chunksize, 1,
                                                    s1.ctypes.data_as(C.c_void_p), m1.ctypes.data_as(C.c_void_p)))
         sums[j], maxs[j] = s1[0], m1[0]
     d_s = DeviceArray(ctx, (nchunks,), np.float64).set(sums)
