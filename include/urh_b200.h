@@ -117,9 +117,9 @@ int urh_center_window_stats(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t
 int urh_center_window_var(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double* h_out2);
 int urh_center_histogram_tiles(urh_ctx* ctx, const float* d_qad, int64_t n, int64_t r0, int64_t r1, double hmin, double hstep,
                                int64_t nbins, int64_t* h_hist);
-/* replaces auto_interpretation.segment_messages_from_magnitudes (auto_interpretation.pyx:55-111) */
-int urh_segment_messages(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold,
-                         int64_t* h_segments, int64_t cap, int64_t* k);
+/* replaces auto_interpretation.segment_messages_from_magnitudes (auto_interpretation.pyx:55-111): *k = number of messages, fetched
+ * with urh_fetch_segments ((start, end) int64 pairs) */
+int urh_segment_messages(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold, int64_t* k);
 /* Sharded captures: urh_segment_shard_pass = the dense pass of one shard's magnitudes (then urh_shard_candidates with the run
  * carry of the preceding shards and urh_fetch_candidates); urh_segments_from_runs = the state machine of
  * auto_interpretation.pyx:69-111 over the concatenated run table of all shards (pure host code). */

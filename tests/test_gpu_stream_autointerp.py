@@ -170,7 +170,7 @@ def test_segment_shim_streams_once_past_the_first_buffer(ctx, monkeypatch):
     from urh_b200.ainterpretation import AutoInterpretation as AI
     from urh_b200.cythonext import signal_functions as sf
 
-    nmsg = (1 << 16) + 5   # more messages than the resident shim's first buffer holds
+    nmsg = (1 << 16) + 5   # more messages than a 2^16-pair buffer holds
     levels = np.tile(runs((10, 1), (10, 0)), nmsg)
     iq = from_levels(levels, np.float32, np.random.default_rng(3))
     ref = seg_resident(ctx, iq, 0.5)

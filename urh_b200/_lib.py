@@ -96,7 +96,7 @@ SIGNATURES = {
     "urh_center_window_stats": (i32, [vp, vp, i64, i64, i64, vp]),
     "urh_center_window_var": (i32, [vp, vp, i64, i64, i64, vp]),
     "urh_center_histogram_tiles": (i32, [vp, vp, i64, i64, i64, C.c_double, C.c_double, i64, vp]),
-    "urh_segment_messages": (i32, [vp, vp, i32, i64, f32, vp, i64, C.POINTER(i64)]),
+    "urh_segment_messages": (i32, [vp, vp, i32, i64, f32, C.POINTER(i64)]),
     "urh_plateau_lengths": (i32, [vp, vp, i64, f32, i32, vp, i64, C.POINTER(i64)]),
     "urh_median_filter": (i32, [vp, vp, i64, C.c_uint, vp]),
     "urh_arr2decibel": (i32, [vp, vp, i64, vp]),

@@ -54,11 +54,7 @@ struct urh_ctx {
     // twiddles of the last window size urh_spectrogram_bgra ran with (spectrogram.cu; 4096 entries allocated)
     void* img_tw;
     int img_tw_n;
-    // sharded segmenter state between urh_segment_shard_pass and urh_shard_candidates / urh_fetch_candidates (arena memory)
-    void* shard_tiles;
-    void* shard_staging;
-    int shard_cap, shard_tol;
-    int64_t shard_n;
+    // sharded segmenter state between urh_segment_shard_pass and urh_shard_candidates / urh_fetch_candidates (stats.cu)
     void* shard_state;
     // NCCL (nccl.cu)
     int64_t costas_stats[3];
@@ -96,7 +92,7 @@ struct urh_ctx {
     int64_t stream_free_low, stream_chunks;
     size_t arena_live;   // bytes of the arena requests live since the last reset (released ones not counted)
     size_t arena_peak;   // the most arena_live reached since the last reset
-    // (start, end) pairs of the last urh_segment_messages_iq_stream call (urh_fetch_segments)
+    // (start, end) pairs of the last urh_segment_messages(_iq_stream) call (urh_fetch_segments)
     std::vector<int64_t> segments;
 };
 

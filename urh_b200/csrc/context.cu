@@ -28,8 +28,6 @@ extern "C" int urh_ctx_create(int device, urh_ctx** out) {
     ctx->h_stage[0] = ctx->h_stage[1] = nullptr;
     ctx->h_stage_bytes = 0;
     ctx->fft_valid = false;
-    ctx->shard_tiles = nullptr;
-    ctx->shard_staging = nullptr;
     ctx->shard_state = nullptr;
     ctx->costas_shard = nullptr;
     ctx->bits_valid = 0;

@@ -566,9 +566,10 @@ static StreamSizes stream_sizes(int64_t n, int dtype, int tol, int64_t chunk_sam
     return z;
 }
 
-// Message segmentation from IQ (stats.cu urh_segment_messages_iq_stream): the arena of one pass of the sharded segmenter over `tiles`
-// tiles of float64 magnitudes (urh_segment_shard_pass: tile table, staging, closing-run total; urh_shard_candidates: heads, offsets,
-// counts, the candidates, at most one per 10 samples).  Its scans use the look-back workspace (scan_workspace_bytes), not the arena.
+// Message segmentation (stats.cu urh_segment_messages, urh_segment_messages_iq_stream): the arena of one segmenter pass over `tiles`
+// tiles of magnitudes (the run table: tile table, staging; the candidate collector: heads, offsets, counts, closing run, the
+// candidates, at most one per 10 samples), with a second closing-run slot to spare.  Its scans use the look-back workspace
+// (scan_workspace_bytes), not the arena.
 static int64_t segment_arena_bytes(int64_t tiles) {
     const int64_t cap = URH_TILE / 10 + 2, cand = tiles * URH_TILE / 10 + 3;
     return r256(tiles * (int64_t)sizeof(UrhTileSummary)) + r256(tiles * cap * 4) + 2 * r256(2 * (int64_t)sizeof(RunCarry)) +
@@ -1194,56 +1195,6 @@ extern "C" int urh_demod_digitize_psk_stream(urh_ctx* ctx, const void* h_iq, int
                          contiguous_download(ctx, (const char*)d_qad, z.cs * 4, (char*)h_qad_out, 4), place_after_pad));
     *k = sd.rows;
     return urh_costas_stream_end(ctx, &cs);
-}
-
-// ---- sharded message segmentation (SURVEY 8e) -----------------------------------------------------------------------------------
-// urh_segment_shard_pass (stats.cu) leaves its shard's tile table in the context; once the ranks have exchanged their closing runs,
-// urh_shard_candidates turns it into the shard's candidate table with global positions and urh_fetch_candidates copies that to the
-// host.
-struct UrhShardState {
-    UrhCandidates cand;
-};
-static UrhShardState* shard_state(urh_ctx* ctx) {
-    if (!ctx->shard_state) ctx->shard_state = calloc(1, sizeof(UrhShardState));
-    return (UrhShardState*)ctx->shard_state;
-}
-
-// After the summaries were exchanged: carry_* describe the run that ends right before this shard (fold of the preceding shards'
-// summaries; carry_valid = 0 on the first shard).  Positions are global.
-// *last_cand_cls = class of the shard's last candidate (meaningful when *count > 0).
-extern "C" int urh_shard_candidates(urh_ctx* ctx, int carry_valid, int carry_cls, int64_t carry_len, int64_t global_offset,
-                                    int64_t* count, const int64_t** d_pos, const int16_t** d_cls, int* last_cand_cls) {
-    if (!ctx->shard_tiles) URH_FAIL(ctx, URH_ERR_INVALID, "urh_segment_shard_pass must precede urh_shard_candidates");
-    UrhShardCarry in;
-    in.valid = carry_valid; in.cls = carry_cls; in.len = carry_len;
-    UrhShardState* S = shard_state(ctx);
-    URH_CHECK(urh_collect_candidates_shard(ctx, ctx->shard_n, ctx->shard_tol, (const UrhTileSummary*)ctx->shard_tiles,
-                                           (const uint32_t*)ctx->shard_staging, ctx->shard_cap, in, global_offset, &S->cand));
-    *count = S->cand.count;
-    if (d_pos) *d_pos = S->cand.pos;
-    if (d_cls) *d_cls = S->cand.cls;
-    if (last_cand_cls) {
-        *last_cand_cls = 0;
-        if (S->cand.count > 0) {
-            int16_t v = 0;
-            URH_CUDA(ctx, cudaMemcpyAsync(&v, S->cand.cls + S->cand.count - 1, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
-            URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-            *last_cand_cls = v;
-        }
-    }
-    ctx->shard_tiles = nullptr;
-    return URH_OK;
-}
-
-// host copies of the candidate table urh_shard_candidates left on the device
-extern "C" int urh_fetch_candidates(urh_ctx* ctx, int64_t* h_pos, int16_t* h_cls, int64_t count) {
-    UrhShardState* S = shard_state(ctx);
-    if (count < 0 || count > S->cand.count) URH_FAIL(ctx, URH_ERR_INVALID, "fetch_candidates: count exceeds the table");
-    if (count == 0) return URH_OK;
-    URH_CUDA(ctx, cudaMemcpyAsync(h_pos, S->cand.pos, (size_t)count * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaMemcpyAsync(h_cls, S->cand.cls, (size_t)count * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
-    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return URH_OK;
 }
 
 extern "C" int urh_fetch_pulses(urh_ctx* ctx, int64_t* h_rows, int64_t k) {

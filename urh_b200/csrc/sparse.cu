@@ -86,15 +86,9 @@ int urh_shard_run_total(urh_ctx* ctx, int64_t n, const UrhTileSummary* tiles, in
     return URH_OK;
 }
 
-int urh_collect_candidates(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummary* tiles, const uint32_t* staging,
-                           int stage_cap, UrhCandidates* out) {
-    UrhShardCarry none;
-    none.valid = 0; none.cls = 0; none.len = 0;
-    return urh_collect_candidates_shard(ctx, n, tol, tiles, staging, stage_cap, none, 0, out);
-}
-
-int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummary* tiles, const uint32_t* staging,
-                                 int stage_cap, UrhShardCarry carry_in, int64_t global_offset, UrhCandidates* out) {
+int urh_collect_candidates_shard(urh_ctx* ctx, const UrhRunTable& rt, UrhShardCarry carry_in, int64_t global_offset, UrhCandidates* out) {
+    const int64_t n = rt.n;
+    const UrhTileSummary* tiles = rt.tiles;
     const int64_t ntiles = urh_div_up(n, URH_TILE);
     int32_t* head_rel;
     int64_t* offset;
@@ -105,7 +99,7 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
     URH_CHECK(urh_arena(ctx, 4, &d_count));
     URH_CHECK(urh_arena(ctx, 2, &d_total_run));
     RunHeads fh;
-    fh.tiles = tiles; fh.n = n; fh.tol = tol; fh.head_rel = head_rel;
+    fh.tiles = tiles; fh.n = n; fh.tol = rt.tol; fh.head_rel = head_rel;
     fh.has_in = carry_in.valid ? 1 : 0;
     fh.in.len = carry_in.len; fh.in.cls = carry_in.cls; fh.in.flags = 0;
     // the total is the shard's own closing run, without the carry of the preceding shards
@@ -122,6 +116,7 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
         memcpy(&tr, raw, sizeof(tr));
         out->last_cls = tr.cls;
         out->last_len = tr.len;
+        out->whole = (tr.flags & 1) ? 1 : 0;
     }
     out->count = C;
     out->pos = nullptr;
@@ -130,6 +125,6 @@ int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTile
     URH_CHECK(urh_arena(ctx, (size_t)C, &out->pos));
     URH_CHECK(urh_arena(ctx, (size_t)C, &out->cls));
     const unsigned gg = (unsigned)urh_div_up(ntiles * 32, 256);
-    URH_LAUNCH(ctx, k_gather, gg, 256, 0, tiles, staging, stage_cap, head_rel, offset, ntiles, global_offset, out->pos, out->cls);
+    URH_LAUNCH(ctx, k_gather, gg, 256, 0, tiles, rt.staging, rt.cap, head_rel, offset, ntiles, global_offset, out->pos, out->cls);
     return URH_OK;
 }

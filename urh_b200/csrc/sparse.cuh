@@ -107,30 +107,35 @@ struct FinishShard {
 // The pulse table of the tiles dz's dense pass filled (finish.cu).  *k = the rows this finish added.
 int finish_tiles(urh_ctx* ctx, const UrhDigitizer& dz, const FinishShard& sh, int64_t* k);
 
+// The tile table of a dense pass with a binary classifier over n samples (the segmenter, the plateau RLE; stats.cu)
+struct UrhRunTable {
+    int64_t n;
+    int tol, cap;             // tolerance; staged candidates per tile
+    UrhTileSummary* tiles;
+    uint32_t* staging;
+};
+
 struct UrhCandidates {
     int64_t count;   // number of candidates (host copy)
     int64_t* pos;    // device: absolute sample index run_start + tolerance
     int16_t* cls;    // device: class of the run
-    // the run that contains the LAST sample of the stream (host copies): class and length
+    // the run that contains the LAST sample of the table, without the carry (host copies): class, length, 1 if it is the whole table
     int32_t last_cls;
     int64_t last_len;
+    int whole;
 };
 
-// Stitch runs across tile edges (scan over the tile table), add the per-tile head candidates and gather
-// everything into `out` (arena memory).  Synchronises once to learn the candidate count.
-int urh_collect_candidates(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummary* tiles, const uint32_t* staging,
-                           int stage_cap, UrhCandidates* out);
-
-// Sharded captures: the run that ends at the end of the PRECEDING shards (class, length); valid = 0 for the first shard.
+// The run that ends at the end of the PRECEDING shards or chunks (class, length); valid = 0 for the first one.
 struct UrhShardCarry {
     int valid;
     int cls;
     int64_t len;
 };
-// As urh_collect_candidates, with the carry of the preceding shards folded in and positions offset by
-// `global_offset` (the shard's first sample index in the whole capture).
-int urh_collect_candidates_shard(urh_ctx* ctx, int64_t n, int tol, const UrhTileSummary* tiles, const uint32_t* staging,
-                                 int stage_cap, UrhShardCarry carry_in, int64_t global_offset, UrhCandidates* out);
-// The shard's own run summary for the exchange: h_out = {last_cls, last_len, whole (1 if the shard is one run)}.
+// Stitch runs across tile edges (scan over the tile table) from the carry, add the per-tile head candidates and gather everything
+// into `out` (arena memory), positions offset by `global_offset` (the table's first sample index in the whole capture).
+// Synchronises once to learn the candidate count.
+int urh_collect_candidates_shard(urh_ctx* ctx, const UrhRunTable& rt, UrhShardCarry carry_in, int64_t global_offset, UrhCandidates* out);
+// The shard's own run summary for the exchange before its candidates are collected: h_out = {last_cls, last_len, whole (1 if the
+// shard is one run)}.
 int urh_shard_run_total(urh_ctx* ctx, int64_t n, const UrhTileSummary* tiles, int64_t* h_out);
 

@@ -214,43 +214,67 @@ extern "C" int urh_noise_chunk_stats(urh_ctx* ctx, const void* d_mags, int is_f6
 }
 
 // ---- run tables for the segmenter and the plateau RLE ----------------------------------------------------------------
-// mode 0: class = x > thr (segment_messages, tolerance 9 <=> 10 consecutive samples, auto_interpretation.pyx:69)
-// mode 1: class = x <= thr ? 0 : 1 (get_plateau_lengths, tolerance 0: every run start)
-// Candidates (position, class) are returned to the host (they are few); *h_last = {last_cls, last_len, first_cls}.
+// SrcAbove: class = x > thr (segment_messages, tolerance 9 <=> 10 consecutive samples, auto_interpretation.pyx:69)
+// SrcCenter: class = x <= thr ? 0 : 1 (get_plateau_lengths, tolerance 0: every run start)
+// The dense pass of one call or chunk, its tables the first of a fresh arena.  first_above != NULL: *first_above = sample 0 > thr,
+// compared in T (double for float64 magnitudes); it is read before the pass is enqueued, so the wait covers only earlier work.
 template <typename SRC, typename T>
-static int run_table(urh_ctx* ctx, const T* d_x, int64_t n, float thr, int tol, int64_t** h_pos, int16_t** h_cls,
-                     int64_t* count, int64_t* h_last) {
+static int run_table(urh_ctx* ctx, const T* d_x, int64_t n, float thr, int tol, UrhRunTable* rt, int* first_above) {
     urh_arena_reset(ctx);
+    if (first_above) {
+        T x0;
+        URH_CUDA(ctx, cudaMemcpyAsync(&x0, d_x, sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        *first_above = (x0 > (T)thr) ? 1 : 0;
+    }
     UrhClassify cls;
     memset(&cls, 0, sizeof(cls));
     cls.noise_value = 0.0f;
     cls.order = 2;
     cls.thr[0] = thr;
     const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = URH_TILE / (tol + 1) + 2;
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
+    rt->n = n;
+    rt->tol = tol;
+    rt->cap = stage_cap_for(tol);
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &rt->tiles));
+    URH_CHECK(urh_arena(ctx, (size_t)ntiles * rt->cap, &rt->staging));
     const unsigned grid = (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
     const int vec_in = (((uintptr_t)d_x % (2 * sizeof(T))) == 0) ? 1 : 0;
-    URH_LAUNCH(ctx, (k_dense_f32<SRC, T>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_x, n, vec_in, cls, tol, tiles, staging, cap,
+    URH_LAUNCH(ctx, (k_dense_f32<SRC, T>), grid, URH_WARPS_PER_BLOCK * 32, 0, d_x, n, vec_in, cls, tol, rt->tiles, rt->staging, rt->cap,
                (int16_t*)nullptr, 0);
-    UrhCandidates cand;
-    URH_CHECK(urh_collect_candidates(ctx, n, tol, tiles, staging, cap, &cand));
-    *count = cand.count;
-    h_last[0] = cand.last_cls;
-    h_last[1] = cand.last_len;
-    *h_pos = nullptr;
-    *h_cls = nullptr;
-    if (cand.count > 0) {
-        *h_pos = (int64_t*)malloc((size_t)cand.count * sizeof(int64_t));
-        *h_cls = (int16_t*)malloc((size_t)cand.count * sizeof(int16_t));
-        URH_CUDA(ctx, cudaMemcpyAsync(*h_pos, cand.pos, (size_t)cand.count * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CUDA(ctx, cudaMemcpyAsync(*h_cls, cand.cls, (size_t)cand.count * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
     return URH_OK;
+}
+
+// candidates [0, count) of c in host memory (synchronises)
+static int candidates_to_host(urh_ctx* ctx, const UrhCandidates& c, int64_t count, int64_t* h_pos, int16_t* h_cls) {
+    if (count == 0) return URH_OK;
+    URH_CUDA(ctx, cudaMemcpyAsync(h_pos, c.pos, (size_t)count * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaMemcpyAsync(h_cls, c.cls, (size_t)count * sizeof(int16_t), cudaMemcpyDeviceToHost, ctx->stream));
+    URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return URH_OK;
+}
+
+// urh_collect_candidates_shard with the candidates appended to host lists (they are few); *c keeps the table's closing run
+static int collect_on_host(urh_ctx* ctx, const UrhRunTable& rt, UrhShardCarry carry, int64_t global_offset, UrhCandidates* c,
+                           std::vector<int64_t>& pos, std::vector<int16_t>& cls) {
+    URH_CHECK(urh_collect_candidates_shard(ctx, rt, carry, global_offset, c));
+    const size_t at = pos.size();
+    pos.resize(at + (size_t)c->count);
+    cls.resize(at + (size_t)c->count);
+    return candidates_to_host(ctx, *c, c->count, pos.data() + at, cls.data() + at);
+}
+
+// The run that ends after a piece (chunk or shard) of a capture: the piece's closing run, extended by the carry (the run that ends
+// right before the piece) if the piece is one whole run of the carry's class.  dist.py fold_closing_run is the same rule.
+static UrhShardCarry fold_closing_run(UrhShardCarry carry, const UrhCandidates& piece) {
+    if (carry.valid && piece.whole && piece.last_cls == carry.cls) {
+        carry.len += piece.last_len;
+    } else {
+        carry.cls = piece.last_cls;
+        carry.len = piece.last_len;
+    }
+    carry.valid = 1;
+    return carry;
 }
 
 // The two-state machine of segment_messages_from_magnitudes over the run table (host; the runs of >= 10 samples are few):
@@ -284,82 +308,39 @@ extern "C" int urh_segments_from_runs(const int64_t* h_pos, const int16_t* h_cls
     return URH_OK;
 }
 
-// One shard of a capture whose magnitudes are spread over the ranks: the dense pass (class = above the threshold, tolerance 9)
-// leaves the tile table for urh_shard_candidates (carry of the preceding shards, global positions).
-// h_summary = {last_cls, last_len, whole, class of the shard's first sample}.
-extern "C" int urh_segment_shard_pass(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold, int64_t* h_summary) {
-    if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "empty shard");
-    urh_arena_reset(ctx);
-    UrhClassify cls;
-    memset(&cls, 0, sizeof(cls));
-    cls.noise_value = 0.0f;
-    cls.order = 2;
-    cls.thr[0] = noise_threshold;
-    const int tol = 9;
-    const int64_t ntiles = urh_div_up(n, URH_TILE);
-    const int cap = URH_TILE / (tol + 1) + 2;
-    UrhTileSummary* tiles;
-    uint32_t* staging;
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles, &tiles));
-    URH_CHECK(urh_arena(ctx, (size_t)ntiles * cap, &staging));
-    const unsigned grid = (unsigned)urh_div_up(ntiles, URH_WARPS_PER_BLOCK);
-    double f0 = 0.0;
-    if (is_f64) {
-        const int vec_in = (((uintptr_t)d_mags % 16) == 0) ? 1 : 0;
-        URH_LAUNCH(ctx, (k_dense_f32<SrcAbove, double>), grid, URH_WARPS_PER_BLOCK * 32, 0, (const double*)d_mags, n, vec_in, cls, tol, tiles,
-                   staging, cap, (int16_t*)nullptr, 0);
-        URH_CUDA(ctx, cudaMemcpyAsync(&f0, d_mags, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    } else {
-        const int vec_in = (((uintptr_t)d_mags % 8) == 0) ? 1 : 0;
-        URH_LAUNCH(ctx, (k_dense_f32<SrcAbove, float>), grid, URH_WARPS_PER_BLOCK * 32, 0, (const float*)d_mags, n, vec_in, cls, tol, tiles,
-                   staging, cap, (int16_t*)nullptr, 0);
-        float f32 = 0.f;
-        URH_CUDA(ctx, cudaMemcpyAsync(&f32, d_mags, sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        f0 = (double)f32;
-    }
-    ctx->shard_tiles = tiles;
-    ctx->shard_staging = staging;
-    ctx->shard_cap = cap;
-    ctx->shard_n = n;
-    ctx->shard_tol = tol;
-    URH_CHECK(urh_shard_run_total(ctx, n, tiles, h_summary));   // synchronises
-    h_summary[3] = (is_f64 ? (f0 > (double)noise_threshold) : ((float)f0 > noise_threshold)) ? 1 : 0;
+// the segments of a capture of n samples from all its candidates into the context (urh_fetch_segments); last = the run that ends it
+static int segments_to_ctx(urh_ctx* ctx, const std::vector<int64_t>& pos, const std::vector<int16_t>& cls, int first_above,
+                           UrhShardCarry last, int64_t n, int64_t* k) {
+    const int64_t cap = (int64_t)pos.size() + 1;   // a message starts at sample 0 or at a candidate
+    ctx->segments.resize((size_t)(2 * cap));
+    URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, last.cls, last.len, n, ctx->segments.data(),
+                                     cap, k));
+    ctx->segments.resize((size_t)(2 * *k));
     return URH_OK;
 }
 
-// segment_messages_from_magnitudes (auto_interpretation.pyx:55-111).  d_mags float32 (is_f64=0) or float64.
-// h_segments receives (start, end) pairs, capacity `cap` pairs; *k = number of messages (may exceed cap: call again).
-extern "C" int urh_segment_messages(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold,
-                                    int64_t* h_segments, int64_t cap, int64_t* k) {
+// segment_messages_from_magnitudes (auto_interpretation.pyx:55-111).  d_mags float32 (is_f64=0) or float64.  *k = number of
+// messages; their (start, end) pairs stay in the context for urh_fetch_segments.
+extern "C" int urh_segment_messages(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold, int64_t* k) {
     *k = 0;
+    ctx->segments.clear();
     if (n <= 0) return URH_OK;
-    int64_t* pos = nullptr;
-    int16_t* cl = nullptr;
-    int64_t count = 0, last[2];
-    float first = 0.f;
-    if (is_f64) {
-        double f0;
-        URH_CUDA(ctx, cudaMemcpyAsync(&f0, d_mags, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CHECK((run_table<SrcAbove, double>(ctx, (const double*)d_mags, n, noise_threshold, 9, &pos, &cl, &count, last)));
-        first = (f0 > (double)noise_threshold) ? 1.f : 0.f;
-    } else {
-        float f0;
-        URH_CUDA(ctx, cudaMemcpyAsync(&f0, d_mags, sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-        URH_CHECK((run_table<SrcAbove, float>(ctx, (const float*)d_mags, n, noise_threshold, 9, &pos, &cl, &count, last)));
-        first = (f0 > noise_threshold) ? 1.f : 0.f;
-    }
-    const int rc = urh_segments_from_runs(pos, cl, count, first > 0.f ? 1 : 0, (int)last[0], last[1], n, h_segments, cap, k);
-    free(pos);
-    free(cl);
-    return rc;
+    UrhRunTable rt;
+    int first_above = 0;
+    URH_CHECK((is_f64 ? run_table<SrcAbove, double>(ctx, (const double*)d_mags, n, noise_threshold, 9, &rt, &first_above)
+                      : run_table<SrcAbove, float>(ctx, (const float*)d_mags, n, noise_threshold, 9, &rt, &first_above)));
+    UrhCandidates cand;
+    std::vector<int64_t> pos;
+    std::vector<int16_t> cls;
+    URH_CHECK(collect_on_host(ctx, rt, UrhShardCarry{}, 0, &cand, pos, cls));
+    return segments_to_ctx(ctx, pos, cls, first_above, fold_closing_run(UrhShardCarry{}, cand), n, k);
 }
 
 // segment_messages_from_magnitudes(get_magnitudes(iq)) of a host capture of any size (stream_run: chunks of whole tiles).  Each chunk's
-// float64 magnitudes go into a scratch of one chunk, the sharded segmenter's dense pass runs over them, and urh_shard_candidates gives
-// its candidates with global positions from the run that ends right before the chunk (dist.py fold_carry's rule, folded here).  The
-// two-state machine then runs once over all candidates; the segments stay in the context for urh_fetch_segments, so a caller never
-// streams the capture twice to size its buffer.
+// float64 magnitudes go into a scratch of one chunk; the run-table pass over them and the candidate collector, continued from the
+// run that ends right before the chunk and offset to global positions, append the chunk's candidates.  The two-state machine then
+// runs once over all candidates; the segments stay in the context for urh_fetch_segments, so a caller never streams the capture
+// twice to size its buffer.
 extern "C" int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, float noise_threshold,
                                               int64_t chunk_samples, int ring, int64_t* k) {
     if (!h_iq || !k) URH_FAIL(ctx, URH_ERR_INVALID, "segment_messages_iq_stream: bad arguments");
@@ -375,49 +356,86 @@ extern "C" int urh_segment_messages_iq_stream(urh_ctx* ctx, const void* h_iq, in
     std::vector<int64_t> pos;
     std::vector<int16_t> cls;
     int first_above = 0;
-    bool carry_valid = false;
-    int carry_cls = 0;
-    int64_t carry_len = 0;
+    UrhShardCarry carry{};   // the run that ends right before the chunk
     std::vector<UrhWindow> win;
     URH_CHECK(urh_filter_windows(URH_FILTER_TILES, n, n, 0, 0, chunk_samples, nullptr, nullptr, 0, win));
     URH_CHECK(stream_run(ctx, win, R, (const char*)h_iq, urh_iq_bytes(dtype), R.mem, z.src_slot, false,
                          [&](int64_t c, const UrhWindow& w, int s) {
                              URH_CHECK(urh_get_magnitudes(ctx, R.mem + s * z.src_slot + URH_STREAM_PAD, dtype, w.k1 - w.k0, d_mag));
-                             int64_t summary[4];
-                             URH_CHECK(urh_segment_shard_pass(ctx, d_mag, 1, w.k1 - w.k0, noise_threshold, summary));
-                             if (c == 0) first_above = (int)summary[3];
-                             int64_t count = 0;
-                             URH_CHECK(urh_shard_candidates(ctx, carry_valid ? 1 : 0, carry_cls, carry_len, w.k0, &count, nullptr, nullptr,
-                                                            nullptr));
-                             const size_t at = pos.size();
-                             pos.resize(at + (size_t)count);
-                             cls.resize(at + (size_t)count);
-                             URH_CHECK(urh_fetch_candidates(ctx, pos.data() + at, cls.data() + at, count));
-                             // the run that ends after this chunk: this chunk's closing run, continued from the carry if the chunk is one run
-                             if (carry_valid && summary[2] && summary[0] == carry_cls) {
-                                 carry_len += summary[1];
-                             } else {
-                                 carry_cls = (int)summary[0];
-                                 carry_len = summary[1];
-                             }
-                             carry_valid = true;
+                             UrhRunTable rt;
+                             URH_CHECK((run_table<SrcAbove, double>(ctx, d_mag, w.k1 - w.k0, noise_threshold, 9, &rt,
+                                                                    c == 0 ? &first_above : nullptr)));
+                             UrhCandidates cand;
+                             URH_CHECK(collect_on_host(ctx, rt, carry, w.k0, &cand, pos, cls));
+                             carry = fold_closing_run(carry, cand);
                              return URH_OK;
                          },
                          no_download, place_after_pad));
-    int64_t m = 0;
-    URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, carry_cls, carry_len, n, nullptr, 0, &m));
-    ctx->segments.resize((size_t)(2 * m));
-    URH_CHECK(urh_segments_from_runs(pos.data(), cls.data(), (int64_t)pos.size(), first_above, carry_cls, carry_len, n, ctx->segments.data(),
-                                     m, &m));
-    *k = m;
-    return URH_OK;
+    return segments_to_ctx(ctx, pos, cls, first_above, carry, n, k);
 }
 
-// the segments of the last urh_segment_messages_iq_stream call: (start, end) pairs
+// the segments of the last urh_segment_messages or urh_segment_messages_iq_stream call: (start, end) pairs
 extern "C" int urh_fetch_segments(urh_ctx* ctx, int64_t* h_segments, int64_t k) {
     if (k < 0 || 2 * k > (int64_t)ctx->segments.size()) URH_FAIL(ctx, URH_ERR_INVALID, "fetch_segments: k exceeds the last result");
     if (k > 0) memcpy(h_segments, ctx->segments.data(), (size_t)(2 * k) * sizeof(int64_t));
     return URH_OK;
+}
+
+// ---- sharded message segmentation (SURVEY 8e) -----------------------------------------------------------------------------------
+// urh_segment_shard_pass leaves its shard's tile table in the context; once the ranks have exchanged their closing runs,
+// urh_shard_candidates turns it into the shard's candidate table with global positions and urh_fetch_candidates copies that to the
+// host.  Both tables are arena memory; rt.tiles is NULL when no pass is pending.
+struct UrhShardState {
+    UrhRunTable rt;
+    UrhCandidates cand;
+};
+static UrhShardState* shard_state(urh_ctx* ctx) {
+    if (!ctx->shard_state) ctx->shard_state = calloc(1, sizeof(UrhShardState));
+    return (UrhShardState*)ctx->shard_state;
+}
+
+// One shard of a capture whose magnitudes are spread over the ranks: the dense pass (class = above the threshold, tolerance 9).
+// h_summary = {last_cls, last_len, whole, class of the shard's first sample}.
+extern "C" int urh_segment_shard_pass(urh_ctx* ctx, const void* d_mags, int is_f64, int64_t n, float noise_threshold, int64_t* h_summary) {
+    if (n <= 0) URH_FAIL(ctx, URH_ERR_INVALID, "empty shard");
+    UrhShardState* S = shard_state(ctx);
+    int first_above = 0;
+    URH_CHECK((is_f64 ? run_table<SrcAbove, double>(ctx, (const double*)d_mags, n, noise_threshold, 9, &S->rt, &first_above)
+                      : run_table<SrcAbove, float>(ctx, (const float*)d_mags, n, noise_threshold, 9, &S->rt, &first_above)));
+    URH_CHECK(urh_shard_run_total(ctx, n, S->rt.tiles, h_summary));   // synchronises
+    h_summary[3] = first_above;
+    return URH_OK;
+}
+
+// After the summaries were exchanged: carry_* describe the run that ends right before this shard (fold of the preceding shards'
+// summaries; carry_valid = 0 on the first shard).  Positions are global.
+// *last_cand_cls = class of the shard's last candidate (meaningful when *count > 0).
+extern "C" int urh_shard_candidates(urh_ctx* ctx, int carry_valid, int carry_cls, int64_t carry_len, int64_t global_offset,
+                                    int64_t* count, const int64_t** d_pos, const int16_t** d_cls, int* last_cand_cls) {
+    UrhShardState* S = shard_state(ctx);
+    if (!S->rt.tiles) URH_FAIL(ctx, URH_ERR_INVALID, "urh_segment_shard_pass must precede urh_shard_candidates");
+    URH_CHECK(urh_collect_candidates_shard(ctx, S->rt, UrhShardCarry{carry_valid, carry_cls, carry_len}, global_offset, &S->cand));
+    *count = S->cand.count;
+    if (d_pos) *d_pos = S->cand.pos;
+    if (d_cls) *d_cls = S->cand.cls;
+    if (last_cand_cls) {
+        *last_cand_cls = 0;
+        if (S->cand.count > 0) {
+            int16_t v = 0;
+            URH_CUDA(ctx, cudaMemcpyAsync(&v, S->cand.cls + S->cand.count - 1, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+            URH_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+            *last_cand_cls = v;
+        }
+    }
+    S->rt.tiles = nullptr;
+    return URH_OK;
+}
+
+// host copies of the candidate table urh_shard_candidates left on the device
+extern "C" int urh_fetch_candidates(urh_ctx* ctx, int64_t* h_pos, int16_t* h_cls, int64_t count) {
+    UrhShardState* S = shard_state(ctx);
+    if (count < 0 || count > S->cand.count) URH_FAIL(ctx, URH_ERR_INVALID, "fetch_candidates: count exceeds the table");
+    return candidates_to_host(ctx, S->cand, count, h_pos, h_cls);
 }
 
 // get_plateau_lengths (auto_interpretation.pyx:179-208): h_out capacity `cap`; *k = number of plateaus.
@@ -425,15 +443,17 @@ extern "C" int urh_plateau_lengths(urh_ctx* ctx, const float* d_rect, int64_t n,
                                    uint64_t* h_out, int64_t cap, int64_t* k) {
     *k = 0;
     if (n <= 0) return URH_OK;
-    int64_t* pos = nullptr;
-    int16_t* cl = nullptr;
-    int64_t count = 0, last[2];
-    URH_CHECK((run_table<SrcCenter, float>(ctx, d_rect, n, center, 0, &pos, &cl, &count, last)));
+    UrhRunTable rt;
+    URH_CHECK((run_table<SrcCenter, float>(ctx, d_rect, n, center, 0, &rt, nullptr)));
+    UrhCandidates cand;
+    std::vector<int64_t> pos;
+    std::vector<int16_t> cls;
+    URH_CHECK(collect_on_host(ctx, rt, UrhShardCarry{}, 0, &cand, pos, cls));
     // candidates with tolerance 0 are the run starts (the first one is position 0)
     const uint64_t limit = (uint64_t)percentage * (uint64_t)n / 100;
     uint64_t sum = 0;
     int64_t m = 0;
-    for (int64_t j = 1; j < count; j++) {
+    for (size_t j = 1; j < pos.size(); j++) {
         // the reference checks `current_sum >= limit` at the top of every sample iteration, i.e. before a
         // boundary at pos[j] can append the run that ends there
         if (sum >= limit) break;
@@ -443,8 +463,6 @@ extern "C" int urh_plateau_lengths(urh_ctx* ctx, const float* d_rect, int64_t n,
         sum += len;
     }
     if (limit == 0) m = 0;
-    free(pos);
-    free(cl);
     *k = m;
     return URH_OK;
 }

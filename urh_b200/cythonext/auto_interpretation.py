@@ -19,15 +19,12 @@ def segment_messages_from_magnitudes(magnitudes, noise_threshold: float) -> list
         return []
     ctx = magnitudes.ctx if on_device else _lib.default_context()
     d = magnitudes if on_device else to_device(magnitudes, ctx)
-    cap = 1 << 16
-    while True:
-        seg = np.empty((cap, 2), dtype=np.int64)
-        k = C.c_int64(0)
-        ctx.check(ctx.lib.urh_segment_messages(ctx.handle, C.c_void_p(d.ptr), int(d.dtype == np.float64), n,
-                                               float(noise_threshold), seg.ctypes.data_as(C.c_void_p), cap, C.byref(k)))
-        if k.value <= cap:
-            return [(int(a), int(b)) for a, b in seg[: k.value]]
-        cap = k.value
+    k = C.c_int64(0)
+    ctx.check(ctx.lib.urh_segment_messages(ctx.handle, C.c_void_p(d.ptr), int(d.dtype == np.float64), n, float(noise_threshold),
+                                           C.byref(k)))
+    seg = np.empty((k.value, 2), dtype=np.int64)
+    ctx.check(ctx.lib.urh_fetch_segments(ctx.handle, seg.ctypes.data_as(C.c_void_p), k.value))
+    return [(int(a), int(b)) for a, b in seg]
 
 
 def get_plateau_lengths(rect_data, center, percentage: int = 25) -> np.ndarray:

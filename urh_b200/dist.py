@@ -23,17 +23,23 @@ from .device import DeviceArray, to_device
 
 
 # ---- pure host logic (unit-tested on CPU with gloo, tests/test_dist_cpu.py) -----------------------------------------
+def fold_closing_run(carry, cls, length, whole):
+    """The run (cls, len) that ends after a shard whose closing run is (cls, length): extended by `carry`, the run that ends right
+    before the shard (None for the first), if the shard is one whole run of the carry's class.  The streamed segmenter (stats.cu)
+    folds its chunks by the same rule."""
+    if carry is not None and whole and cls == carry[0]:
+        return (cls, carry[1] + length)
+    return (cls, length)
+
+
 def fold_carry(summaries):
     """summaries: list of (last_cls, last_len, whole) per rank, in rank order.
     Returns for every rank the run that ends right before its shard: None for rank 0, else (cls, len)."""
     out = []
-    carry = None  # (cls, len, whole)
+    carry = None
     for cls, length, whole in summaries:
-        out.append(None if carry is None else (carry[0], carry[1]))
-        if carry is not None and whole and cls == carry[0]:
-            carry = (cls, carry[1] + length, carry[2])
-        else:
-            carry = (cls, length, bool(whole) and carry is None)
+        out.append(carry)
+        carry = fold_closing_run(carry, cls, length, whole)
     return out
 
 
@@ -400,7 +406,8 @@ def segment_messages_sharded(ctx, hx, d_mag, global_offset, n_total, noise_thres
     ctx.check(lib.urh_segment_shard_pass(ctx.handle, C.c_void_p(d_mag.ptr), int(d_mag.dtype == np.float64), n_local,
                                          float(noise_threshold), summary))
     every = hx.allgather((int(summary[0]), int(summary[1]), int(summary[2]), int(summary[3])))
-    carries = fold_carry([(c, l, w) for c, l, w, _ in every])
+    runs = [(c, l, w) for c, l, w, _ in every]
+    carries = fold_carry(runs)
     carry = carries[hx.rank]
     count = C.c_int64(0)
     ctx.check(lib.urh_shard_candidates(ctx.handle, int(carry is not None), carry[0] if carry else 0, carry[1] if carry else 0,
@@ -412,13 +419,7 @@ def segment_messages_sharded(ctx, hx, d_mag, global_offset, n_total, noise_thres
     tables = hx.allgather((pos, cls))
     pos_all = np.ascontiguousarray(np.concatenate([t[0] for t in tables]))
     cls_all = np.ascontiguousarray(np.concatenate([t[1] for t in tables]))
-    # the run that ends the capture: fold every shard's closing run
-    last_cls, last_len = None, 0
-    for c, l, w, _ in every:
-        if last_cls is not None and w and c == last_cls:
-            last_len += l
-        else:
-            last_cls, last_len = c, l
+    last_cls, last_len = fold_closing_run(carries[-1], *runs[-1])   # the run that ends the capture
     cap = max(16, len(pos_all) + 2)
     seg = np.empty((cap, 2), dtype=np.int64)
     k = C.c_int64(0)
