@@ -213,6 +213,21 @@ int urh_gather_samples(urh_ctx* ctx, const float* d_x, int64_t n, int64_t start,
  * h_out != NULL: the band is also copied to that (pinned) host buffer, asynchronously; synchronise before reading it. */
 int urh_fta_records(urh_ctx* ctx, const float* d_db, int64_t frames, int window_size, int64_t row0, int64_t nrows,
                     const double* d_freqs, double time_width, int include_amplitude, uint8_t* d_out, void* h_out);
+/* IQArray.export_to_sub (IQArray.py:275-319): the RAW_Data body of the Flipper Zero .sub file of the (n, 2) capture d_iq (any
+ * URH_DT_*), i.e. everything the reference writes after "Protocol: RAW" and before the final newline, from the runs of
+ * convert_to(uint8)[:, 0] (DESIGN §4.12).  d_out holds at least urh_sub_export_bound(n) bytes; *h_bytes receives the body's length
+ * (synchronises the context stream).  n >= 1: the reference fails on an empty capture before it writes anything. */
+int64_t urh_sub_export_bound(int64_t n);
+int urh_sub_export(urh_ctx* ctx, const void* d_iq, int dtype, int64_t n, uint8_t* d_out, int64_t capacity, int64_t* h_bytes);
+/* The same body for a HOST capture h_iq of any size whose uint8 column (n bytes) and chain tables (about n / 4 bytes) fit the device:
+ * the capture goes through the ring (stream_ring.cuh; chunks of whole tiles, urh_filter_windows URH_FILTER_TILES) and only its
+ * column I stays, as uint8; the body is written to the file descriptor fd (write(2), at its current position) in pieces of the
+ * chunk's tiles, each generated on the device while nothing else is queued.  *h_bytes receives the body's length.  ring = 2 .. 8. */
+int urh_sub_export_stream(urh_ctx* ctx, const void* h_iq, int dtype, int64_t n, int fd, int64_t chunk_samples, int ring, int64_t* h_bytes);
+/* Device bytes of urh_sub_export on a capture it must upload (streamed = 0: capture, body and scratch) or of urh_sub_export_stream
+ * (streamed = 1: ring slots, scratch and one body piece), scratch counted by the streamed entries' arena rule; export_to_sub streams
+ * when the resident value exceeds the device budget, as use_stream does. */
+int urh_sub_export_footprint(int64_t n, int dtype, int streamed, int64_t chunk_samples, int ring, int64_t* h_bytes);
 
 /* ---- signal views (path_creator.pyx; view.cu) ---------------------------------------------------------------------------------
  * The source is sample d_src[i * stride], i < n, of dtype URH_DT_*: stride 1 for qad or a 1-D capture, 2 for one column of an

@@ -161,6 +161,10 @@ SIGNATURES = {
     "urh_spectrogram_bgra": (i32, [vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i32, C.c_double, C.c_double, i32, vp]),
     "urh_gather_samples": (i32, [vp, vp, i64, i64, i64, i64, vp]),
     "urh_fta_records": (i32, [vp, vp, i64, i32, i64, i64, vp, C.c_double, i32, vp, vp]),
+    "urh_sub_export_bound": (i64, [i64]),
+    "urh_sub_export": (i32, [vp, vp, i32, i64, vp, i64, C.POINTER(i64)]),
+    "urh_sub_export_stream": (i32, [vp, vp, i32, i64, i32, i64, i32, C.POINTER(i64)]),
+    "urh_sub_export_footprint": (i32, [i64, i32, i32, i64, i32, C.POINTER(i64)]),
     "urh_path_minmax": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, vp]),
     "urh_qpath_streams": (i32, [vp, vp, i32, i64, i64, i64, i64, i64, i64, vp, vp, i32, vp, vp]),
     "urh_modulate_stats": (i32, [vp, vp]),

@@ -13,8 +13,19 @@ import wave
 import numpy as np
 
 from ..cythonext.util import get_magnitudes
+from ..device import DeviceArray
 
 _INT_TYPES = (np.uint8, np.int8, np.uint16, np.int16)
+
+
+def _sub_loop_error(data):
+    """the exception the reference's export_to_sub loop (IQArray.py:281-304) raises for a capture that is not a non-empty (n, 2)
+    array: every sample of a 1-D capture is a numpy.uint8 scalar without len(); after no sample at all, lastvalue was never set"""
+    for value in np.zeros(min(len(data), 1), np.uint8):
+        len(value)
+    if False:
+        lastvalue = None
+    return lastvalue  # noqa: F821
 
 
 class IQArray(object):
@@ -290,3 +301,72 @@ class IQArray(object):
         f.setframerate(sample_rate)
         f.writeframes(self.convert_to(np.int16))
         f.close()
+
+    # bytes of the .sub body copied from the device and written per step of export_to_sub
+    SUB_WRITE_BYTES = 64 << 20
+
+    def export_to_sub(self, filename, frequency=433920000, preset="FuriHalSubGhzPresetOok650Async"):
+        """The Flipper Zero RAW file of IQArray.py:275-319: run lengths of convert_to(uint8)[:, 0], signed by value > 127, 512 per
+        RAW_Data line.  The body is generated on the device (DESIGN §4.12): from the cached capture or one upload of a host capture
+        (urh_sub_export, written in SUB_WRITE_BYTES pieces), or, for a host capture whose resident footprint exceeds the device budget
+        (the rule of use_stream, $URH_B200_DEVICE_BUDGET included), streamed through the ring and written to the file piece by piece
+        (urh_sub_export_stream).  The reference's exceptions for an empty or 1-D capture are raised before the file is created; a
+        failure after it was opened removes it."""
+        from .. import _lib
+        from ..cythonext import signal_functions as sf
+
+        data = self.__data
+        if data.ndim == 2 and len(data):
+            if data.dtype not in [np.dtype(t) for t in _INT_TYPES + (np.float32,)]:
+                raise NotImplementedError("Conversion from {} to {} not supported", data.dtype, np.uint8)
+        else:
+            _sub_loop_error(data)
+        if data.shape[1] != 2:
+            # the reference reads column 0 of rows of any width; the device entries read (n, 2) captures
+            col = np.ascontiguousarray(data[:, 0])
+            return IQArray(np.stack([col, col], axis=1), _owned=True).export_to_sub(filename, frequency, preset)
+        n = len(data)
+        code = _lib.dtype_code(data.dtype)
+        cached = self._device is not None and len(self._device) == n
+        ctx = self._device.ctx if cached else _lib.default_context()
+        stream = False
+        if not cached:
+            fp = ctypes.c_int64(0)
+            ctx.check(ctx.lib.urh_sub_export_footprint(n, code, 0, sf.FILTER_STREAM_CHUNK, sf.STREAM_RING, ctypes.byref(fp)))
+            stream = fp.value > sf.device_budget(ctx)
+        body = None
+        nbytes = ctypes.c_int64(0)
+        if not stream:
+            dev = self.device()
+            cap = int(ctx.lib.urh_sub_export_bound(n))
+            body = DeviceArray(ctx, (cap,), np.uint8)
+        try:
+            if body is not None:
+                ctx.check(ctx.lib.urh_sub_export(ctx.handle, ctypes.c_void_p(dev.ptr), code, n, ctypes.c_void_p(body.ptr), cap,
+                                                 ctypes.byref(nbytes)))
+            try:
+                with open(filename, "w") as subfile:
+                    subfile.write("Filetype: Flipper SubGhz RAW File\n")
+                    subfile.write("Version: 1\n")
+                    subfile.write("Frequency: {}\n".format(frequency))
+                    subfile.write("Preset: {}\n".format(preset))
+                    subfile.write("Protocol: RAW")
+                    subfile.flush()
+                    if body is None:
+                        src = np.ascontiguousarray(data)
+                        ctx.check(ctx.lib.urh_sub_export_stream(ctx.handle, src.ctypes.data_as(ctypes.c_void_p), code, n, subfile.fileno(),
+                                                                sf.FILTER_STREAM_CHUNK, sf.STREAM_RING, ctypes.byref(nbytes)))
+                    else:
+                        piece = np.empty(min(nbytes.value, self.SUB_WRITE_BYTES), np.uint8)
+                        for at in range(0, nbytes.value, len(piece) or 1):
+                            m = min(len(piece), nbytes.value - at)
+                            ctx.check(ctx.lib.urh_memcpy_d2h(ctx.handle, piece.ctypes.data_as(ctypes.c_void_p), ctypes.c_void_p(body.ptr + at), m))
+                            subfile.buffer.write(piece[:m].data)
+                    subfile.buffer.write(b"\n")
+            except BaseException:
+                if os.path.exists(filename):
+                    os.remove(filename)
+                raise
+        finally:
+            if body is not None:
+                body.free()
